@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — images/sec of the denoise + decode hot path (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W [--impl ours|reference] [--workload C4|C2|C3]
+  python bench.py --gpus N --steps K --warmup W [--impl ours|reference] [--workload C4|C2|C3] [--dump-outputs DIR]
   (N > 1: launched by torchrun, one rank per GPU; batch sharded by image, no per-step collective.)
 
 A "step" = one batch of images through the whole hot path (sample_euler over all denoise steps + VAE decode).
@@ -11,10 +11,15 @@ Default workload C4: FLUX.1-schnell, 1024x1024 (latent 128x128), 4 steps, cfg 0,
 Printed JSON (rank 0, one line): metric/value/unit/... per the driver contract, plus
   e2e          same metric through the public API with HOST inputs (pinned text embeddings -> H2D, host numpy noise
                -> H2D, uint8 images -> D2H) every step
-  roofline     the tcgen05 GEMM kernel (dominant: 81% of C4 FLOPs): algorithmic FLOPs / CUDA-event time of every
-               GEMM launch of one instrumented step, vs the measured bf16 peak (MEASURED_PEAKS.json)
+  roofline     the wgmma GEMM kernel (dominant: 81% of C4 FLOPs): algorithmic FLOPs / CUDA-event time of every
+               GEMM launch of one instrumented step, vs the bf16 peak (MEASURED_PEAKS.json when present, else the
+               H100 SXM data-sheet figure)
   cpu_baseline the oracle (CPU restatement of the reference MLX path, "port") timed on the host cores on a bounded
                sample, extrapolated to images/sec (rank 0, N = 1 only)
+
+--dump-outputs DIR writes what the last timed step computed (the final latents and the decoded images in [0, 1], as
+float32 .npy files, at most 64 MB in all) so that two builds can be compared output for output; with the same arguments
+the inputs (synthetic weights, embeddings, noise seeds) are identical from run to run.
 """
 from __future__ import annotations
 
@@ -68,35 +73,19 @@ def workload_config(workload, per_gpu, world):
             "l2": "inputs larger than L2 (the MMDiT weights, 23.8 GB for FLUX, are streamed once per forward)"}
 
 
-def committed_gemm_traffic():
-    """dram__bytes_read + dram__bytes_write of ONE launch of the dominant kernel (gemm2_tc_kernel, default configuration,
-    on the largest C4 shape, 16384 x 12288 x 3072 + GELU) from the committed ncu capture of the kernel as it is timed
-    here; algorithmic bytes of that launch are (16384 + 12288) * 3072 * 2 + 16384 * 12288 * 2 = 579 MB."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_gemm_dram.json")))
-        for r in d["rows"]:
-            if r["config"] == "base" and r["shape_MNK"].startswith("16384 12288 3072"):
-                return float(r["dram_bytes_total"]), ("profiles/r02_ncu_gemm_dram.json: gemm2_tc_kernel (default config) "
-                                                      "16384x12288x3072+GELU, bytes per launch")
-    except Exception:
-        pass
-    return None, None
-
-
 def vae_roofline(decode_ms, images, lat, peaks):
-    """The decode of the last timed step against both roofs (SURVEY.md §8d: 10.472 TFLOP and a 13.46 GB fusion model per
-    1024^2 image, both linear in pixels).  HBM bytes per image are the ncu-measured dram__bytes of one whole decode
-    (profiles/r02_vae_dram_B{1,4}_norm1.txt: 12.44 GB at batch 1, 13.36 GB at batch 4 for 1024^2), not re-measured here."""
+    """The decode of the last timed step against both roofs, from shapes (SURVEY.md §8d: 10.472 TFLOP and a 13.46 GB
+    fusion model of the minimum HBM traffic per 1024^2 image, both linear in pixels) over the CUDA-event decode time.
+    The HBM bytes are the algorithmic model, not a measured count."""
     px = (lat / 128.0) ** 2
     ms_img = decode_ms / max(images, 1)
     tflop = 10.472 * px
-    gb = (12.44 if images == 1 else 13.36) * px
+    gb = 13.46 * px
     return {"ms_per_image": ms_img, "tflop_per_image": tflop, "tensor_tflops": tflop / (ms_img * 1e-3),
             "tensor_frac": tflop / (ms_img * 1e-3) / peaks["bf16_tflops"],
-            "dram_gb_per_image": gb, "dram_gb_model": 13.46 * px, "dram_over_model": gb / (13.46 * px),
-            "dram_gbs": gb / (ms_img * 1e-3), "hbm_frac": gb / (ms_img * 1e-3) / peaks["hbm_gbs"],
-            "dram_source": "profiles/r02_vae_dram_B{1,4}_norm1.txt (ncu dram__bytes_read+write of one decode)",
-            "bound": "tensor (3x3 convs at ~780 FLOP/B); the HBM-bound kernels are listed in DESIGN.md §5"}
+            "dram_gb_model": gb, "model_gbs": gb / (ms_img * 1e-3), "hbm_frac": gb / (ms_img * 1e-3) / peaks["hbm_gbs"],
+            "dram_source": "algorithmic fusion model (SURVEY.md §8d), not measured",
+            "bound": "tensor (3x3 convs at ~780 FLOP/B)"}
 
 
 def load_peaks():
@@ -105,11 +94,12 @@ def load_peaks():
         d = json.load(open(p))
         return {"bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d["bf16_tflops_sustained"],
                 "hbm_gbs": d["hbm_gbs"], "source": "measured"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (dense bf16, HBM3), not measured; no sustained figure is known without a measurement
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": None, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -238,6 +228,26 @@ def cpu_baseline(workload: str, repeats: int = 2, budget_s: float = 40.0):
 
 
 # ------------------------------------------------------------------------------------------------ our arm
+DUMP_BUDGET_BYTES = 64_000_000 - 4096     # 64 MB in all, .npy headers (128 bytes each) included
+
+
+def dump_outputs(out_dir, outputs):
+    """outputs of the last timed step -> out_dir/<name>.npy (float32).  An array that does not fit the remaining budget
+    is replaced by a fixed, seeded sample of its elements (<name>.npy) and their flat indices (<name>_index.npy)."""
+    os.makedirs(out_dir, exist_ok=True)
+    left = DUMP_BUDGET_BYTES
+    for name, t in outputs.items():
+        a = t.detach().float().cpu().numpy().astype(np.float32)
+        if a.nbytes > left:
+            n = max(1, left // 12)                     # 4 bytes of value + 8 bytes of index per sampled element
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=min(n, a.size), replace=False))
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+            left -= idx.size * 8
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        left -= a.nbytes
+
+
 def run_ours(args):
     import diffusionkit_b200 as dk
     from diffusionkit_b200 import dist as dkd, ops
@@ -294,6 +304,7 @@ def run_ours(args):
         out = pipe._decode(lat16, want_u8=True)
         ev[2].record()
         split["ev"] = ev
+        split["outputs"] = {"latents": latent, "images": out[0]}     # out = (float images in [0, 1], uint8 images)
         return out
 
     def step_e2e():
@@ -324,6 +335,8 @@ def run_ours(args):
     barrier()
     launches = ops.launch_count() - launches0
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, split["outputs"])
     split["denoise"] = split["ev"][0].elapsed_time(split["ev"][1])
     split["decode"] = split["ev"][1].elapsed_time(split["ev"][2])
     t_mine = e0.elapsed_time(e1) / 1e3
@@ -380,7 +393,8 @@ def run_ours(args):
     value = n_images / t_dev
     n_img_tok, hp = (lat // 2) ** 2, lat // 2
     flops_img = mmdit_flops_per_forward(cfg, n_img_tok, T) * steps * reps
-    mmdit_frac = (flops_img * per_gpu * args.steps / t_dev) / (peaks["bf16_tflops_sustained"] * 1e12)
+    mmdit_frac = ((flops_img * per_gpu * args.steps / t_dev) / (peaks["bf16_tflops_sustained"] * 1e12)
+                  if peaks["bf16_tflops_sustained"] else None)
     achieved = gemm_stats["flops"] / t_gemm / 1e12 if t_gemm > 0 else 0.0
     h2d = cond_host.numel() * cond_host.element_size() + pooled_host.numel() * pooled_host.element_size() + \
         noise_dev.numel() * 4
@@ -399,11 +413,11 @@ def run_ours(args):
         "gpu_launches": int(launches),
         "clocks": clk,
         "roofline": {"bound": "tensor",
-                     "kernel": "gemm2_tc_kernel / gemm_tc_kernel (tcgen05 GEMMs: every nn.Linear of the MMDiT)",
+                     "kernel": "gemm_wgmma_kernel (every nn.Linear of the MMDiT)",
                      "achieved": achieved, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-                     "frac": achieved / peaks["bf16_tflops"], "traffic": committed_gemm_traffic()[0],
-                     "traffic_source": committed_gemm_traffic()[1],
-                     "peak_source": f"{peaks['source']} bf16 burst (sustained {peaks['bf16_tflops_sustained']})",
+                     "frac": achieved / peaks["bf16_tflops"],
+                     "peak_source": (f"{peaks['source']} bf16 burst (sustained {peaks['bf16_tflops_sustained']})"
+                                     if peaks["bf16_tflops_sustained"] else f"{peaks['source']} bf16 dense peak"),
                      "launches_timed": n_gemm, "gemm_seconds_of_one_step": t_gemm},
         "mmdit_tensor_frac_sustained": mmdit_frac,
         "last_step_ms": {"denoise": split["denoise"], "decode": split["decode"]},
@@ -413,10 +427,7 @@ def run_ours(args):
         # the one-time weight replication, split: lazy NCCL communicator creation / rank-0 init / the broadcast itself
         "weights_timing": {k: (round(v, 4) if isinstance(v, float) else v) for k, v in wt.items()},
     }
-    try:
-        line["vae_roofline"] = vae_roofline(split["decode"], per_gpu, lat, peaks)
-    except Exception:  # informational only
-        pass
+    line["vae_roofline"] = vae_roofline(split["decode"], per_gpu, lat, peaks)
     if world == 1 and not args.no_cpu_baseline:
         try:
             line["cpu_baseline"] = cpu_baseline(args.workload)
@@ -466,6 +477,8 @@ def main():
     ap.add_argument("--workload", default="C4", choices=sorted(WORKLOADS))
     ap.add_argument("--images-per-gpu", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs to DIR/<name>.npy (float32, at most 64 MB)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-"""diffusionkit_b200 — B200-native denoise + decode engine behind DiffusionKit's `diffusionkit.mlx`
+"""diffusionkit_b200 — H100-native denoise + decode engine behind DiffusionKit's `diffusionkit.mlx`
 DiffusionPipeline / FluxPipeline API (reference: argmaxinc/DiffusionKit, python/src/diffusionkit/mlx/__init__.py).
 
     from diffusionkit_b200 import FluxPipeline

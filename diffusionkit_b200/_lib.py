@@ -53,7 +53,6 @@ SIGNATURES = {
     "dk_ln_modulate": (i32, [vp, i32, vp, vp, vp, vp, i64, i32, i32, i32, f32, vp]),
     "dk_qk_norm_rope": (i32, [vp, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, f32, vp]),
     "dk_attention_fwd": (i32, [vp, i32, vp, i32, i32, i32, i32, f32, i32, vp, i64, vp, i64, vp]),
-    "dk_attention_tuning": (i32, [i32, i32, i32]),
     "dk_silu_add": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, vp]),
     "dk_act": (i32, [vp, i32, vp, vp, i64, i32, vp]),
     "dk_patchify": (i32, [vp, i32, vp, vp, i32, i32, i32, i32, i32, vp]),
@@ -147,7 +146,7 @@ class Context:
     def __init__(self, device: int = 0):
         self.lib = load()
         if not torch.cuda.is_available():
-            raise DkError("no CUDA device: diffusionkit_b200 runs on B200 (sm_100a) only; there is no CPU fallback")
+            raise DkError("no CUDA device: diffusionkit_b200 runs on H100 (sm_90a) only; there is no CPU fallback")
         h = vp()
         rc = self.lib.dk_ctx_create(device, C.byref(h))
         if rc != 0:

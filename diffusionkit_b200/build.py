@@ -1,4 +1,4 @@
-"""In-tree build of libdkb200.so (nvcc, sm_100a only).  `python -m diffusionkit_b200.build`."""
+"""In-tree build of libdkb200.so (nvcc, sm_90a only).  `python -m diffusionkit_b200.build`."""
 import os
 import subprocess
 import sys
@@ -6,9 +6,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdkb200.so")
-SOURCES = ["api.cu", "gemm.cu", "gemm2.cu", "conv_fused.cu", "attention.cu", "attention_v5.cu", "attention_v6.cu", "elementwise.cu", "text.cu"]
+SOURCES = ["api.cu", "gemm.cu", "conv_fused.cu", "attention.cu", "elementwise.cu", "text.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall",
     "--expt-relaxed-constexpr",

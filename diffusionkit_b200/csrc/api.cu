@@ -13,7 +13,7 @@ void dk_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* dk_last_error(void) { return g_err; }
-extern "C" const char* dk_version(void) { return "dkb200 0.1.0 (sm_100a)"; }
+extern "C" const char* dk_version(void) { return "dkb200 0.1.0 (sm_90a)"; }
 
 extern "C" int dk_ctx_create(int device, dk_ctx** out) {
   DK_REQUIRE(out != nullptr, "dk_ctx_create: null out");
@@ -30,7 +30,7 @@ extern "C" int dk_ctx_create(int device, dk_ctx** out) {
   DK_CHECK_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   DK_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-  DK_REQUIRE(prop.major == 10, "dk_ctx_create: device %d is sm_%d%d; this library is built for sm_100a only", device,
+  DK_REQUIRE(prop.major == 9 && prop.minor == 0, "dk_ctx_create: device %d is sm_%d%d; this library is built for sm_90a only", device,
              prop.major, prop.minor);
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;

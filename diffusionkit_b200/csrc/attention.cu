@@ -1,573 +1,223 @@
-// K3 — attention forward softmax(scale * Q K^T) V for sm_100a: tcgen05 MMAs with S and O accumulators in TMEM,
-// TMA-fed 128B-swizzled Q/K/V tiles, online softmax on S read back with tcgen05.ld.
+// K3 — attention forward softmax(scale * Q K^T) V for sm_90a: wgmma with S and O accumulators in registers,
+// TMA-fed 128B-swizzled Q/K/V tiles, online softmax in registers, P fed back to the PV wgmma as a register operand.
 // Replaces mx.fast.scaled_dot_product_attention (reference mlx/mmdit.py:562-563,643,687-688,736): no mask,
 // non-causal, joint [text|image] sequence, head dim 64 (SD3) or 128 (FLUX).
 //
-// This file: the current kernel (v3: two 128-row Q tiles per CTA, two softmax warpgroups per tile, P kept in TMEM) and
-// the C entry point.  (The earlier generations — P through shared memory, one softmax warpgroup per tile — and the
-// variants measured and rejected in round 2 are in the git history; DESIGN.md lists what each taught.)
+// One CTA per (128-row Q tile, head, batch), 384 threads:
+//   warpgroup 0 (warp 0): TMA producer — Q once, then K and V tiles of 128 keys through a two-deep ring (K and V on
+//                         separate barriers, so S = Q K^T starts before V has landed)
+//   warpgroups 1, 2     : 64 query rows each — S = Q K^T (m64n128, A and B from shared memory), masked online softmax
+//                         on the S fragment (a row is spread over the four lanes of a quad), O = O * alpha + P V
+//                         (m64nD, P from registers: the S accumulator layout of 16 key columns IS the A fragment
+//                         layout of one k16 step), O / l -> global.
 #include "attention.cuh"
 
 namespace dk {
 
-// ================================================================================================
-// v3: as v2 (two 128-row Q tiles per CTA, P kept in TMEM) but TWO softmax warpgroups per Q tile: warpgroup (w, hh)
-// owns the 64-key half hh of every row of tile w (both halves can reach the same TMEM lanes because lane access is
-// by warp %% 4).  Same-box measurements of v2: 1058 TFLOP/s with the softmax vs 1485 with the softmax work removed —
-// the single warp per scheduler could not hide the TMEM / MUFU latencies; v3 doubles the warps per scheduler and halves
-// the per-thread row.  The two halves of a row exchange their partial row max through shared memory (one named
-// barrier per tile) so that both use the same running max; partial row sums are combined once at the end.
-// ================================================================================================
-// 18 warps: 0-15 softmax (g = warp >> 2, TMEM lane quarter = warp & 3), 16 TMA producer, 17 MMA issuer.
-// 576 threads -> 112 registers per thread at launch, enough for every role without setmaxnreg (a 640-thread layout
-// with setmaxnreg dead-locked: register redistribution is bounded by the CTA's launch allocation).
-constexpr int ATT3_THREADS = 576;
+constexpr int ATT_THREADS = 384;
 
-// POLY4: of every four exponentials, how many run on the FMA pipe (ex2_poly) instead of MUFU.EX2 (0, 1 or 2)
-// VAR bits: 4 = split P publication (see launch_attention_v3); 32 = streamed exponential pass: the 64 scores of a
-// thread go through two 16-column register buffers, the next TMEM read in flight behind the current chunk and the TMEM
-// stores waited for only at the two publications, instead of two load -> wait -> compute -> store -> wait rounds;
-// 16 = diagnostic instantiation that records SM-clock timestamps of every hand-over (DK_ATT_TRACE).
-template <typename T, int D, int POLY4, int VAR>
-__device__ __forceinline__ void attention_v3_body(const CUtensorMap& tmQKV, const AttParams& p) {
+template <typename T, int D>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attention_fwd_kernel(const __grid_constant__ CUtensorMap tm, const AttParams p) {
   using H16 = Half16<T>;
-  using Cfg = Att2Cfg<D>;
+  using Cfg = AttCfg<D>;
   constexpr int KS = Cfg::KS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem + Cfg::OFF_Q;
   uint8_t* sK = smem + Cfg::OFF_K;
   uint8_t* sV = smem + Cfg::OFF_V;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
-  uint64_t* q_full = bars + 0;
-  uint64_t* k_full = bars + 1;             // [KS]
-  uint64_t* k_empty = k_full + KS;         // [KS]
-  uint64_t* v_full = k_empty + KS;         // [KS]
-  uint64_t* v_empty = v_full + KS;         // [KS]
-  uint64_t* s_full = v_empty + KS;         // [2]  QK_w(j) retired
-  uint64_t* p_full = s_full + 2;           // [2]  softmax_w(j) published P_w(j) (128 arrivals)
-  uint64_t* o_full = p_full + 2;           // [2]  PV_w(n-1) retired
-  uint64_t* p_half = o_full + 2;           // [2]  VAR 4: first 32 keys of every thread's P published (256 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(p_half + 2);
-  float* xch = reinterpret_cast<float*>(smem + Cfg::OFF_BAR + 256);   // [tile 2][half 2][row 128] partial max / sum
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
+  uint64_t* k_full = q_full + 1;
+  uint64_t* v_full = k_full + KS;
+  uint64_t* kv_empty = v_full + KS;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (2 * ATT_BQ);
+  const int wg = threadIdx.x >> 7;
+  const int q0 = blockIdx.x * ATT_BQ;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
   const int h = p.heads * D;
-  const int n_tiles = (p.S + ATT_BKV - 1) / ATT_BKV;
-  const int row_base = b * p.S;
+  const int row0 = b * p.S;               // first row of this batch in the packed [B*S, 3h] tensor
+  const int nkv = (p.S + ATT_BKV - 1) / ATT_BKV;
+  constexpr uint32_t TILE_BYTES = ATT_BKV * D * 2;
 
-  if (warp == 16 && lane == 0) {
-    tma_prefetch_desc(&tmQKV);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm);
     mbar_init(q_full, 1);
     for (int i = 0; i < KS; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], 256);
-      mbar_init(&o_full[i], 1);
-      mbar_init(&p_half[i], 256);
+      mbar_init(&kv_empty[i], 8);   // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 17) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // VAR bit 16 (diagnostic instantiation only): SM-clock timestamps of one CTA's hand-overs, step by step
-  //   trace[step][slot]: slots 0-19 softmax group g = 2*w + hh (5 each: S ready, max pass done, partner max read,
-  //   first half of P published, P published), 20-27 MMA issuer (4 per tile: first-half P seen, PV part 0 issued,
-  //   P seen, PV part 1 + next QK^T issued), 28 = K/V stage loaded (producer)
-  constexpr int TRACE_STEPS = 34, TRACE_SLOTS = 32;
-  const bool trace_cta = (VAR & 16) && p.trace != nullptr && blockIdx.x == 3 && blockIdx.y == 1 && blockIdx.z == 0;
-  auto stamp = [&](int step, int slot) {
-    if constexpr ((VAR & 16) != 0) {
-      if (trace_cta && step < TRACE_STEPS) p.trace[step * TRACE_SLOTS + slot] = clock64();
-    }
-  };
 
-  if (warp >= 16) {
-    if (warp == 16) {
-      // ------------------------------------------------------------------ TMA producer (converged warp, elected issue)
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer, converged warp
+    if (warp != 0) return;
+    if (elect_one_sync()) {
+      mbar_arrive_expect_tx(q_full, ATT_BQ * D * 2);
+#pragma unroll
+      for (int c = 0; c < D / 64; ++c) tma_load_2d(sQ + c * (ATT_BQ * 128), &tm, q_full, head * D + c * 64, row0 + q0);
+    }
+    __syncwarp();
+    uint32_t stage = 0, phase = 0;
+    for (int j = 0; j < nkv; ++j) {
+      mbar_wait_warp(&kv_empty[stage], phase ^ 1);
       if (elect_one_sync()) {
-        mbar_arrive_expect_tx(q_full, 2 * Cfg::TILE_BYTES);
+        const int kr = row0 + j * ATT_BKV;
+        mbar_arrive_expect_tx(&k_full[stage], TILE_BYTES);
 #pragma unroll
-        for (int w = 0; w < 2; ++w)
+        for (int c = 0; c < D / 64; ++c)
+          tma_load_2d(sK + stage * TILE_BYTES + c * (ATT_BKV * 128), &tm, &k_full[stage], h + head * D + c * 64, kr);
+        mbar_arrive_expect_tx(&v_full[stage], TILE_BYTES);
 #pragma unroll
-          for (int a = 0; a < D / 64; ++a)
-            tma_load_2d(sQ + w * Cfg::TILE_BYTES + a * 16384, &tmQKV, q_full, head * D + a * 64,
-                        row_base + q0 + w * ATT_BQ);
+        for (int c = 0; c < D / 64; ++c)
+          tma_load_2d(sV + stage * TILE_BYTES + c * (ATT_BKV * 128), &tm, &v_full[stage], 2 * h + head * D + c * 64, kr);
       }
       __syncwarp();
-      int st = 0;
-      uint32_t par = 0;
-      for (int j = 0; j < n_tiles; ++j) {
-        const int kv_row = row_base + j * ATT_BKV;
-        mbar_wait(&k_empty[st], par ^ 1);
-        if (elect_one_sync()) {
-          mbar_arrive_expect_tx(&k_full[st], Cfg::TILE_BYTES);
-#pragma unroll
-          for (int a = 0; a < D / 64; ++a)
-            tma_load_2d(sK + st * Cfg::TILE_BYTES + a * 16384, &tmQKV, &k_full[st], h + head * D + a * 64, kv_row);
-        }
-        __syncwarp();
-        mbar_wait(&v_empty[st], par ^ 1);
-        if (elect_one_sync()) {
-          mbar_arrive_expect_tx(&v_full[st], Cfg::TILE_BYTES);
-#pragma unroll
-          for (int a = 0; a < D / 64; ++a)
-            tma_load_2d(sV + st * Cfg::TILE_BYTES + a * 16384, &tmQKV, &v_full[st], 2 * h + head * D + a * 64, kv_row);
-        }
-        __syncwarp();
-        if (++st == KS) {
-          st = 0;
-          par ^= 1;
-        }
-      }
-    } else if (warp == 17) {
-      // ------------------------------------------------------------------ MMA issuer (converged warp, elected issue)
-      constexpr uint32_t idesc_qk = make_idesc_f16(ATT_BQ, ATT_BKV, H16::is_bf16, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_f16(ATT_BQ, D, H16::is_bf16, false, true);
-      const uint32_t desc_hi = smem_desc_hi_sw128(1024);
-      const uint32_t q_lo0 = smem_desc_lo(smem_u32(sQ), 0);
-      const uint32_t k_lo0 = smem_desc_lo(smem_u32(sK), 0);
-      const uint32_t v_lo0 = smem_desc_lo(smem_u32(sV), 16384);   // MN-major: LBO = stride between 64-wide d atoms
-      constexpr uint32_t TILE16 = Cfg::TILE_BYTES >> 4;
-      // S_w = Q_w K^T : K = d in 16-wide slices (slice k lives in 64-column atom k>>2 at +32 B * (k&3))
-      auto issue_qk = [&](int w, int st) {
-        const uint32_t q_lo = q_lo0 + w * TILE16;
-        const uint32_t k_lo = k_lo0 + st * TILE16;
-        const uint32_t d_tmem = tmem_base + Cfg::TMEM_S + w * 128;
-#pragma unroll
-        for (int k = 0; k < D / 16; ++k) {
-          const uint32_t off = ((k >> 2) * 16384 + (k & 3) * 32) >> 4;
-          umma_ss(d_tmem, smem_desc_join(q_lo + off, desc_hi), smem_desc_join(k_lo + off, desc_hi), idesc_qk,
-                  k != 0 ? 1u : 0u);
-        }
-        umma_commit(&s_full[w]);
-      };
-      // O_w += P_w V : A = P_w from TMEM (16 keys = 8 columns per slice), B = V slice of 16 key rows (2048 B apart)
-      auto issue_pv = [&](int w, int st, bool first) {
-        const uint32_t v_lo = v_lo0 + st * TILE16;
-        const uint32_t p_tmem = tmem_base + Cfg::TMEM_S + w * 128;
-        const uint32_t d_tmem = tmem_base + Cfg::TMEM_O + w * 128;
-#pragma unroll
-        for (int k = 0; k < ATT_BKV / 16; ++k)   // keys 0-63 -> P columns [0,32), keys 64-127 -> P columns [64,96)
-          umma_ts(d_tmem, p_tmem + (k >> 2) * 64 + (k & 3) * 8, smem_desc_join(v_lo + k * (2048 >> 4), desc_hi),
-                  idesc_pv, (!first || k != 0) ? 1u : 0u);
-      };
-      // VAR 4: the PV MMAs of the key slices whose P is published first (keys 0-31 and 64-95: the first 32 keys of both
-      // threads of every row) are issued while the exponentials of the other 32 keys are still running
-      auto issue_pv_part = [&](int w, int st, bool first, int part) {
-        const uint32_t v_lo = v_lo0 + st * TILE16;
-        const uint32_t p_tmem = tmem_base + Cfg::TMEM_S + w * 128;
-        const uint32_t d_tmem = tmem_base + Cfg::TMEM_O + w * 128;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const int k = (kk >> 1) * 4 + part * 2 + (kk & 1);   // part 0: 0, 1, 4, 5   part 1: 2, 3, 6, 7
-          umma_ts(d_tmem, p_tmem + (k >> 2) * 64 + (k & 3) * 8, smem_desc_join(v_lo + k * (2048 >> 4), desc_hi),
-                  idesc_pv, (!first || part != 0 || kk != 0) ? 1u : 0u);
-        }
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      if (elect_one_sync()) {
-        issue_qk(0, 0);
-        issue_qk(1, 0);
-        umma_commit(&k_empty[0]);
-      }
-      __syncwarp();
-      int st = 0;
-      uint32_t par = 0;
-      if constexpr ((VAR & 4) != 0) {
-        for (int j = 0; j < n_tiles; ++j) {
-          const int st_n = (st + 1 == KS) ? 0 : st + 1;
-          const uint32_t par_n = (st + 1 == KS) ? (par ^ 1) : par;
-          const bool more = j + 1 < n_tiles;
-          mbar_wait(&v_full[st], par);
-#pragma unroll
-          for (int w = 0; w < 2; ++w) {
-            mbar_wait(&p_half[w], j & 1);
-            tc_fence_after();
-            if (lane == 0) stamp(j, 20 + 4 * w);
-            if (elect_one_sync()) issue_pv_part(w, st, j == 0, 0);
-            __syncwarp();
-            if (lane == 0) stamp(j, 21 + 4 * w);
-            mbar_wait(&p_full[w], j & 1);
-            if (more && w == 0) mbar_wait(&k_full[st_n], par_n);
-            tc_fence_after();
-            if (lane == 0) stamp(j, 22 + 4 * w);
-            if (elect_one_sync()) {
-              issue_pv_part(w, st, j == 0, 1);
-              if (w == 1) umma_commit(&v_empty[st]);
-              if (!more) umma_commit(&o_full[w]);
-              if (more) {
-                issue_qk(w, st_n);
-                if (w == 1) umma_commit(&k_empty[st_n]);
-              }
-            }
-            __syncwarp();
-            if (lane == 0) stamp(j, 23 + 4 * w);
-          }
-          st = st_n;
-          par = par_n;
-        }
-      } else
-      for (int j = 0; j < n_tiles; ++j) {
-        const int st_n = (st + 1 == KS) ? 0 : st + 1;
-        const uint32_t par_n = (st + 1 == KS) ? (par ^ 1) : par;
-        const bool more = j + 1 < n_tiles;
-        mbar_wait(&v_full[st], par);
-        if (p.debug < 4) mbar_wait(&p_full[0], j & 1);   // debug 4: tensor-side throughput without the softmax round trip
-        if (more) mbar_wait(&k_full[st_n], par_n);
-        tc_fence_after();
-        if (elect_one_sync()) {
-          if (p.debug != 5) issue_pv(0, st, j == 0);
-          if (!more) umma_commit(&o_full[0]);
-          if (more && p.debug != 6) issue_qk(0, st_n);
-          if (more && p.debug == 6) umma_commit(&s_full[0]);
-        }
-        __syncwarp();
-        if (p.debug < 4) mbar_wait(&p_full[1], j & 1);
-        tc_fence_after();
-        if (elect_one_sync()) {
-          if (p.debug != 5) issue_pv(1, st, j == 0);
-          umma_commit(&v_empty[st]);
-          if (!more) umma_commit(&o_full[1]);
-          if (more) {
-            if (p.debug != 6) issue_qk(1, st_n);
-            if (p.debug == 6) umma_commit(&s_full[1]);
-            umma_commit(&k_empty[st_n]);
-          }
-        }
-        __syncwarp();
-        st = st_n;
-        par = par_n;
+      if (++stage == KS) {
+        stage = 0;
+        phase ^= 1;
       }
     }
-  } else {
-    // -------------------------------------------------------------------- softmax warpgroups: g = 2*w + hh
-    const int g = warp >> 2;
-    const int w = g >> 1;       // Q tile
-    const int hh = g & 1;       // key half of every 128-key tile
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    const uint32_t t_s = t_lane + Cfg::TMEM_S + w * 128 + hh * 64;      // this thread's 64 scores
-    constexpr int OC = D / 2;                                           // O columns owned by this half
-    const uint32_t t_o = t_lane + Cfg::TMEM_O + w * 128 + hh * OC;
-    float* my_x = xch + (w * 2 + hh) * 128 + r;
-    const float* peer_x = xch + (w * 2 + (hh ^ 1)) * 128 + r;
-    float m_run = -INFINITY;
-    float l_run = 0.f;
-    const float sl2 = p.scale_log2;
-    // publication of this thread's P columns: TMEM stores complete -> ordered before the arrive -> arrive
-    auto publish = [&](uint64_t* bar) {
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(bar);
-    };
+    return;
+  }
 
-    for (int j = 0; j < n_tiles; ++j) {
-      mbar_wait(&s_full[w], j & 1);
-      tc_fence_after();
-      const bool tr = quarter == 0 && lane == 0;
-      if (tr) stamp(j, 5 * g + 0);
-      const int kv_valid = p.S - j * ATT_BKV - hh * 64;   // valid keys in this half (tail tile only matters)
-      // pass 1: partial row max over this half's 64 scores
-      float mx_half;
-      uint32_t sr[2][32];
-      {
-        tmem_ld_32x32(t_s, sr[0]);
-        tmem_ld_32x32(t_s + 32, sr[1]);
-        tmem_ld_wait();
-        if (kv_valid < 64) {
+  // -------------------------------------------------------------------- consumers: query rows q0 + 64*cw ..
+  const int cw = wg - 1;
+  const float sl2 = p.scale_log2;
+  float o[D / 2];
 #pragma unroll
-          for (int c = 0; c < 2; ++c)
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY};   // running max (log2 domain) of rows lane/4 and lane/4 + 8
+  float l_run[2] = {0.f, 0.f};               // this thread's share of the running row sums
+  const int col0 = 2 * (lane & 3);
+
+  mbar_wait(q_full, 0);
+  const uint32_t q_base = smem_u32(sQ) + cw * 64 * 128;
+  uint32_t stage = 0, phase = 0;
+  for (int j = 0; j < nkv; ++j) {
+    const int kv_valid = p.S - j * ATT_BKV;
+    const uint32_t k_base = smem_u32(sK + stage * TILE_BYTES);
+    const uint32_t v_base = smem_u32(sV + stage * TILE_BYTES);
+    float s[ATT_BKV / 2];
+    mbar_wait(&k_full[stage], phase);
+    wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (c * 32 + i >= kv_valid) sr[c][i] = 0xff800000u;  // -inf
+    for (int kk = 0; kk < D / 16; ++kk) {
+      const uint32_t koff = (kk >> 2) * (ATT_BKV * 128) + (kk & 3) * 32;
+      Wgmma<ATT_BKV, H16::is_bf16, 0>::ss(s, make_smem_desc_sw128(q_base + (kk >> 2) * (ATT_BQ * 128) + (kk & 3) * 32, 16, 1024),
+                                         make_smem_desc_sw128(k_base + koff, 16, 1024), kk != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+
+    // masked online softmax; s[4*jj + 2*i + e] is row lane/4 + 8i, key 8*jj + col0 + e
+    float alpha[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < ATT_BKV / 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = s[4 * jj + 2 * i + e];
+          if (kv_valid < ATT_BKV && 8 * jj + col0 + e >= kv_valid) v = -INFINITY;   // only the last tile is ragged
+          mx = fmaxf(mx, v);
         }
-        {
-          float mx0 = -INFINITY, mx1 = -INFINITY;
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[i], mx * sl2);
+      alpha[i] = ex2_approx(m_run[i] - m_new);
+      m_run[i] = m_new;
+      float ls = 0.f;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            mx0 = fmaxf(mx0, __uint_as_float(sr[0][i]));
-            mx1 = fmaxf(mx1, __uint_as_float(sr[1][i]));
-          }
-          mx_half = fmaxf(mx0, mx1);
+      for (int jj = 0; jj < ATT_BKV / 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = s[4 * jj + 2 * i + e];
+          v = ex2_approx(fmaf(v, sl2, -m_new));
+          ls += v;
         }
+      l_run[i] = l_run[i] * alpha[i] + ls;
+    }
+#pragma unroll
+    for (int jj = 0; jj < D / 8; ++jj)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        o[4 * jj + 2 * i] *= alpha[i];
+        o[4 * jj + 2 * i + 1] *= alpha[i];
       }
-      if (tr) stamp(j, 5 * g + 1);
-      *my_x = mx_half;
-      named_bar_sync(1 + w, 256);   // both halves of tile w: partial maxima visible
-      const float mx = fmaxf(mx_half, *peer_x) * sl2;
-      if (tr) stamp(j, 5 * g + 2);
-      const float m_new = fmaxf(m_run, mx);
-      const bool need = (m_new - m_run) > 8.0f;   // identical in both halves (same inputs)
-      if (__any_sync(0xffffffffu, need)) {
-        const float alpha = ex2_approx(m_run - m_new);
-        m_run = m_new;
-        l_run *= alpha;
-        if (j > 0) {
+    uint32_t pa[ATT_BKV / 16][4];
 #pragma unroll
-          for (int c = 0; c < OC / 32; ++c) {
-            uint32_t o[32];
-            tmem_ld_32x32(t_o + c * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x32(t_o + c * 32, o);
-          }
-        }
-      }
-      // pass 2: P = exp2(s * sl2 - m_run) written over this half's OWN score columns (16 packed columns per 32 keys), so
-      // no thread ever overwrites scores another thread still has to read
-      // (the tail mask lives in a branch of its own: as a per-element select inside the main loop it was 26 % of all
-      //  instructions the kernel issued — ncu, ISETP + FSEL — on every step of every tile)
-      float ls0 = 0.f, ls1 = 0.f;
-      if ((VAR & 32) && kv_valid >= 64) {
-        uint32_t sa[16], sb[16], pk[8];
-        // 16 scores -> 8 packed P columns (same element order, poly pattern and summation order as the plain form)
-        auto chunk = [&](const uint32_t (&sc)[16]) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float x0 = fmaf(__uint_as_float(sc[2 * i]), sl2, -m_run);
-            const float x1 = fmaf(__uint_as_float(sc[2 * i + 1]), sl2, -m_run);
-            const float e0 = ex2_approx(x0);
-            const float e1 = (POLY4 == 2 || (POLY4 == 1 && (i & 1))) ? ex2_poly(x1) : ex2_approx(x1);
-            ls0 += e0;
-            ls1 += e1;
-            pk[i] = H16::pack(e0, e1);
-          }
-        };
-        tmem_ld_32x16(t_s, sa);
-        tmem_ld_wait();
-        tmem_ld_32x16(t_s + 16, sb);
-        chunk(sa);
-        tmem_st_32x8(t_s, pk);          // P columns [0, 8) lie inside score chunk 0, already in registers
-        tmem_ld_wait();
-        tmem_ld_32x16(t_s + 32, sa);
-        chunk(sb);
-        tmem_st_32x8(t_s + 8, pk);
-        tmem_ld_wait();
-        tmem_ld_32x16(t_s + 48, sb);
-        chunk(sa);
-        if (VAR & 4) {
-          publish(&p_half[w]);          // the stores of chunks 0 and 1 were issued a whole chunk ago
-          if (tr) stamp(j, 5 * g + 3);
-        }
-        tmem_st_32x8(t_s + 16, pk);     // columns [16, 24): score chunk 1, consumed
-        tmem_ld_wait();
-        chunk(sb);
-        tmem_st_32x8(t_s + 24, pk);
-      } else if (kv_valid >= 64) {
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t sc[32];
-          tmem_ld_32x32(t_s + c * 32, sc);
-          tmem_ld_wait();
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float x0 = fmaf(__uint_as_float(sc[2 * i]), sl2, -m_run);
-            const float x1 = fmaf(__uint_as_float(sc[2 * i + 1]), sl2, -m_run);
-            const float e0 = ex2_approx(x0);
-            const float e1 = (POLY4 == 2 || (POLY4 == 1 && (i & 1))) ? ex2_poly(x1) : ex2_approx(x1);
-            ls0 += e0;
-            ls1 += e1;
-            pk[i] = H16::pack(e0, e1);
-          }
-          tmem_st_32x16(t_s + c * 16, pk);
-          if ((VAR & 4) && c == 0) {
-            publish(&p_half[w]);
-            if (tr) stamp(j, 5 * g + 3);
-          }
-        }
-      } else {
-#pragma unroll 1
-        for (int c = 0; c < 2; ++c) {
-          uint32_t sc[32];
-          tmem_ld_32x32(t_s + c * 32, sc);
-          tmem_ld_wait();
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float a0 = __uint_as_float(sc[2 * i]), a1 = __uint_as_float(sc[2 * i + 1]);
-            if (c * 32 + 2 * i >= kv_valid) a0 = -INFINITY;
-            if (c * 32 + 2 * i + 1 >= kv_valid) a1 = -INFINITY;
-            const float e0 = ex2_approx(fmaf(a0, sl2, -m_run));
-            const float e1 = ex2_approx(fmaf(a1, sl2, -m_run));
-            ls0 += e0;
-            ls1 += e1;
-            pk[i] = H16::pack(e0, e1);
-          }
-          tmem_st_32x16(t_s + c * 16, pk);
-          if ((VAR & 4) && c == 0) publish(&p_half[w]);
-        }
-      }
-      l_run += ls0 + ls1;
-      publish(&p_full[w]);
-      if (tr) stamp(j, 5 * g + 4);
+    for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
+      pa[kk][0] = H16::pack(s[8 * kk + 0], s[8 * kk + 1]);
+      pa[kk][1] = H16::pack(s[8 * kk + 2], s[8 * kk + 3]);
+      pa[kk][2] = H16::pack(s[8 * kk + 4], s[8 * kk + 5]);
+      pa[kk][3] = H16::pack(s[8 * kk + 6], s[8 * kk + 7]);
     }
 
-    // epilogue: combine the two partial row sums, O_w / l -> global (each half writes its D/2 columns)
-    mbar_wait(&o_full[w], 0);
-    tc_fence_after();
-    *my_x = l_run;
-    named_bar_sync(1 + w, 256);
-    const float inv_l = 1.0f / (l_run + *peer_x);
-    const int s_idx = q0 + w * ATT_BQ + r;
-    const bool row_ok = s_idx < p.S;
-    T* dst = nullptr;
-    if (row_ok) {
-      if (s_idx < p.split)
-        dst = reinterpret_cast<T*>(p.out0) + (static_cast<long long>(b) * p.split + s_idx) * p.ld0 + head * D + hh * OC;
-      else
-        dst = reinterpret_cast<T*>(p.out1) +
-              (static_cast<long long>(b) * (p.S - p.split) + (s_idx - p.split)) * p.ld1 + head * D + hh * OC;
-    }
+    // O += P V: V tile rows = keys (K of the MMA), 128-byte lines = 64 head-dim columns (MN-major, transposed B)
+    mbar_wait(&v_full[stage], phase);
+    wgmma_fence();
 #pragma unroll
-    for (int c = 0; c < OC / 32; ++c) {
-      uint32_t o[32];
-      tmem_ld_32x32(t_o + c * 32, o);
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int gq = 0; gq < 4; ++gq) {
-          uint4 pk4;
-          pk4.x = H16::pack(__uint_as_float(o[gq * 8 + 0]) * inv_l, __uint_as_float(o[gq * 8 + 1]) * inv_l);
-          pk4.y = H16::pack(__uint_as_float(o[gq * 8 + 2]) * inv_l, __uint_as_float(o[gq * 8 + 3]) * inv_l);
-          pk4.z = H16::pack(__uint_as_float(o[gq * 8 + 4]) * inv_l, __uint_as_float(o[gq * 8 + 5]) * inv_l);
-          pk4.w = H16::pack(__uint_as_float(o[gq * 8 + 6]) * inv_l, __uint_as_float(o[gq * 8 + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(dst + c * 32 + gq * 8) = pk4;
-        }
-      }
+    for (int kk = 0; kk < ATT_BKV / 16; ++kk)
+      Wgmma<D, H16::is_bf16, 1>::rs(o, pa[kk], make_smem_desc_sw128(v_base + kk * 16 * 128, ATT_BKV * 128, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[stage]);
+    if (++stage == KS) {
+      stage = 0;
+      phase ^= 1;
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 17) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  // epilogue: complete the row sums over the quad, O / l -> global
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float l = l_run[i];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv_l = 1.0f / l;
+    const int s_idx = q0 + cw * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+    if (s_idx >= p.S) continue;
+    T* dst;
+    if (s_idx < p.split)
+      dst = reinterpret_cast<T*>(p.out0) + (static_cast<long long>(b) * p.split + s_idx) * p.ld0 + head * D;
+    else
+      dst = reinterpret_cast<T*>(p.out1) + (static_cast<long long>(b) * (p.S - p.split) + (s_idx - p.split)) * p.ld1 +
+            head * D;
+#pragma unroll
+    for (int jj = 0; jj < D / 8; ++jj)
+      *reinterpret_cast<uint32_t*>(dst + 8 * jj + col0) =
+          H16::pack(o[4 * jj + 2 * i] * inv_l, o[4 * jj + 2 * i + 1] * inv_l);
   }
-}
-
-
-template <typename T, int D, int POLY4, int VAR = 0>
-__global__ void __launch_bounds__(ATT3_THREADS, 1)
-attention_fwd_v3_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttParams p) {
-  attention_v3_body<T, D, POLY4, VAR>(tmQKV, p);
-}
-
-template <typename T, int D, int POLY4, int VAR = 0>
-static int launch_attention_v3p(dk_ctx* ctx, const CUtensorMap& tm, const AttParams& p, cudaStream_t stream) {
-  using Cfg = Att2Cfg<D>;
-  constexpr int SMEM = Cfg::SMEM_BYTES + 2 * 2 * 128 * 4;   // + partial max / sum exchange
-  auto kern = attention_fwd_v3_kernel<T, D, POLY4, VAR>;
-  static bool configured = false;
-  if (!configured) {
-    DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    configured = true;
-  }
-  dim3 grid(dk_ceil_div(p.S, 2 * ATT_BQ), p.heads, p.B);
-  kern<<<grid, ATT3_THREADS, SMEM, stream>>>(tm, p);
-  DK_LAUNCH_CHECK(ctx);
-  return 0;
-}
-// tuning state: [0] split, [1] poly, [2] stream; -1 = not set (kernel default).  Initialised from the environment
-// (DK_ATT_SPLIT / DK_ATT_POLY / DK_ATT_STREAM), overridable in-process through dk_attention_tuning (same-box A/Bs).
-static int g_att_tuning[3] = {-2, -2, -2};
-static int att_tuning(int i) {
-  if (g_att_tuning[i] == -2) {
-    static const char* names[3] = {"DK_ATT_SPLIT", "DK_ATT_POLY", "DK_ATT_STREAM"};
-    const char* e = getenv(names[i]);
-    g_att_tuning[i] = e ? atoi(e) : -1;
-  }
-  return g_att_tuning[i];
 }
 
 template <typename T, int D>
-static int launch_attention_v3(dk_ctx* ctx, const CUtensorMap& tm, const AttParams& p, cudaStream_t stream) {
-  // Tuning knobs (defaults = the best same-box A/Bs of round 2, profiles/r02_att_*.txt):
-  //   DK_ATT_SPLIT  (default 1): publish P in two parts so that the PV MMAs of the keys published first are issued
-  //                  while the last exponentials are still running (+4.7 % at d = 128)
-  //   DK_ATT_STREAM (default 1, needs the split): streamed exponential pass (VAR bit 32): softmax leg 2130 -> 1910
-  //                  clocks per step in the timestamp trace; over six same-box sweeps +1-3 % at S = 4352 / d = 128,
-  //                  +5-7 % at S = 1280 (C2) and +4-5 % at d = 64
-  //   DK_ATT_POLY   (default 0 for d = 128, 1 for d = 64): of every four exponentials, how many run as a cubic on the
-  //                  FMA pipe instead of MUFU.EX2 (d = 64 is MUFU-bound 2:1: +8-10 %; at d = 128 one in four is a tie
-  //                  at S = 4352 and costs 7 % at S = 1280, two cost 5-10 %)
-  static const char* impl = getenv("DK_ATTENTION_IMPL");
-  const int poly_env = att_tuning(1), split_env = att_tuning(0), stream_env = att_tuning(2);
-  const bool plain = impl != nullptr && impl[0] == '3' && impl[1] == 'p';   // round-1 behaviour: no split, no poly
-  const bool split = !plain && (split_env >= 0 ? split_env != 0 : true);
-  const int poly = plain ? 0 : (poly_env >= 0 ? (poly_env > 2 ? 2 : poly_env) : (D == 64 ? 1 : 0));
-  const bool streamed = split && (stream_env >= 0 ? stream_env != 0 : true);
-  if constexpr (D == 128 && std::is_same<T, __nv_bfloat16>::value) {
-    // DK_ATT_TRACE=<file>: run the diagnostic instantiation (timestamps, poly 0) and dump the table
-    static const char* trace_path = getenv("DK_ATT_TRACE");
-    if (trace_path != nullptr) {
-      constexpr int N = 34 * 32;
-      long long* dbuf = nullptr;
-      DK_CHECK_CUDA(cudaMalloc(&dbuf, N * sizeof(long long)));
-      DK_CHECK_CUDA(cudaMemsetAsync(dbuf, 0, N * sizeof(long long), stream));
-      AttParams pt = p;
-      pt.trace = dbuf;
-      const int rc = streamed ? launch_attention_v3p<__nv_bfloat16, 128, 0, 4 | 16 | 32>(ctx, tm, pt, stream)
-                              : launch_attention_v3p<__nv_bfloat16, 128, 0, 4 | 16>(ctx, tm, pt, stream);
-      DK_CHECK_CUDA(cudaStreamSynchronize(stream));
-      static long long host[N];
-      DK_CHECK_CUDA(cudaMemcpy(host, dbuf, N * sizeof(long long), cudaMemcpyDeviceToHost));
-      cudaFree(dbuf);
-      if (FILE* f = fopen(trace_path, "w")) {
-        for (int i = 0; i < 34; ++i) {
-          for (int k = 0; k < 32; ++k) fprintf(f, "%lld ", host[i * 32 + k]);
-          fprintf(f, "\n");
-        }
-        fclose(f);
-      }
-      return rc;
-    }
+static int launch_attention(dk_ctx* ctx, const CUtensorMap& tm, const AttParams& p, cudaStream_t stream) {
+  auto kern = attention_fwd_kernel<T, D>;
+  static bool configured = false;
+  if (!configured) {
+    DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<D>::SMEM_BYTES));
+    configured = true;
   }
-  if (streamed) {
-    if (poly <= 0) return launch_attention_v3p<T, D, 0, 4 | 32>(ctx, tm, p, stream);
-    if (poly == 1) return launch_attention_v3p<T, D, 1, 4 | 32>(ctx, tm, p, stream);
-    return launch_attention_v3p<T, D, 2, 4 | 32>(ctx, tm, p, stream);
-  }
-  if (split) {
-    if (poly <= 0) return launch_attention_v3p<T, D, 0, 4>(ctx, tm, p, stream);
-    if (poly == 1) return launch_attention_v3p<T, D, 1, 4>(ctx, tm, p, stream);
-    return launch_attention_v3p<T, D, 2, 4>(ctx, tm, p, stream);
-  }
-  if (poly <= 0) return launch_attention_v3p<T, D, 0>(ctx, tm, p, stream);
-  if (poly == 1) return launch_attention_v3p<T, D, 1>(ctx, tm, p, stream);
-  return launch_attention_v3p<T, D, 2>(ctx, tm, p, stream);
+  dim3 grid(dk_ceil_div(p.S, ATT_BQ), p.heads, p.B);
+  kern<<<grid, ATT_THREADS, AttCfg<D>::SMEM_BYTES, stream>>>(tm, p);
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
 }
 
 }  // namespace dk
 
 using namespace dk;
-
-extern "C" int dk_attention_tuning(int split, int poly, int stream) {
-  g_att_tuning[0] = split < 0 ? -1 : split;
-  g_att_tuning[1] = poly < 0 ? -1 : poly;
-  g_att_tuning[2] = stream < 0 ? -1 : stream;
-  return 0;
-}
 
 extern "C" int dk_attention_fwd(dk_ctx* ctx, int dtype, const void* qkv, int B, int S, int heads, int d, float scale,
                                 int split, void* out0, long long ld0, void* out1, long long ld1, void* stream_) {
@@ -596,37 +246,14 @@ extern "C" int dk_attention_fwd(dk_ctx* ctx, int dtype, const void* qkv, int B, 
   p.heads = heads;
   p.split = split;
   p.scale_log2 = scale * 1.44269504088896341f;
-  {
-    static const int dbg = [] { const char* e = getenv("DK_ATT_DEBUG"); return e ? atoi(e) : 0; }();
-    p.debug = dbg;
-  }
   p.out0 = out0;
   p.ld0 = ld0;
   p.out1 = out1;
   p.ld1 = ld1;
-  // default: v3 with the split P publication and the streamed exponential pass (launch_attention_v3); DK_ATTENTION_IMPL=5 selects the persistent
-  // single-pass kernel of attention_v5.cu, 3p the round-1 form of v3
-  static const bool use_v5 = [] {
-    const char* e = getenv("DK_ATTENTION_IMPL");
-    return e != nullptr && e[0] == '5';
-  }();
-  if (use_v5) return dk_launch_attention_v5(ctx, dtype, d, tm, p, stream);
-  static const int env_v6 = [] {   // 6: two threads per row, 7: one thread per row, 8: 7 + one issuer warp per tile
-    const char* e = getenv("DK_ATTENTION_IMPL");
-    return (e != nullptr && (e[0] == '6' || e[0] == '7' || e[0] == '8')) ? e[0] - '0' : 0;
-  }();
-  if (env_v6 != 0 || (att_tuning(2) >= 2 && att_tuning(2) <= 4)) {   // 64-key steps, double-buffered scores (attention_v6.cu)
-    const int one = (env_v6 == 8 || att_tuning(2) == 4) ? 2 : ((env_v6 == 7 || att_tuning(2) == 3) ? 1 : 0);
-    CUtensorMap tm64;
-    const uint32_t box64[2] = {64, 64};
-    if (int rc = dk_make_tmap_16b(ctx, &tm64, qkv, 2, dims, strides, box64)) return rc;
-    const int pe = att_tuning(1);
-    return dk_launch_attention_v6(ctx, dtype, d, pe >= 0 ? pe : (d == 64 ? 1 : 0), one, tm, tm64, p, stream);
-  }
   if (dtype == DK_BF16) {
-    if (d == 128) return launch_attention_v3<__nv_bfloat16, 128>(ctx, tm, p, stream);
-    return launch_attention_v3<__nv_bfloat16, 64>(ctx, tm, p, stream);
+    if (d == 128) return launch_attention<__nv_bfloat16, 128>(ctx, tm, p, stream);
+    return launch_attention<__nv_bfloat16, 64>(ctx, tm, p, stream);
   }
-  if (d == 128) return launch_attention_v3<__half, 128>(ctx, tm, p, stream);
-  return launch_attention_v3<__half, 64>(ctx, tm, p, stream);
+  if (d == 128) return launch_attention<__half, 128>(ctx, tm, p, stream);
+  return launch_attention<__half, 64>(ctx, tm, p, stream);
 }

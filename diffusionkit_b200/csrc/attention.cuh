@@ -1,10 +1,9 @@
-// Shared definitions of the attention kernels (attention.cu: v3, the default; attention_v5.cu: the persistent variant).
+// Shared definitions of the attention kernel (attention.cu).
 #pragma once
 
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
-
-#include <type_traits>
 
 #include "common.cuh"
 #include "host.h"
@@ -17,41 +16,22 @@ constexpr int ATT_BKV = 128;
 struct AttParams {
   int B, S, heads, split;
   float scale_log2;  // scale * log2(e)
-  int debug;         // timing experiments only (DK_ATT_DEBUG): 1 = skip the exponentials, 2 = also skip the max pass
   void* out0;
   long long ld0;
   void* out1;
   long long ld1;
-  long long* trace = nullptr;   // diagnostic instantiation only (DK_ATT_TRACE)
 };
 
-// two 128-row Q tiles per CTA, K / V rings shared by both (v2, v2a, v3)
+// one 128-row Q tile per CTA, K / V ring of KS tiles of 128 keys
 template <int D>
-struct Att2Cfg {
-  static constexpr int KS = (D == 128) ? 2 : 4;      // K / V ring depth
+struct AttCfg {
+  static constexpr int KS = 2;
   static constexpr int TILE_BYTES = 128 * D * 2;
-  static constexpr int OFF_Q = 0;                    // Q_A, Q_B
-  static constexpr int OFF_K = 2 * TILE_BYTES;
+  static constexpr int OFF_Q = 0;
+  static constexpr int OFF_K = TILE_BYTES;
   static constexpr int OFF_V = OFF_K + KS * TILE_BYTES;
   static constexpr int OFF_BAR = OFF_V + KS * TILE_BYTES;
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int TMEM_S = 0;     // + 128 * w
-  static constexpr int TMEM_O = 256;   // + 128 * w
 };
 
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-
 }  // namespace dk
-
-// v5 (attention_v5.cu, DK_ATTENTION_IMPL=5): persistent CTAs, register-resident scores, speculative exponentials
-int dk_launch_attention_v5(dk_ctx* ctx, int dtype, int d, const CUtensorMap& tm, const dk::AttParams& p,
-                           cudaStream_t stream);
-
-// v6 (attention_v6.cu, DK_ATTENTION_IMPL=6): 64-key steps with double-buffered score accumulators
-int dk_launch_attention_v6(dk_ctx* ctx, int dtype, int d, int poly, int one_thread_per_row, const CUtensorMap& tmQ,
-                           const CUtensorMap& tmKV, const dk::AttParams& p, cudaStream_t stream);

@@ -1,8 +1,8 @@
-// diffusionkit_b200 — sm_100a device-side primitives (hand-written PTX wrappers).
+// diffusionkit_b200 — sm_90a device-side primitives (hand-written PTX wrappers).
 //
-// Everything here is the Blackwell programming model spelled out directly:
+// Everything here is the Hopper programming model spelled out directly:
 // mbarrier producer/consumer pipelines, TMA tiled loads (cp.async.bulk.tensor),
-// tcgen05 MMA with TMEM accumulators, tcgen05.ld epilogue reads.  No CUTLASS.
+// wgmma warpgroup MMAs with register accumulators.  No CUTLASS.
 #pragma once
 
 #include <cuda.h>
@@ -11,6 +11,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include "wgmma.cuh"
 
 namespace dk {
 
@@ -83,7 +85,7 @@ __device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
   __syncwarp();
 }
 
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05 operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -115,163 +117,21 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
 }
 
 // --------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA issue, commit, TMEM loads
+// wgmma (warpgroup MMA): A and B read from shared memory through matrix descriptors (A optionally from registers),
+// D accumulated in registers of the 128 threads of a warpgroup.
 // --------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_in_smem, uint32_t ncols) {  // whole warp, .sync.aligned
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_in_smem)),
-               "r"(ncols)
-               : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Arrive (count 1) on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-// Implies tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; single thread issues on behalf of the CTA.  16-bit inputs, fp32 accumulate.
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M=128 rows = TMEM lanes, K 16-bit elements packed two per 32-bit
-// column) is read from tensor memory — used for P in attention (P overlays the S accumulator's columns).
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// --------------------------------------------------------------------------------------------
-// CTA pairs (cluster of 2, tcgen05 cta_group::2): one MMA spans the two SMs of a TPC
-// --------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local_addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  // default (.release.cta) semantics: a cluster-scope release would make the issuing thread drain its outstanding
-  // memory operations (ERRBAR, ~1 us) on every arrive
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx_cluster(uint32_t cluster_addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cluster.b64 _, [%0], %1;" ::"r"(cluster_addr),
-               "r"(bytes)
-               : "memory");
-}
-// TMA store (shared::cta -> global) of a 2-D box, tracked by the thread's bulk async-group
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src_smem, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(map)),
-               "r"(src_smem), "r"(c0), "r"(c1)
-               : "memory");
-}
-// L2 eviction policy for streaming data (written once, read by a later kernel): keeps the operand tiles resident
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap* map, uint32_t src_smem, int c0, int c1,
-                                                  uint64_t policy) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;" ::"l"(
-                   reinterpret_cast<uint64_t>(map)),
-               "r"(src_smem), "r"(c0), "r"(c1), "l"(policy)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all of this thread's committed bulk stores have finished READING shared memory (the buffer may be rewritten)
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// ... and have completed (writes performed)
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// TMA load issued by either CTA of a pair; the transaction bytes are signalled on the barrier at `bar_cluster_addr`
-// (a shared::cluster address — the leader CTA's barrier), the data lands in this CTA's shared memory.
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* map, uint32_t bar_cluster_addr, int c0,
-                                                 int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair_hint(void* dst, const CUtensorMap* map, uint32_t bar_cluster_addr, int c0,
-                                                      int c1, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, "
-      "{%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "l"(policy)
-      : "memory");
-}
-// 0: no hint (evict_normal), 1: evict_first (streamed once), 2: evict_last (operand re-read by later tiles)
-__device__ __forceinline__ uint64_t l2_policy(int kind) {
-  uint64_t p;
-  if (kind == 1)
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  else if (kind == 2)
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  else
-    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_in_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_in_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D (256 rows: 128 TMEM lanes in each CTA of the pair) (+)= A * B, operands read from both CTAs' shared memory at the
-// same offsets; issued by one thread of the leader CTA.
-__device__ __forceinline__ void umma_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the barrier at the same smem offset in every CTA of `cta_mask` once the pair's MMAs retire
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
+// keep the accumulator registers live across the asynchronous MMAs (the compiler must not move reads or writes of them
+// across a wgmma_wait)
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 template <int N>
@@ -288,48 +148,25 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-// exp2 on the FMA pipe (the MUFU unit does 16 ex2 / clk / SM and is the co-bottleneck of attention's softmax):
-// round x to the nearest integer n with the 1.5*2^23 trick, 2^x = 2^n * p(x - n), p = cubic minimax of 2^f on
-// [-0.5, 0.5] (max rel. error 7.5e-5, far below the 16-bit rounding of P), 2^n applied by adding n to the exponent field.
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -126.0f);
-  const float t = x + 12582912.0f;
-  const float f = x - (t - 12582912.0f);
-  float p = fmaf(0.055171624f, f, 0.24261114f);
-  p = fmaf(p, f, 0.69326097f);
-  p = fmaf(p, f, 0.99992806f);
-  return __uint_as_float(__float_as_uint(p) + (__float_as_uint(t) << 23));
-}
-
-// Shared-memory matrix descriptor (sm_100 format, version 1) for a 128B-swizzled tile whose rows are
-// 128-byte lines as written by a TMA box with a 64 x 16-bit inner extent.
+// Shared-memory matrix descriptor (sm_90 wgmma format) for a 128B-swizzled tile whose rows are 128-byte lines as
+// written by a TMA box with a 64 x 16-bit inner extent.
 //   K-major  operand: rows = M/N index, the 128B line holds 64 consecutive K.  SBO = 1024 B (8-row group stride).
+//                     Stepping K by 16 inside the line is a 32-byte start-address step.
 //   MN-major operand: rows = K index, the 128B line holds 64 consecutive M/N.  SBO = 1024 B (8 K-rows),
 //                     LBO = byte stride between successive 64-wide M/N atoms.
+// The swizzle is a function of the shared-memory address bits (chunk ^= line & 7) for the TMA write and the operand
+// read alike, so a start address shifted by whole 128-byte lines addresses the shifted tile (base offset field 0).
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);           // [0,14)  start address >> 4
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;      // [16,30) leading byte offset >> 4
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;      // [32,46) stride byte offset >> 4
-  d |= static_cast<uint64_t>(1) << 46;                               // [46,48) descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                               // [61,64) layout: SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                               // [62,64) layout: SWIZZLE_128B
   return d;
 }
 
-// Split form for issue loops: the high word is loop invariant, the low word is (LBO field | start address >> 4); stepping
-// through stages / K slices is one integer add on the low word.
-__device__ __forceinline__ uint32_t smem_desc_hi_sw128(uint32_t sbo_bytes) {
-  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);
-}
-__device__ __forceinline__ uint32_t smem_desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-__device__ __forceinline__ uint64_t smem_desc_join(uint32_t lo, uint32_t hi) {
-  return (static_cast<uint64_t>(hi) << 32) | lo;
-}
-
-// One lane of a converged warp (the tcgen05 / TMA issue idiom: the whole warp runs the loop so addresses stay in
-// uniform registers; only the issue itself is predicated on the elected lane).
+// One lane of a converged warp (the TMA issue idiom: the whole warp runs the loop so addresses stay in uniform
+// registers; only the issue itself is predicated on the elected lane).
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile(
@@ -340,62 +177,20 @@ __device__ __forceinline__ bool elect_one_sync() {
   return pred != 0;
 }
 
-// Instruction descriptor for kind::f16 (fp16/bf16 in, fp32 accumulate).
-//   [4,6) c format (1 = f32); [7,10) a format (0 = f16, 1 = bf16); [10,13) b format;
-//   [15] a major (0 = K, 1 = MN); [16] b major; [17,23) N >> 3; [24,29) M >> 4.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, bool is_bf16, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | ((is_bf16 ? 1u : 0u) << 7) | ((is_bf16 ? 1u : 0u) << 10) | ((a_mn_major ? 1u : 0u) << 15) |
-         ((b_mn_major ? 1u : 0u) << 16) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+// Accumulator fragment of one m64nN wgmma (this thread's N/2 floats) -> fp32 rows of a shared-memory staging tile.
+// Fragment layout: warp w of the warpgroup owns rows 16w..16w+15; d[4j + 2i + e] is row 16w + lane/4 + 8i,
+// column 8j + 2*(lane%4) + e.
+template <int N>
+__device__ __forceinline__ void stage_acc_rows(float* stage, int ld, int row0, const float (&d)[N / 2]) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + (t >> 5) * 16 + ((t & 31) >> 2);
+  const int c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+      *reinterpret_cast<float2*>(stage + (r + 8 * i) * ld + 8 * j + c) = make_float2(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
 }
-
-// TMEM -> registers: this warp's 32 lanes (TMEM lanes 32*(warp%4) ..), 32 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // --------------------------------------------------------------------------------------------
 // 16-bit type traits (bf16 for FLUX, fp16 for SD3 — reference: mlx/__init__.py:76,610)

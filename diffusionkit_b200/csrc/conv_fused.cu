@@ -1,4 +1,4 @@
-// K7 — fused VAE convolution for sm_100a: [GroupNorm-apply + SiLU] -> [nearest 2x] -> conv 3x3 -> [+bias, +skip]
+// K7 — fused VAE convolution for sm_90a: [GroupNorm-apply + SiLU] -> [nearest 2x] -> conv 3x3 -> [+bias, +skip]
 // -> output + GroupNorm partial statistics of the output, one kernel.
 // Replaces, per ResnetBlock2D / upsample stage of the reference decoder (mlx/vae.py:60-101, 20-25, 146-147):
 //   nn.GroupNorm + nn.SiLU (a separate HBM round trip in round 1), upsample_nearest (a 4x-sized tensor written and read
@@ -8,10 +8,10 @@
 // TMA box brings the (R+2) x 130 pixel halo of the raw input into shared memory (128B-swizzled, one 128-byte line per
 // pixel; out-of-image pixels are zero-filled by the TMA unit = the zero padding).  The nine taps are NOT nine loads:
 // tap (dy, dx) of output row r is the run of 128 consecutive pixel lines starting at halo pixel (r + dy, dx), i.e. the
-// same shared-memory tile read through a UMMA descriptor whose start address is shifted by whole lines.  Every input
+// same shared-memory tile read through a wgmma descriptor whose start address is shifted by whole lines.  Every input
 // byte crosses L2 -> SM once per 64-channel block and n-tile (round 1: nine times).
 //
-// Because the halo is staged once, the GroupNorm affine + SiLU can run ON it: six transform warps rewrite the tile in
+// Because the halo is staged once, the GroupNorm affine + SiLU can run ON it: the consumer threads rewrite the tile in
 // place (normalise with the per-(image, channel) scale/shift table, SiLU with one MUFU.TANH, back to 16 bits; padding
 // pixels stay zero, as the reference pads AFTER the activation) before the MMAs read it — once per input element, not
 // once per tap.
@@ -21,20 +21,15 @@
 // phases (py, px) are four 4-tap convolutions over the SAME halo tile (2.25x fewer FLOPs than convolving the
 // upsampled tensor); the epilogue scatters each phase to its stride-2 output pixels.
 //
-// CTA pairs (cluster of 2, tcgen05 cta_group::2, M = 256): the two CTAs own vertically adjacent row blocks, each loads
-// its own halo and HALF of every 128 x 64 weight tile; shared-memory operand traffic per MMA is 96 B/clk instead of
-// the 128 B/clk a single-CTA 128 x 128 tile needs (the 1024^2 x 128-channel layers ran at 0.85 PFLOP/s for that reason).
-//
-//   warp 14     TMA producer   halo boxes (double buffered per 64-channel block) and weight half-tiles (ring);
-//                              also allocates TMEM: 512 columns = 2 accumulator sets x R rows x 128 channels
-//   warp 15     MMA issuer     leader CTA only
-//   warps 4-11  epilogue       bias, skip, store, per-(pixel row, group) statistics of the stored values
-//   warps 0-3, 12, 13 transform  GroupNorm affine + SiLU in place on the halo (a pass-through when there is no norm);
-//               (measured against transform = warps 8-13 above an epilogue on warps 0-7: 1.22 vs 1.54 ms on the
-//               1024^2 x 128 norm+SiLU layer)
-// The schedulers favour the highest warp id of their quarter, so the single-thread MMA issuer and the TMA producer sit
-// ABOVE every other warp: with the issuer as warp 1 the mere loop skeleton of a busy transform warp on the same
-// scheduler cost 25 % of the kernel's throughput (measured).
+// One CTA per work item (R x 128 output pixels x 128 output channels of one image / phase), 384 threads:
+//   warpgroup 0 (warp 0) TMA producer: halo boxes (double buffered per 64-channel block) and 128 x 64 weight tiles
+//                        (ring)
+//   warpgroups 1, 2      output row r = warpgroup - 1: two wgmma m64n128k16 chains (pixels 0-63 and 64-127 of the
+//                        row) per tap, A = the halo tile read through a line-shifted descriptor.  Before the MMAs of
+//                        a block the 256 threads apply GroupNorm affine + SiLU in place on the halo (a pass-through
+//                        when there is no norm).
+//   epilogue             the accumulators go through an fp32 staging tile in the (then idle) pipeline buffers; bias,
+//                        skip, store, per-(pixel row, group) statistics of the stored values.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -48,23 +43,24 @@ constexpr int CF_BN = 128;
 constexpr int CF_HW = CF_TW + 2;                       // halo width in pixels
 constexpr int CF_HR = CF_R + 2;                        // halo rows
 constexpr int CF_A_BYTES = CF_HR * CF_HW * 128;        // 66,560 (65 KB) per 64-channel block
-constexpr int CF_B_BYTES = (CF_BN / 2) * 64 * 2;       // 8 KB: this CTA's half of one tap's weight tile
-constexpr int CF_A_BUFS = 2;                            // halo buffers (a third one at the price of a 3-deep weight ring was measured: slower)
-constexpr int CF_B_STAGES = 10;                         // weight ring: 8 KB per stage; at 3 stages the kernel loses 20-40 %
-constexpr int CF_THREADS = 512;
-constexpr int CF_TWARPS = 6;                           // transform warps: 0-3, 12, 13
-constexpr int CF_STAT_BYTES = 2 * 8 * CF_R * 2 * 8 * 2 * 4;   // [parity][warp][row][chunk][group<=8][sum,sumsq]
+constexpr int CF_B_BYTES = CF_BN * 64 * 2;             // 16 KB: one tap's 128 x 64 weight tile
+constexpr int CF_A_BUFS = 2;                            // halo buffers
+constexpr int CF_B_STAGES = 4;                          // weight ring
+constexpr int CF_THREADS = 384;
+constexpr int CF_STAGE_LD = CF_BN + 4;                  // fp32 staging row stride (floats)
+constexpr int CF_STAT_BYTES = 8 * CF_R * 2 * 8 * 2 * 4;  // [warp][row][chunk][group<=8][sum,sumsq]
 constexpr int CF_OFF_B = CF_A_BUFS * CF_A_BYTES;
 constexpr int CF_OFF_STAT = CF_OFF_B + CF_B_STAGES * CF_B_BYTES;
 constexpr int CF_OFF_BAR = CF_OFF_STAT + CF_STAT_BYTES;
 constexpr int CF_SMEM_BYTES = CF_OFF_BAR + 256 + 1024;
+static_assert(CF_OFF_STAT >= CF_R * CF_TW * CF_STAGE_LD * 4, "conv_fused: the staging tile reuses the pipeline buffers");
 static_assert(CF_SMEM_BYTES <= 232448, "conv_fused: shared memory budget");
 
 struct ConvFParams {
   int B, H, W;          // grid of tile coordinates = the conv INPUT image (source image in upsample mode)
   int Cin, Cout;
   int up;               // 0: 3x3 conv (output H x W); 1: nearest 2x then 3x3 conv, by sub-pixel phases (output 2H x 2W)
-  int tiles_x, tiles_y; // W / 128, H / (2 * R)
+  int tiles_x, tiles_y; // W / 128, H / R
   int n_tiles;          // Cout / 128
   const void* bias;     // [Cout] or null
   const void* res;      // output-shaped skip tensor or null
@@ -74,19 +70,10 @@ struct ConvFParams {
   const void* beta;
   int G;
   int silu;
-  int debug;            // timing experiments (DK_CF_DEBUG): 1 transform = load/store only, 2 = math only, 3 = neither
   float* out_partial;   // [B, slots, out_G, 2] per-(128-pixel row segment, group) (sum, sumsq) of the output, or null
   int out_G;
 };
 
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const CUtensorMap* map, uint32_t bar_cluster_addr, int c0,
-                                                 int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -166,7 +153,7 @@ __device__ __forceinline__ void cf_chunk_stats(const float (&v)[32], float* dst,
 }
 
 template <typename T>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CF_THREADS, 1)
+__global__ void __launch_bounds__(CF_THREADS, 1)
 conv_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const ConvFParams p) {
   using H16 = Half16<T>;
   extern __shared__ uint8_t smem_raw[];
@@ -175,370 +162,302 @@ conv_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
   uint8_t* sB = smem + CF_OFF_B;            // [CF_B_STAGES][CF_B_BYTES]
   float* sstat = reinterpret_cast<float*>(smem + CF_OFF_STAT);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + CF_OFF_BAR);
-  uint64_t* a_land = bars;                  // [CF_A_BUFS] local: TMA halo landed in THIS CTA
-  uint64_t* a_ready = a_land + CF_A_BUFS;   // [CF_A_BUFS] leader's copy live: both CTAs' halos transformed
-  uint64_t* a_empty = a_ready + CF_A_BUFS;  // [CF_A_BUFS] multicast commit: the MMAs reading the buffer have retired
-  uint64_t* b_full = a_empty + CF_A_BUFS;   // [CF_B_STAGES] leader's copy live (2 expect_tx arrivals)
-  uint64_t* b_empty = b_full + CF_B_STAGES; // [CF_B_STAGES] multicast commit
-  uint64_t* tfull = b_empty + CF_B_STAGES;  // [2] multicast commit: accumulator set complete
-  uint64_t* tempty = tfull + 2;             // [2] leader's copy live: 16 epilogue-warp arrivals
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* a_land = bars;                  // [CF_A_BUFS] TMA halo landed
+  uint64_t* a_empty = a_land + CF_A_BUFS;   // [CF_A_BUFS] the MMAs reading the buffer have retired (8 consumer warps)
+  uint64_t* b_full = a_empty + CF_A_BUFS;   // [CF_B_STAGES]
+  uint64_t* b_empty = b_full + CF_B_STAGES; // [CF_B_STAGES] (8 consumer warps)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair_id = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-  const int phases = p.up ? 4 : 1;
-  const int total_items = p.B * p.tiles_y * p.tiles_x * phases * p.n_tiles;
+  const int wg = threadIdx.x >> 7;
   const int cblocks = p.Cin / 64;
   const int ntaps = p.up ? 4 : 9;
+  CfItem it;
+  cf_decode(p, blockIdx.x, it);
+  const int py = it.phase >> 1, px = it.phase & 1;
+  const int y0 = it.ty * CF_R;
+  const int x0 = it.tx * CF_TW;
 
-  if (warp == 14 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
-  }
-  if (warp == 15 && lane == 0) {
     for (int i = 0; i < CF_A_BUFS; ++i) {
       mbar_init(&a_land[i], 1);
-      mbar_init(&a_ready[i], 2 * CF_TWARPS);
-      mbar_init(&a_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 16);
+      mbar_init(&a_empty[i], 8);
     }
     for (int i = 0; i < CF_B_STAGES; ++i) {
-      mbar_init(&b_full[i], 2);
-      mbar_init(&b_empty[i], 1);
+      mbar_init(&b_full[i], 1);
+      mbar_init(&b_empty[i], 8);
     }
     fence_barrier_init();
   }
-  cluster_sync_all();
-  if (warp == 14) {
-    tmem_alloc_pair(tmem_slot, 512);
-    tmem_relinquish_pair();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 14) {
-    // ------------------------------------------------------------------ TMA producer (both CTAs), converged warp
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer, converged warp
+    if (warp != 0) return;
     uint32_t bst = 0, bph = 0;     // weight ring
     uint32_t abuf = 0, aph = 0;    // halo double buffer
-    for (int item = pair_id; item < total_items; item += num_pairs) {
-      CfItem it;
-      cf_decode(p, item, it);
-      const int y0 = (it.ty * 2 + static_cast<int>(rank)) * CF_R;
-      const int x0 = it.tx * CF_TW;
-      const int w_row = it.phase * p.Cout + it.nt * CF_BN + static_cast<int>(rank) * (CF_BN / 2);
-      for (int cb = 0; cb < cblocks; ++cb) {
-        mbar_wait_warp(&a_empty[abuf], aph ^ 1);
+    const int w_row = it.phase * p.Cout + it.nt * CF_BN;
+    for (int cb = 0; cb < cblocks; ++cb) {
+      mbar_wait_warp(&a_empty[abuf], aph ^ 1);
+      if (elect_one_sync()) {
+        mbar_arrive_expect_tx(&a_land[abuf], CF_A_BYTES);
+        tma_load_4d(sA + abuf * CF_A_BYTES, &tmX, &a_land[abuf], cb * 64, x0 - 1, y0 - 1, it.b);
+      }
+      __syncwarp();
+      if (++abuf == CF_A_BUFS) {
+        abuf = 0;
+        aph ^= 1;
+      }
+      for (int tap = 0; tap < ntaps; ++tap) {
+        mbar_wait_warp(&b_empty[bst], bph ^ 1);
         if (elect_one_sync()) {
-          mbar_arrive_expect_tx(&a_land[abuf], CF_A_BYTES);
-          tma_load_4d(sA + abuf * CF_A_BYTES, &tmX, &a_land[abuf], cb * 64, x0 - 1, y0 - 1, it.b);
+          mbar_arrive_expect_tx(&b_full[bst], CF_B_BYTES);
+          tma_load_2d(sB + bst * CF_B_BYTES, &tmW, &b_full[bst], tap * p.Cin + cb * 64, w_row);
         }
         __syncwarp();
-        if (++abuf == CF_A_BUFS) {
-          abuf = 0;
-          aph ^= 1;
-        }
-        for (int tap = 0; tap < ntaps; ++tap) {
-          mbar_wait_warp(&b_empty[bst], bph ^ 1);
-          if (elect_one_sync()) {
-            const uint32_t full_leader = mapa_u32(smem_u32(&b_full[bst]), 0);
-            mbar_arrive_expect_tx_cluster(full_leader, CF_B_BYTES);
-            tma_load_2d_pair(sB + bst * CF_B_BYTES, &tmW, full_leader, tap * p.Cin + cb * 64, w_row);
-          }
-          __syncwarp();
-          if (++bst == CF_B_STAGES) {
-            bst = 0;
-            bph ^= 1;
-          }
+        if (++bst == CF_B_STAGES) {
+          bst = 0;
+          bph ^= 1;
         }
       }
     }
-  } else if (warp == 15) {
-    if (leader) {
-      // ---------------------------------------------------------------- MMA issuer (leader CTA only), converged warp
-      constexpr uint32_t idesc = make_idesc_f16(256, CF_BN, H16::is_bf16, false, false);
-      const uint32_t desc_hi = smem_desc_hi_sw128(1024);
-      const uint32_t a_addr0 = smem_u32(sA);
-      const uint32_t b_lo0 = smem_desc_lo(smem_u32(sB), 0);
-      uint32_t bst = 0, bph = 0, abuf = 0, aph = 0, n_it = 0;
-      for (int item = pair_id; item < total_items; item += num_pairs, ++n_it) {
-        CfItem it;
-        cf_decode(p, item, it);
-        const int py = it.phase >> 1, px = it.phase & 1;
-        const uint32_t acc = n_it & 1u;
-        mbar_wait_warp(&tempty[acc], ((n_it >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        for (int cb = 0; cb < cblocks; ++cb) {
-          mbar_wait_warp(&a_ready[abuf], aph);
-          tc_fence_after();
-          for (int tap = 0; tap < ntaps; ++tap) {
-            // halo offset of this tap: 3x3 -> (tap / 3, tap % 3); phase (py, px) of the upsampled conv -> (a + py, b + px)
-            const int dy = p.up ? ((tap >> 1) + py) : (tap / 3);
-            const int dx = p.up ? ((tap & 1) + px) : (tap - (tap / 3) * 3);
-            mbar_wait_warp(&b_full[bst], bph);
-            tc_fence_after();
-            if (elect_one_sync()) {
-              const uint32_t b_lo = b_lo0 + bst * (CF_B_BYTES >> 4);
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers: output row rr of the item
+  const int rr = wg - 1;
+  const int tid = threadIdx.x - 128;          // 0..255
+  float acc0[CF_BN / 2], acc1[CF_BN / 2];     // pixels 0-63 / 64-127 of the row
 #pragma unroll
-              for (int rr = 0; rr < CF_R; ++rr) {
-                const uint32_t a_addr = a_addr0 + abuf * CF_A_BYTES + ((rr + dy) * CF_HW + dx) * 128;
-                // line-shifted start address, descriptor base-offset field left 0: the 128B swizzle is a function of the
-                // shared-memory ADDRESS bits (chunk ^= line & 7), for the TMA write and for the operand read alike —
-                // verified on hardware (setting base offset = (address >> 7) & 7 produces wrong results)
-                const uint32_t a_lo = smem_desc_lo(a_addr, 0);
-                const uint32_t d_tmem = tmem_base + acc * (CF_R * CF_BN) + rr * CF_BN;
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  umma_ss_pair(d_tmem, smem_desc_join(a_lo + k * 2, desc_hi), smem_desc_join(b_lo + k * 2, desc_hi), idesc,
-                               (cb | tap | k) != 0 ? 1u : 0u);
-              }
-              umma_commit_pair(&b_empty[bst], 3);
-              if (tap == ntaps - 1) {
-                umma_commit_pair(&a_empty[abuf], 3);
-                if (cb == cblocks - 1) umma_commit_pair(&tfull[acc], 3);
-              }
-            }
-            __syncwarp();
-            if (++bst == CF_B_STAGES) {
-              bst = 0;
-              bph ^= 1;
-            }
-          }
-          if (++abuf == CF_A_BUFS) {
-            abuf = 0;
-            aph ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp < 4 || warp >= 12) {
-    // ------------------------------------------------------------------ transform warps: GroupNorm affine + SiLU in place
-    // Six warps (192 threads); a thread owns one logical 16-byte chunk (8 channels) of every 24th halo pixel, two pixels
-    // per iteration with both shared-memory loads issued first.  Budget per 64-channel block: the MMAs of the block take
-    // 9 taps x 2 rows x 256 clk = 4608 clk; 33,280 halo elements need 2080 clk of MUFU.TANH (16 / clk / SM).
-    const int tw = warp >= 12 ? warp - 8 : warp;         // 0..5
-    const int tid = tw * 32 + lane;                       // 0..191
-    constexpr int TT = CF_TWARPS * 32;
+  for (int i = 0; i < CF_BN / 2; ++i) {
+    acc0[i] = 0.f;
+    acc1[i] = 0.f;
+  }
+  {
+    constexpr int TT = 256;
     const int chunk = tid & 7;                 // logical 16-byte chunk = 8 channels of the 64-channel block
     const int cpg = p.gn_stats != nullptr ? p.Cin / p.G : 1;
-    uint32_t abuf = 0, aph = 0;
-    for (int item = pair_id; item < total_items; item += num_pairs) {
-      CfItem it;
-      cf_decode(p, item, it);
-      const int y0 = (it.ty * 2 + static_cast<int>(rank)) * CF_R;
-      const int x0 = it.tx * CF_TW;
-      for (int cb = 0; cb < cblocks; ++cb) {
-        mbar_wait(&a_land[abuf], aph);
-        if (p.gn_stats != nullptr) {
-          // per-channel (scale, shift) of this image: y = x * (rstd * gamma) + (beta - mean * rstd * gamma); the 8
-          // channels of this thread's chunk come straight from global memory (a few hundred bytes per image, L1-resident)
-          float sc[8], sh[8];
-          {
-            const int c0 = cb * 64 + chunk * 8;
-            const uint4 g4 = *reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(p.gamma) + c0);
-            const uint4 b4 = *reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(p.beta) + c0);
-            const uint32_t gw[4] = {g4.x, g4.y, g4.z, g4.w}, bw[4] = {b4.x, b4.y, b4.z, b4.w};
+    uint32_t bst = 0, bph = 0, abuf = 0, aph = 0;
+    for (int cb = 0; cb < cblocks; ++cb) {
+      mbar_wait(&a_land[abuf], aph);
+      if (p.gn_stats != nullptr) {
+        // GroupNorm affine + SiLU in place.  Per-channel (scale, shift) of this image: y = x * (rstd * gamma) +
+        // (beta - mean * rstd * gamma); the 8 channels of this thread's chunk come straight from global memory
+        float sc[8], sh[8];
+        {
+          const int c0 = cb * 64 + chunk * 8;
+          const uint4 g4 = *reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(p.gamma) + c0);
+          const uint4 b4 = *reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(p.beta) + c0);
+          const uint32_t gw[4] = {g4.x, g4.y, g4.z, g4.w}, bw[4] = {b4.x, b4.y, b4.z, b4.w};
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 gf = H16::unpack(gw[i]), bf = H16::unpack(bw[i]);
+          for (int i = 0; i < 4; ++i) {
+            const float2 gf = H16::unpack(gw[i]), bf = H16::unpack(bw[i]);
 #pragma unroll
-              for (int h2 = 0; h2 < 2; ++h2) {
-                const int g = (c0 + 2 * i + h2) / cpg;
-                const float mean = __ldg(p.gn_stats + (it.b * p.G + g) * 2), rstd = __ldg(p.gn_stats + (it.b * p.G + g) * 2 + 1);
-                const float ga = h2 ? gf.y : gf.x, be = h2 ? bf.y : bf.x;
-                sc[2 * i + h2] = rstd * ga;
-                sh[2 * i + h2] = be - mean * rstd * ga;
-              }
+            for (int h2 = 0; h2 < 2; ++h2) {
+              const int g = (c0 + 2 * i + h2) / cpg;
+              const float mean = __ldg(p.gn_stats + (it.b * p.G + g) * 2), rstd = __ldg(p.gn_stats + (it.b * p.G + g) * 2 + 1);
+              const float ga = h2 ? gf.y : gf.x, be = h2 ? bf.y : bf.x;
+              sc[2 * i + h2] = rstd * ga;
+              sh[2 * i + h2] = be - mean * rstd * ga;
             }
           }
-          const uint32_t base = smem_u32(sA) + abuf * CF_A_BYTES;
-          const bool do_silu = p.silu != 0;
-          // padding pixels (outside the image) stay zero: the reference pads AFTER the activation
-          auto in_image = [&](int q) {
-            const int hr = q / CF_HW, hx = q - hr * CF_HW;
-            const int gy = y0 - 1 + hr, gx = x0 - 1 + hx;
-            return q < CF_HR * CF_HW && gy >= 0 && gy < p.H && gx >= 0 && gx < p.W;
-          };
-          auto xform = [&](uint32_t (&w)[4]) {
+        }
+        const uint32_t base = smem_u32(sA) + abuf * CF_A_BYTES;
+        const bool do_silu = p.silu != 0;
+        // padding pixels (outside the image) stay zero: the reference pads AFTER the activation
+        auto in_image = [&](int q) {
+          const int hr = q / CF_HW, hx = q - hr * CF_HW;
+          const int gy = y0 - 1 + hr, gx = x0 - 1 + hx;
+          return q < CF_HR * CF_HW && gy >= 0 && gy < p.H && gx >= 0 && gx < p.W;
+        };
+        auto xform = [&](uint32_t (&w)[4]) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 f = H16::unpack(w[i]);
-              float a = fmaf(f.x, sc[2 * i], sh[2 * i]);
-              float b = fmaf(f.y, sc[2 * i + 1], sh[2 * i + 1]);
-              if (do_silu) {   // x * sigmoid(x) = h + h * tanh(h), h = x / 2: one MUFU op per element
-                const float ha = 0.5f * a, hb = 0.5f * b;
-                a = fmaf(ha, tanh_approx(ha), ha);
-                b = fmaf(hb, tanh_approx(hb), hb);
-              }
-              w[i] = H16::pack(a, b);
+          for (int i = 0; i < 4; ++i) {
+            const float2 f = H16::unpack(w[i]);
+            float a = fmaf(f.x, sc[2 * i], sh[2 * i]);
+            float b = fmaf(f.y, sc[2 * i + 1], sh[2 * i + 1]);
+            if (do_silu) {   // x * sigmoid(x) = h + h * tanh(h), h = x / 2: one MUFU op per element
+              const float ha = 0.5f * a, hb = 0.5f * b;
+              a = fmaf(ha, tanh_approx(ha), ha);
+              b = fmaf(hb, tanh_approx(hb), hb);
             }
-          };
-          for (int q0 = (p.debug & 8) ? CF_HR * CF_HW : (tid >> 3); q0 < CF_HR * CF_HW; q0 += 2 * (TT / 8)) {
-            const int q1 = q0 + TT / 8;
-            const bool ok0 = in_image(q0), ok1 = in_image(q1);
-            const uint32_t addr0 = base + q0 * 128 + ((chunk ^ (q0 & 7)) << 4);
-            const uint32_t addr1 = base + q1 * 128 + ((chunk ^ (q1 & 7)) << 4);
-            uint32_t w0[4] = {0u, 0u, 0u, 0u}, w1[4] = {0u, 0u, 0u, 0u};
-            const bool mem = !(p.debug & 2), math = !(p.debug & 1);
-            if (ok0 && mem) asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0[0]), "=r"(w0[1]), "=r"(w0[2]), "=r"(w0[3]) : "r"(addr0));
-            if (ok1 && mem) asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w1[0]), "=r"(w1[1]), "=r"(w1[2]), "=r"(w1[3]) : "r"(addr1));
-            if (math) {
-              xform(w0);
-              xform(w1);
-            }
-            if (ok0 && mem) asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr0), "r"(w0[0]), "r"(w0[1]), "r"(w0[2]), "r"(w0[3]) : "memory");
-            if (ok1 && mem) asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr1), "r"(w1[0]), "r"(w1[1]), "r"(w1[2]), "r"(w1[3]) : "memory");
-            if (!mem && (w0[0] ^ w1[3]) == 0x12345u) asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr0), "r"(w0[1]) : "memory");   // keep the math alive
+            w[i] = H16::pack(a, b);
           }
-          if (!(p.debug & 4)) fence_proxy_async_smem();   // generic-proxy writes -> visible to the tensor core's operand reads
+        };
+        for (int q0 = tid >> 3; q0 < CF_HR * CF_HW; q0 += 2 * (TT / 8)) {
+          const int q1 = q0 + TT / 8;
+          const bool ok0 = in_image(q0), ok1 = in_image(q1);
+          const uint32_t addr0 = base + q0 * 128 + ((chunk ^ (q0 & 7)) << 4);
+          const uint32_t addr1 = base + q1 * 128 + ((chunk ^ (q1 & 7)) << 4);
+          uint32_t w0[4] = {0u, 0u, 0u, 0u}, w1[4] = {0u, 0u, 0u, 0u};
+          if (ok0) asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0[0]), "=r"(w0[1]), "=r"(w0[2]), "=r"(w0[3]) : "r"(addr0));
+          if (ok1) asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w1[0]), "=r"(w1[1]), "=r"(w1[2]), "=r"(w1[3]) : "r"(addr1));
+          xform(w0);
+          xform(w1);
+          if (ok0) asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr0), "r"(w0[0]), "r"(w0[1]), "r"(w0[2]), "r"(w0[3]) : "memory");
+          if (ok1) asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr1), "r"(w1[0]), "r"(w1[1]), "r"(w1[2]), "r"(w1[3]) : "memory");
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&a_ready[abuf]), 0));
-        if (++abuf == CF_A_BUFS) {
-          abuf = 0;
-          aph ^= 1;
+        fence_proxy_async_smem();   // generic-proxy writes -> visible to the tensor core's operand reads
+        named_bar_sync(1, 256);     // the whole halo is transformed before either warpgroup reads it
+      }
+      const uint32_t a_addr0 = smem_u32(sA) + abuf * CF_A_BYTES;
+      uint32_t prev = 0;
+      for (int tap = 0; tap < ntaps; ++tap) {
+        // halo offset of this tap: 3x3 -> (tap / 3, tap % 3); phase (py, px) of the upsampled conv -> (a + py, b + px)
+        const int dy = p.up ? ((tap >> 1) + py) : (tap / 3);
+        const int dx = p.up ? ((tap & 1) + px) : (tap - (tap / 3) * 3);
+        mbar_wait(&b_full[bst], bph);
+        const uint32_t b_addr = smem_u32(sB) + bst * CF_B_BYTES;
+        const uint32_t a_addr = a_addr0 + ((rr + dy) * CF_HW + dx) * 128;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint32_t acc_on = (cb | tap | k) != 0 ? 1u : 0u;
+          const uint64_t db = make_smem_desc_sw128(b_addr + k * 32, 16, 1024);
+          Wgmma<CF_BN, H16::is_bf16, 0>::ss(acc0, make_smem_desc_sw128(a_addr + k * 32, 16, 1024), db, acc_on);
+          Wgmma<CF_BN, H16::is_bf16, 0>::ss(acc1, make_smem_desc_sw128(a_addr + 64 * 128 + k * 32, 16, 1024), db, acc_on);
         }
+        wgmma_commit();
+        if (tap > 0) {   // the previous tap's MMAs have retired: its weight stage can be refilled
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&b_empty[prev]);
+        }
+        prev = bst;
+        if (++bst == CF_B_STAGES) {
+          bst = 0;
+          bph ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) {
+        mbar_arrive(&b_empty[prev]);
+        mbar_arrive(&a_empty[abuf]);
+      }
+      if (++abuf == CF_A_BUFS) {
+        abuf = 0;
+        aph ^= 1;
       }
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 4-11): this CTA's R x 128 output pixels
-    const int quarter = warp & 3;
-    const int half = (warp - 4) >> 2;           // 64-channel half of the 128-channel tile
-    const int xl = quarter * 32 + lane;         // pixel inside the 128-pixel segment
-    const T* bias = reinterpret_cast<const T*>(p.bias);
-    const T* res = reinterpret_cast<const T*>(p.res);
-    T* out = reinterpret_cast<T*>(p.out);
-    const int Hout = p.up ? 2 * p.H : p.H, Wout = p.up ? 2 * p.W : p.W;
-    const int cpg_out = p.out_partial != nullptr ? p.Cout / p.out_G : 8;
-    const int slots = (Hout * Wout) / CF_TW;
-    uint32_t n_it = 0;
-    for (int item = pair_id; item < total_items; item += num_pairs, ++n_it) {
-      CfItem it;
-      cf_decode(p, item, it);
-      const int py = it.phase >> 1, px = it.phase & 1;
-      const uint32_t acc = n_it & 1u;
-      const int y0 = (it.ty * 2 + static_cast<int>(rank)) * CF_R;
-      const int x = it.tx * CF_TW + xl;
-      const int n_base = it.nt * CF_BN + half * 64;
-      mbar_wait_warp(&tfull[acc], (n_it >> 1) & 1u);
-      tc_fence_after();
-      float* st_my = sstat + (((n_it & 1u) * 8 + (warp - 4)) * CF_R) * (2 * 8 * 2);
+    reg_fence(acc0);
+    reg_fence(acc1);
+  }
+
+  // ------------------------------------------------------------------ epilogue: R x 128 output pixels
+  // every load has landed and every MMA has retired once both warpgroups pass this barrier: the pipeline buffers
+  // become the fp32 staging tile [R * 128 pixels][CF_STAGE_LD]
+  float* stg = reinterpret_cast<float*>(smem);
+  named_bar_sync(1, 256);
+  stage_acc_rows<CF_BN>(stg, CF_STAGE_LD, rr * CF_TW, acc0);
+  stage_acc_rows<CF_BN>(stg, CF_STAGE_LD, rr * CF_TW + 64, acc1);
+  named_bar_sync(1, 256);
+
+  const int ew = warp - 4;                    // 0..7
+  const int quarter = ew & 3;
+  const int half = ew >> 2;                   // 64-channel half of the 128-channel tile
+  const int xl = quarter * 32 + lane;         // pixel inside the 128-pixel segment
+  const T* bias = reinterpret_cast<const T*>(p.bias);
+  const T* res = reinterpret_cast<const T*>(p.res);
+  T* out = reinterpret_cast<T*>(p.out);
+  const int Hout = p.up ? 2 * p.H : p.H, Wout = p.up ? 2 * p.W : p.W;
+  const int cpg_out = p.out_partial != nullptr ? p.Cout / p.out_G : 8;
+  const int slots = (Hout * Wout) / CF_TW;
+  const int x = x0 + xl;
+  const int n_base = it.nt * CF_BN + half * 64;
+  float* st_my = sstat + (ew * CF_R) * (2 * 8 * 2);
+#pragma unroll 1
+  for (int r2 = 0; r2 < CF_R; ++r2) {
+    const int oy = p.up ? 2 * (y0 + r2) + py : (y0 + r2);
+    const int ox = p.up ? 2 * x + px : x;
+    const long long orow = (static_cast<long long>(it.b) * Hout + oy) * Wout + ox;
 #pragma unroll
-      for (int rr = 0; rr < CF_R; ++rr) {
-        const int oy = p.up ? 2 * (y0 + rr) + py : (y0 + rr);
-        const int ox = p.up ? 2 * x + px : x;
-        const long long orow = (static_cast<long long>(it.b) * Hout + oy) * Wout + ox;
+    for (int ch = 0; ch < 2; ++ch) {
+      const float* src = stg + (r2 * CF_TW + xl) * CF_STAGE_LD + half * 64 + ch * 32;
+      const int n0 = n_base + ch * 32;
+      float v[32];
 #pragma unroll
-        for (int ch = 0; ch < 2; ++ch) {
-          uint32_t r[32];
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * (CF_R * CF_BN) + rr * CF_BN +
-                            half * 64 + ch * 32,
-                        r);
-          tmem_ld_wait();
-          if (rr == CF_R - 1 && ch == 1) {   // this warp's last TMEM read of the accumulator set
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[acc]), 0));
-          }
-          const int n0 = n_base + ch * 32;
-          float v[32];
+      for (int j = 0; j < 4; ++j) {
+        if (n0 + j * 8 >= p.Cout) {   // narrow output tile (conv_out): channels beyond Cout do not exist
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (n0 + j * 8 >= p.Cout) {   // narrow output tile (conv_out): channels beyond Cout do not exist
+          for (int i = 0; i < 8; ++i) v[j * 8 + i] = 0.f;
+          continue;
+        }
+        const float4 a4 = *reinterpret_cast<const float4*>(src + j * 8);
+        const float4 b4f = *reinterpret_cast<const float4*>(src + j * 8 + 4);
+        const float r[8] = {a4.x, a4.y, a4.z, a4.w, b4f.x, b4f.y, b4f.z, b4f.w};
+        float bv[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (bias != nullptr) {
+          const uint4 b4 = *reinterpret_cast<const uint4*>(bias + n0 + j * 8);
+          const uint32_t bw[4] = {b4.x, b4.y, b4.z, b4.w};
 #pragma unroll
-              for (int i = 0; i < 8; ++i) v[j * 8 + i] = 0.f;
-              continue;
-            }
-            float bv[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            if (bias != nullptr) {
-              const uint4 b4 = *reinterpret_cast<const uint4*>(bias + n0 + j * 8);
-              const uint32_t bw[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float2 f = H16::unpack(bw[i]);
-                bv[2 * i] = f.x;
-                bv[2 * i + 1] = f.y;
-              }
-            }
-            float rv[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            if (res != nullptr) {
-              const uint4 r4 = *reinterpret_cast<const uint4*>(res + orow * p.Cout + n0 + j * 8);
-              const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float2 f = H16::unpack(rw[i]);
-                rv[2 * i] = f.x;
-                rv[2 * i + 1] = f.y;
-              }
-            }
-            uint32_t w16[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float a = __uint_as_float(r[j * 8 + 2 * i]) + bv[2 * i] + rv[2 * i];
-              const float b = __uint_as_float(r[j * 8 + 2 * i + 1]) + bv[2 * i + 1] + rv[2 * i + 1];
-              w16[i] = H16::pack(a, b);
-              const float2 back = H16::unpack(w16[i]);   // statistics of what is STORED
-              v[j * 8 + 2 * i] = back.x;
-              v[j * 8 + 2 * i + 1] = back.y;
-            }
-            *reinterpret_cast<uint4*>(out + orow * p.Cout + n0 + j * 8) = make_uint4(w16[0], w16[1], w16[2], w16[3]);
-          }
-          if (p.out_partial != nullptr) {
-            float* dst = st_my + ((rr * 2 + ch) * 8) * 2;
-            if (cpg_out == 4)
-              cf_chunk_stats<4>(v, dst, lane);
-            else if (cpg_out == 8)
-              cf_chunk_stats<8>(v, dst, lane);
-            else
-              cf_chunk_stats<16>(v, dst, lane);
+          for (int i = 0; i < 4; ++i) {
+            const float2 f = H16::unpack(bw[i]);
+            bv[2 * i] = f.x;
+            bv[2 * i + 1] = f.y;
           }
         }
+        float rv[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (res != nullptr) {
+          const uint4 r4 = *reinterpret_cast<const uint4*>(res + orow * p.Cout + n0 + j * 8);
+          const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float2 f = H16::unpack(rw[i]);
+            rv[2 * i] = f.x;
+            rv[2 * i + 1] = f.y;
+          }
+        }
+        uint32_t w16[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float a = r[2 * i] + bv[2 * i] + rv[2 * i];
+          const float b = r[2 * i + 1] + bv[2 * i + 1] + rv[2 * i + 1];
+          w16[i] = H16::pack(a, b);
+          const float2 back = H16::unpack(w16[i]);   // statistics of what is STORED
+          v[j * 8 + 2 * i] = back.x;
+          v[j * 8 + 2 * i + 1] = back.y;
+        }
+        *reinterpret_cast<uint4*>(out + orow * p.Cout + n0 + j * 8) = make_uint4(w16[0], w16[1], w16[2], w16[3]);
       }
       if (p.out_partial != nullptr) {
-        // fold the four pixel quarters in fixed order (deterministic) and publish one (sum, sumsq) per 128-pixel row
-        // segment and group
-        named_bar_sync(1, 256);
-        const int ng = 32 / cpg_out;
-        const int t = threadIdx.x - 128;        // 0..255
-        const int per_row = 2 * 2 * ng;         // halves x chunks x groups of this tile, per output row
-        if (t < CF_R * per_row) {
-          const int rr = t / per_row;
-          const int rem = t - rr * per_row;
-          const int hf = rem / (2 * ng);
-          const int ch = (rem / ng) & 1;
-          const int g = rem % ng;
-          float s = 0.f, q = 0.f;
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {
-            const float* src = sstat + (((n_it & 1u) * 8 + (hf * 4 + qd)) * CF_R) * (2 * 8 * 2) + ((rr * 2 + ch) * 8 + g) * 2;
-            s += src[0];
-            q += src[1];
-          }
-          const int oy = p.up ? 2 * (y0 + rr) + py : (y0 + rr);
-          // slot: one per (output row, 128 consecutive stored pixels of one phase)
-          const int slot = p.up ? ((oy * p.tiles_x + it.tx) * 2 + px) : (oy * p.tiles_x + it.tx);
-          const int gidx = (it.nt * CF_BN + hf * 64 + ch * 32) / cpg_out + g;
-          float* dst = p.out_partial + ((static_cast<long long>(it.b) * slots + slot) * p.out_G + gidx) * 2;
-          dst[0] = s;
-          dst[1] = q;
-        }
+        float* dst = st_my + ((r2 * 2 + ch) * 8) * 2;
+        if (cpg_out == 4)
+          cf_chunk_stats<4>(v, dst, lane);
+        else if (cpg_out == 8)
+          cf_chunk_stats<8>(v, dst, lane);
+        else
+          cf_chunk_stats<16>(v, dst, lane);
       }
     }
   }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 14) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
+  if (p.out_partial != nullptr) {
+    // fold the four pixel quarters in fixed order (deterministic) and publish one (sum, sumsq) per 128-pixel row
+    // segment and group
+    named_bar_sync(1, 256);
+    const int ng = 32 / cpg_out;
+    const int per_row = 2 * 2 * ng;         // halves x chunks x groups of this tile, per output row
+    if (tid < CF_R * per_row) {
+      const int r2 = tid / per_row;
+      const int rem = tid - r2 * per_row;
+      const int hf = rem / (2 * ng);
+      const int ch = (rem / ng) & 1;
+      const int g = rem % ng;
+      float s = 0.f, q = 0.f;
+#pragma unroll
+      for (int qd = 0; qd < 4; ++qd) {
+        const float* src = sstat + ((hf * 4 + qd) * CF_R) * (2 * 8 * 2) + ((r2 * 2 + ch) * 8 + g) * 2;
+        s += src[0];
+        q += src[1];
+      }
+      const int oy = p.up ? 2 * (y0 + r2) + py : (y0 + r2);
+      // slot: one per (output row, 128 consecutive stored pixels of one phase)
+      const int slot = p.up ? ((oy * p.tiles_x + it.tx) * 2 + px) : (oy * p.tiles_x + it.tx);
+      const int gidx = (it.nt * CF_BN + hf * 64 + ch * 32) / cpg_out + g;
+      float* dst = p.out_partial + ((static_cast<long long>(it.b) * slots + slot) * p.out_G + gidx) * 2;
+      dst[0] = s;
+      dst[1] = q;
+    }
   }
 }
 
@@ -632,7 +551,7 @@ extern "C" int dk_conv3x3_fused(dk_ctx* ctx, int dtype, const void* x, const voi
   p.Cout = Cout;
   p.up = up ? 1 : 0;
   p.tiles_x = W / CF_TW;
-  p.tiles_y = H / (2 * CF_R);
+  p.tiles_y = H / CF_R;
   p.n_tiles = (Cout + CF_BN - 1) / CF_BN;
   p.bias = bias;
   p.res = res;
@@ -644,8 +563,6 @@ extern "C" int dk_conv3x3_fused(dk_ctx* ctx, int dtype, const void* x, const voi
   p.silu = silu;
   p.out_partial = out_partial;
   p.out_G = out_G;
-  static const int dbg = [] { const char* v = getenv("DK_CF_DEBUG"); return v ? atoi(v) : 0; }();
-  p.debug = dbg;
 
   CUtensorMap tmX, tmW;
   {
@@ -660,12 +577,11 @@ extern "C" int dk_conv3x3_fused(dk_ctx* ctx, int dtype, const void* x, const voi
     const int taps = up ? 4 : 9;
     const uint64_t dims[2] = {static_cast<uint64_t>(taps) * Cin, static_cast<uint64_t>(up ? 4 : 1) * Cout};
     const uint64_t strides[1] = {static_cast<uint64_t>(taps) * Cin * 2};
-    const uint32_t box[2] = {64, CF_BN / 2};
+    const uint32_t box[2] = {64, CF_BN};
     if (int rc = dk_make_tmap_16b(ctx, &tmW, w, 2, dims, strides, box)) return rc;
   }
   const long long items = static_cast<long long>(B) * p.tiles_y * p.tiles_x * (up ? 4 : 1) * p.n_tiles;
-  const int max_pairs = ctx->sm_count / 2;
-  const int pairs = items < max_pairs ? static_cast<int>(items) : max_pairs;
+  DK_REQUIRE(items < (1LL << 31), "dk_conv3x3_fused: problem too large");
   if (dtype == DK_BF16) {
     auto kern = conv_fused_kernel<__nv_bfloat16>;
     static bool configured = false;
@@ -673,7 +589,7 @@ extern "C" int dk_conv3x3_fused(dk_ctx* ctx, int dtype, const void* x, const voi
       DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CF_SMEM_BYTES));
       configured = true;
     }
-    kern<<<2 * pairs, CF_THREADS, CF_SMEM_BYTES, stream>>>(tmX, tmW, p);
+    kern<<<static_cast<int>(items), CF_THREADS, CF_SMEM_BYTES, stream>>>(tmX, tmW, p);
   } else {
     auto kern = conv_fused_kernel<__half>;
     static bool configured = false;
@@ -681,7 +597,7 @@ extern "C" int dk_conv3x3_fused(dk_ctx* ctx, int dtype, const void* x, const voi
       DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CF_SMEM_BYTES));
       configured = true;
     }
-    kern<<<2 * pairs, CF_THREADS, CF_SMEM_BYTES, stream>>>(tmX, tmW, p);
+    kern<<<static_cast<int>(items), CF_THREADS, CF_SMEM_BYTES, stream>>>(tmX, tmW, p);
   }
   DK_LAUNCH_CHECK(ctx);
   return 0;

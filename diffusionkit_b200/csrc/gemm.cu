@@ -1,20 +1,19 @@
-// K1 / K7 — persistent warp-specialised tcgen05 GEMM for sm_100a, and its implicit-GEMM 3x3 convolution variant.
+// K1 / K7 — warp-specialised wgmma GEMM for sm_90a, and its implicit-GEMM 3x3 convolution variant.
 //
 //   out = epilogue( A[M,K] * W[N,K]^T )        (nn.Linear — reference mlx/mmdit.py:471-473,532,830-835, ...)
 //   out = epilogue( conv3x3(x NHWC, w OHWI) )  (nn.Conv2d — reference mlx/vae.py:73-81,134-136,349-351,384)
 //
-// Structure (one CTA per SM, 256 threads):
-//   warp 10: TMA producer     — streams 128x64 A tiles and BNx64 W tiles (128B swizzle) through a STAGES-deep
-//                               mbarrier ring.  For the convolution the A tile of tap (dy,dx) is a shifted 4-D
-//                               TMA box of the NHWC input; out-of-bounds elements are zero-filled by the TMA
-//                               unit, which *is* the zero padding — no im2col buffer exists anywhere.
-//   warp 11: MMA issuer       — one thread issues tcgen05.mma (M=128, N=BN, K=16) into a TMEM accumulator;
-//                               tcgen05.commit releases smem stages / publishes the accumulator.
-//   warp 8 : TMEM allocator   — 2*BN columns: two accumulators, so tile i+1's mainloop overlaps tile i's epilogue.
-//   warps 0-7 : epilogue      — tcgen05.ld (lane = row; two warps per TMEM lane quarter, each owning half of the
-//                               tile's columns), fused bias / GELU-erf / adaLN gate / residual, or QK-RMSNorm + RoPE
-//                               on the q/k thirds of a packed QKV projection; 128-bit stores straight to the
-//                               destination row (row remap = joint-sequence scatter).
+// Structure (one 128 x BN output tile per CTA, 384 threads):
+//   warpgroup 0 (warp 0): TMA producer — streams 128x64 A tiles and BNx64 W tiles (128B swizzle) through a
+//                         STAGES-deep mbarrier ring.  For the convolution the A tile of tap (dy,dx) is a shifted 4-D
+//                         TMA box of the NHWC input; out-of-bounds elements are zero-filled by the TMA unit, which
+//                         *is* the zero padding — no im2col buffer exists anywhere.
+//   warpgroups 1, 2     : MMA consumers — each owns 64 rows of the tile: wgmma m64nBNk16 from shared memory into
+//                         register accumulators, one k-block group in flight while the next is issued.
+//   epilogue            : the accumulators go through an fp32 staging tile in the (then idle) pipeline buffers, so
+//                         that each thread owns one tile row: fused bias / GELU-erf / adaLN gate / residual, or
+//                         QK-RMSNorm + RoPE on the q/k thirds of a packed QKV projection; 128-bit stores straight to
+//                         the destination row (row remap = joint-sequence scatter).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -25,29 +24,26 @@ namespace dk {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int UMMA_K = 16;
-// warps 0-7: epilogue (2 per TMEM lane quarter); 8: TMEM allocator; 10: TMA producer; 11: MMA issuer — the schedulers
-// favour the highest warp id of their quarter, so the issuer and the producer sit above the epilogue warps
 constexpr int GEMM_THREADS = 384;
-constexpr int GEMM_W_ALLOC = 8, GEMM_W_TMA = 10, GEMM_W_MMA = 11;
 
 template <int BN>
 struct GemmCfg {
   static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int PIPE_BYTES = STAGES * (A_BYTES + B_BYTES);
+  static constexpr int STAGE_LD = BN + 4;   // fp32 staging row stride (floats): +4 spreads the rows over the banks
+  static_assert(PIPE_BYTES >= BM * STAGE_LD * 4, "the epilogue staging tile reuses the pipeline buffers");
   static constexpr int BAR_BYTES = 256;
-  static constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + BAR_BYTES + 1024;  // +1024: manual alignment slack
-  static constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
+  static constexpr int SMEM_BYTES = PIPE_BYTES + BAR_BYTES + 1024;  // +1024: manual alignment slack
 };
 
 // MODE 0: plain GEMM.  MODE 1: conv3x3 implicit GEMM (A via 4-D TMA boxes).
-// B_MN: W operand given as [K, N] row-major (MN-major UMMA operand) — validates the descriptor form attention uses for V.
+// B_MN: W operand given as [K, N] row-major (MN-major wgmma operand, transposed B).
 template <typename T, int BN, bool B_MN, int MODE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape s,
-               const GemmEpi e, const ConvGeom g) {
-  using H16 = Half16<T>;
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape s,
+                  const GemmEpi e, const ConvGeom g) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   constexpr int A_BYTES = Cfg::A_BYTES;
@@ -58,44 +54,30 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::PIPE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int total_tiles = s.num_m * s.num_n;
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == GEMM_W_TMA && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == GEMM_W_MMA && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 8);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == GEMM_W_ALLOC) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // Grouped rasterisation: consecutive tile ids walk GM m-blocks for one n-block, so the ~148 tiles in flight
+  // Grouped rasterisation: consecutive tile ids walk GM m-blocks for one n-block, so the CTAs resident at a time
   // share a band of A rows and a handful of W column blocks (L2 reuse).
   constexpr int GM = 16;
-  auto decode_tile = [&](int tile, int& m_blk, int& n_blk) {
+  int m_blk, n_blk;
+  {
+    const int tile = blockIdx.x;
     const int group_size = GM * s.num_n;
     const int group = tile / group_size;
     const int first_m = group * GM;
@@ -103,145 +85,133 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int in_group = tile - group * group_size;
     m_blk = first_m + in_group % gsz;
     n_blk = in_group / gsz;
-  };
+  }
 
-  if (warp == GEMM_W_TMA) {
+  if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer, converged warp
+    if (warp != 0) return;
+    int img = 0, y0 = 0, x0 = 0;
+    if (MODE == 1) {
+      const int per_img = g.tiles_x * g.tiles_y;
+      img = m_blk / per_img;
+      const int t = m_blk - img * per_img;
+      y0 = (t / g.tiles_x) * g.TH;
+      x0 = (t % g.tiles_x) * g.TW;
+    }
     uint32_t stage = 0, phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      int m_blk, n_blk;
-      decode_tile(tile, m_blk, n_blk);
-      int img = 0, y0 = 0, x0 = 0;
-      if (MODE == 1) {
-        const int per_img = g.tiles_x * g.tiles_y;
-        img = m_blk / per_img;
-        const int t = m_blk - img * per_img;
-        y0 = (t / g.tiles_x) * g.TH;
-        x0 = (t % g.tiles_x) * g.TW;
-      }
-      for (int kb = 0; kb < s.num_k; ++kb) {
-        mbar_wait_warp(&empty_bar[stage], phase ^ 1);
-        if (elect_one_sync()) {
-          mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
-          uint8_t* a_dst = sA + stage * A_BYTES;
-          uint8_t* b_dst = sB + stage * B_BYTES;
-          if (MODE == 0) {
-            tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
-          } else {
-            const int tap = kb / g.cblocks;
-            const int c0 = (kb - tap * g.cblocks) * BK;
-            const int dy = tap / 3, dx = tap - dy * 3;
-            tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, x0 * g.stride + dx - g.pad, y0 * g.stride + dy - g.pad, img);
-          }
-          if (!B_MN) {
-            tma_load_2d(b_dst, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
-          } else {
+    for (int kb = 0; kb < s.num_k; ++kb) {
+      mbar_wait_warp(&empty_bar[stage], phase ^ 1);
+      if (elect_one_sync()) {
+        mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
+        uint8_t* a_dst = sA + stage * A_BYTES;
+        uint8_t* b_dst = sB + stage * B_BYTES;
+        if (MODE == 0) {
+          tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
+        } else {
+          const int tap = kb / g.cblocks;
+          const int c0 = (kb - tap * g.cblocks) * BK;
+          const int dy = tap / 3, dx = tap - dy * 3;
+          tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, x0 * g.stride + dx - g.pad, y0 * g.stride + dy - g.pad, img);
+        }
+        if (!B_MN) {
+          tma_load_2d(b_dst, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
+        } else {
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
-              tma_load_2d(b_dst + j * (BK * 128), &tmB, &full_bar[stage], n_blk * BN + j * 64, kb * BK);
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
+          for (int j = 0; j < BN / 64; ++j)
+            tma_load_2d(b_dst + j * (BK * 128), &tmB, &full_bar[stage], n_blk * BN + j * 64, kb * BK);
         }
       }
-    }
-  } else if (warp == GEMM_W_MMA) {
-    // -------------------------------------------------------------------- MMA issuer, converged warp
-    constexpr uint32_t idesc = make_idesc_f16(BM, BN, H16::is_bf16, false, B_MN);
-    const uint32_t desc_hi = smem_desc_hi_sw128(1024);
-    const uint32_t a_lo0 = smem_desc_lo(smem_u32(sA), 0);
-    const uint32_t b_lo0 = smem_desc_lo(smem_u32(sB), B_MN ? BK * 128 : 0);
-    uint32_t stage = 0, phase = 0;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const uint32_t acc = it & 1u;
-      const uint32_t acc_phase = (it >> 1) & 1u;
-      mbar_wait_warp(&tempty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < s.num_k; ++kb) {
-        mbar_wait_warp(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one_sync()) {
-          const uint32_t a_lo = a_lo0 + stage * (A_BYTES >> 4);
-          const uint32_t b_lo = b_lo0 + stage * (B_BYTES >> 4);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k)
-            umma_ss(d_tmem, smem_desc_join(a_lo + k * ((UMMA_K * 2) >> 4), desc_hi),
-                    smem_desc_join(b_lo + k * ((B_MN ? UMMA_K * 128 : UMMA_K * 2) >> 4), desc_hi), idesc,
-                    (kb | k) != 0 ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);                        // smem stage reusable once these MMAs retire
-          if (kb == s.num_k - 1) umma_commit(&tfull_bar[acc]);   // accumulator complete
-        }
-        __syncwarp();
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
+      __syncwarp();
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
       }
     }
-  } else if (warp < 8) {
-    // ------------------------------------------------------------------ epilogue (256 threads, lane = tile row)
-    const int quarter = warp & 3;          // TMEM lanes 32*quarter .. 32*quarter+31 are accessible to this warp
-    const int half = warp >> 2;            // which half of the tile's columns this warp drains
-    constexpr int NCH = BN / 64;           // 32-column chunks per warp
-    const int r_in_tile = quarter * 32 + lane;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      int m_blk, n_blk;
-      decode_tile(tile, m_blk, n_blk);
-      const uint32_t acc = it & 1u;
-      const uint32_t acc_phase = (it >> 1) & 1u;
-
-      // destination rows
-      bool row_ok;
-      long long orow, rrow;
-      int batch, pos = 0;
-      if (MODE == 0) {
-        const int m = m_blk * BM + r_in_tile;
-        row_ok = m < s.M;
-        batch = m / e.rpb;
-        const int in_b = m - batch * e.rpb;
-        pos = e.out_row_off + in_b;  // position in the joint sequence (RoPE)
-        orow = static_cast<long long>(batch) * e.out_batch_rows + e.out_row_off + in_b;
-        rrow = static_cast<long long>(batch) * e.res_batch_rows + e.res_row_off + in_b;
-      } else {
-        const int per_img = g.tiles_x * g.tiles_y;
-        const int img = m_blk / per_img;
-        const int t = m_blk - img * per_img;
-        const int y = (t / g.tiles_x) * g.TH + r_in_tile / g.TW;
-        const int x = (t % g.tiles_x) * g.TW + r_in_tile % g.TW;
-        row_ok = (y < g.H) && (x < g.W);
-        batch = img;
-        orow = (static_cast<long long>(img) * g.H + y) * g.W + x;
-        rrow = orow;
-      }
-
-      mbar_wait_warp(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + half * (BN / 2);
-      const int n_half0 = n_blk * BN + half * (BN / 2);
-
-      auto release_acc = [&]() {
-        // accumulator columns of this warp fully drained into registers: hand the TMEM buffer back to the MMA warp
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      };
-
-      gemm_epilogue_drain<T, NCH, MODE>(s, e, t_row, n_half0, row_ok, orow, rrow, batch, pos, release_acc);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == GEMM_W_ALLOC) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  // -------------------------------------------------------------------- MMA consumers: rows 64*cw .. 64*cw+63
+  const int cw = wg - 1;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  {
+    uint32_t stage = 0, phase = 0, prev = 0;
+    for (int kb = 0; kb < s.num_k; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_base = smem_u32(sA + stage * A_BYTES) + cw * 64 * 128;
+      const uint32_t b_base = smem_u32(sB + stage * B_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t da = make_smem_desc_sw128(a_base + k * 32, 16, 1024);
+        const uint64_t db = B_MN ? make_smem_desc_sw128(b_base + k * 16 * 128, BK * 128, 1024)
+                                 : make_smem_desc_sw128(b_base + k * 32, 16, 1024);
+        Wgmma<BN, Half16<T>::is_bf16, B_MN ? 1 : 0>::ss(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      // the previous k-block's MMAs have retired: its stage can be refilled
+      wgmma_wait<1>();
+      if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
   }
+
+  // ------------------------------------------------------------------ epilogue (256 threads, thread = tile row)
+  // every TMA load has landed and every MMA has retired once both warpgroups pass this barrier: the pipeline buffers
+  // become the fp32 staging tile
+  float* stg = reinterpret_cast<float*>(smem);
+  named_bar_sync(1, 256);
+  stage_acc_rows<BN>(stg, Cfg::STAGE_LD, cw * 64, acc);
+  named_bar_sync(1, 256);
+
+  const int ew = warp - 4;               // 0..7
+  const int quarter = ew & 3;            // rows 32*quarter .. 32*quarter+31
+  const int half = ew >> 2;              // which half of the tile's columns this warp drains
+  constexpr int NCH = BN / 64;           // 32-column chunks per thread
+  const int r_in_tile = quarter * 32 + lane;
+
+  // destination rows
+  bool row_ok;
+  long long orow, rrow;
+  int batch, pos = 0;
+  if (MODE == 0) {
+    const int m = m_blk * BM + r_in_tile;
+    row_ok = m < s.M;
+    batch = m / e.rpb;
+    const int in_b = m - batch * e.rpb;
+    pos = e.out_row_off + in_b;  // position in the joint sequence (RoPE)
+    orow = static_cast<long long>(batch) * e.out_batch_rows + e.out_row_off + in_b;
+    rrow = static_cast<long long>(batch) * e.res_batch_rows + e.res_row_off + in_b;
+  } else {
+    const int per_img = g.tiles_x * g.tiles_y;
+    const int img = m_blk / per_img;
+    const int t = m_blk - img * per_img;
+    const int y = (t / g.tiles_x) * g.TH + r_in_tile / g.TW;
+    const int x = (t % g.tiles_x) * g.TW + r_in_tile % g.TW;
+    row_ok = (y < g.H) && (x < g.W);
+    batch = img;
+    orow = (static_cast<long long>(img) * g.H + y) * g.W + x;
+    rrow = orow;
+  }
+  const float* srow = stg + r_in_tile * Cfg::STAGE_LD + half * (BN / 2);
+  auto load32 = [&](int c, uint32_t (&r)[32]) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const float4 v = *reinterpret_cast<const float4*>(srow + c + 4 * q);
+      r[4 * q] = __float_as_uint(v.x);
+      r[4 * q + 1] = __float_as_uint(v.y);
+      r[4 * q + 2] = __float_as_uint(v.z);
+      r[4 * q + 3] = __float_as_uint(v.w);
+    }
+  };
+  gemm_epilogue_drain<T, NCH, MODE>(s, e, load32, n_blk * BN + half * (BN / 2), row_ok, orow, rrow, batch, pos);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -251,15 +221,13 @@ template <typename T, int BN, bool B_MN, int MODE>
 static int launch_gemm_inst(dk_ctx* ctx, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s,
                             const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_tc_kernel<T, BN, B_MN, MODE>;
+  auto kern = gemm_wgmma_kernel<T, BN, B_MN, MODE>;
   static bool configured = false;
   if (!configured) {
     DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     configured = true;
   }
-  const int total = s.num_m * s.num_n;
-  const int grid = total < ctx->sm_count ? total : ctx->sm_count;
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, s, e, g);
+  kern<<<s.num_m * s.num_n, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, s, e, g);
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
@@ -272,8 +240,8 @@ static int launch_gemm_bn(dk_ctx* ctx, int bn, const CUtensorMap& tmA, const CUt
   return launch_gemm_inst<T, 64, B_MN, MODE>(ctx, tmA, tmB, s, e, g, stream);
 }
 
-// Tile-N choice: 256 wide tiles keep the smem operand traffic per MMA lowest (96 B/clk); fall back to narrower tiles
-// when N is small or when 256-wide tiles would leave most of the 148 SMs idle.
+// Tile-N choice: 256 wide tiles keep the shared-memory operand traffic per MMA lowest; fall back to narrower tiles
+// when N is small or when 256-wide tiles would leave most of the SMs idle.
 static int pick_bn(const dk_ctx* ctx, int num_m, int N) {
   if (N <= 64) return 64;
   if (N <= 128) return 128;
@@ -289,18 +257,6 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 }  // namespace dk
 
 using namespace dk;
-
-int dk_launch_gemm_pair(dk_ctx* ctx, int dtype, const void* A, long long lda, const void* W, long long ldw, int M, int N,
-                        int K, const dk::GemmEpi& e, cudaStream_t stream);
-
-// 0: never, 1: heuristic (default), 2: whenever legal.  DK_GEMM_PAIR overrides (A/B measurements, tests).
-static int gemm_pair_mode() {
-  static const int mode = [] {
-    const char* v = getenv("DK_GEMM_PAIR");
-    return v ? atoi(v) : 1;
-  }();
-  return mode;
-}
 
 extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
   DK_REQUIRE(ctx != nullptr && a != nullptr, "dk_gemm: null argument");
@@ -356,14 +312,6 @@ extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
     DK_REQUIRE(a->qk_rope == nullptr || (reinterpret_cast<uintptr_t>(a->qk_rope) & 15u) == 0, "dk_gemm: rope table alignment");
   }
   ConvGeom g = {};
-
-  // CTA-pair kernel (256x256 tiles, cta_group::2) when the tiles fill the machine
-  if (!a->w_n_major && gemm_pair_mode() != 0) {
-    const long long tiles = static_cast<long long>(dk_ceil_div(a->M, 256)) * dk_ceil_div(a->N, 256);
-    const bool big = tiles >= ctx->sm_count / 2 && a->N >= 256 && a->M >= 256;
-    if (gemm_pair_mode() == 2 || big)
-      return dk_launch_gemm_pair(ctx, a->dtype, a->A, a->lda, a->W, a->ldw, a->M, a->N, a->K, e, stream);
-  }
 
   CUtensorMap tmA, tmB;
   {

@@ -1,4 +1,4 @@
-// Shared pieces of the tcgen05 GEMM kernels: problem/epilogue descriptors and the TMEM -> registers -> global
+// Shared pieces of the wgmma GEMM kernel: problem/epilogue descriptors and the accumulator -> global
 // epilogue (bias / GELU-erf / SiLU / adaLN gate / residual, or QK-RMSNorm + RoPE on a packed QKV projection).
 #pragma once
 
@@ -10,7 +10,6 @@ namespace dk {
 struct GemmShape {
   int M, N, K;
   int num_m, num_n, num_k;
-  int gm;   // pair kernel: m-tiles per rasterisation band (0 = default)
 };
 
 struct GemmEpi {
@@ -25,7 +24,7 @@ struct GemmEpi {
   int out_batch_rows, out_row_off;
   int res_batch_rows, res_row_off;
   int act;
-  int debug;  // timing experiments only (DK_GEMM_EPI_DEBUG): 1 = skip the global stores, 2 = skip everything after TMEM->regs
+  int debug;  // timing experiments only (DK_GEMM_EPI_DEBUG): 1 = skip the global stores, 2 = skip everything after the accumulator read
   // fused QK-RMSNorm + RoPE on the q and k thirds of a packed QKV projection (columns [0, 2*qk_h)); qk_d == 0 disables
   const void* qk_qw;   // [d] RMSNorm weight of q (or NULL: no norm)
   const void* qk_kw;   // [d]
@@ -44,34 +43,24 @@ struct ConvGeom {
 };
 
 
-// 16 finished 16-bit values of one row -> global.  One 256-bit store (a full 32-byte sector per thread) when the
-// address allows it: with 128-bit stores every sector is written by two separate requests and the store path cost the
-// pair GEMM 6 % of its sustained (power-capped) throughput.
-__device__ __forceinline__ void store_row16(void* dst, const uint32_t (&w)[8], bool wide) {
-  if (wide) {
-    asm volatile("st.global.cs.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst), "r"(w[0]), "r"(w[1]),
-                 "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-                 : "memory");
-  } else {
-    __stcs(reinterpret_cast<uint4*>(dst), make_uint4(w[0], w[1], w[2], w[3]));
-    __stcs(reinterpret_cast<uint4*>(dst) + 1, make_uint4(w[4], w[5], w[6], w[7]));
-  }
+// 16 finished 16-bit values of one row -> global (two 128-bit streaming stores).
+__device__ __forceinline__ void store_row16(void* dst, const uint32_t (&w)[8]) {
+  __stcs(reinterpret_cast<uint4*>(dst), make_uint4(w[0], w[1], w[2], w[3]));
+  __stcs(reinterpret_cast<uint4*>(dst) + 1, make_uint4(w[4], w[5], w[6], w[7]));
 }
 
-// Drains NCH 32-column chunks of one accumulator row (this thread = one tile row; t_row = TMEM address of the row's
-// first column owned by this warp) and stores the finished 16-bit values.  `release()` is called exactly once, right
-// after the last TMEM read, so the accumulator can be handed back to the MMA warp before the stores retire.
-template <typename T, int NCH, int MODE, typename Release>
-__device__ __forceinline__ void gemm_epilogue_drain(const GemmShape& s, const GemmEpi& e, uint32_t t_row, int n_half0,
-                                                    bool row_ok, long long orow, long long rrow, int batch, int pos,
-                                                    Release release_acc) {
+// Drains NCH 32-column chunks of one accumulator row (this thread = one tile row; load32(c, r) fills r with the fp32
+// bits of the 32 columns starting c columns after the thread's first column) and stores the finished 16-bit values.
+template <typename T, int NCH, int MODE, typename Load>
+__device__ __forceinline__ void gemm_epilogue_drain(const GemmShape& s, const GemmEpi& e, Load load32, int n_half0,
+                                                    bool row_ok, long long orow, long long rrow, int batch, int pos) {
   using H16 = Half16<T>;
   const T* bias = reinterpret_cast<const T*>(e.bias);
   const T* gate = reinterpret_cast<const T*>(e.gate);
   const T* res = reinterpret_cast<const T*>(e.res);
   T* out = reinterpret_cast<T*>(e.out);
   if (MODE == 0 && e.qk_d != 0 && n_half0 < 2 * e.qk_h) {
-  // ---- q / k columns of a packed QKV projection: RMSNorm over each head (two passes over TMEM), then RoPE.
+  // ---- q / k columns of a packed QKV projection: RMSNorm over each head (two passes over the staged row), then RoPE.
   //      reference: q = Linear(m) (16-bit) -> nn.RMSNorm (fp32 accumulate, 16-bit out) -> RoPE in fp32
   //      (mlx/mmdit.py:471-488, 754-764, 934-942)
   const int d = e.qk_d;
@@ -84,8 +73,7 @@ __device__ __forceinline__ void gemm_epilogue_drain(const GemmShape& s, const Ge
 #pragma unroll 1
       for (int c = 0; c < cph; ++c) {
         uint32_t r[32];
-        tmem_ld_32x32(t_row + (hc + c) * 32, r);
-        tmem_ld_wait();
+        load32((hc + c) * 32, r);
         const int n0 = n_half0 + (hc + c) * 32;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -115,9 +103,7 @@ __device__ __forceinline__ void gemm_epilogue_drain(const GemmShape& s, const Ge
 #pragma unroll 1
     for (int c = 0; c < cph; ++c) {
       uint32_t r[32];
-      tmem_ld_32x32(t_row + (hc + c) * 32, r);
-      tmem_ld_wait();
-      if (hc + c == NCH - 1) release_acc();
+      load32((hc + c) * 32, r);
       if (!row_ok || e.debug >= 2) continue;
       const int n0 = n_half0 + (hc + c) * 32;
       const int dcol0 = head_col0 + c * 32;  // column inside the head
@@ -165,7 +151,7 @@ __device__ __forceinline__ void gemm_epilogue_drain(const GemmShape& s, const Ge
         for (int i = 0; i < 4; ++i) w16[(j & 1) * 4 + i] = H16::pack(v[2 * i], v[2 * i + 1]);
         if ((j & 1) && e.debug == 0) {
           T* dst = out + orow * e.ldc + (n - 8);
-          store_row16(dst, w16, (reinterpret_cast<uintptr_t>(dst) & 31u) == 0);
+          store_row16(dst, w16);
         }
       }
     }
@@ -176,9 +162,7 @@ __device__ __forceinline__ void gemm_epilogue_drain(const GemmShape& s, const Ge
 #pragma unroll 1
 for (int chunk = 0; chunk < NCH; ++chunk) {
   uint32_t r[32];
-  tmem_ld_32x32(t_row + chunk * 32, r);
-  tmem_ld_wait();
-  if (chunk == NCH - 1) release_acc();
+  load32(chunk * 32, r);
   const int n0 = n_half0 + chunk * 32;
   if (!row_ok || e.debug >= 2) continue;
 #pragma unroll
@@ -241,114 +225,12 @@ for (int chunk = 0; chunk < NCH; ++chunk) {
     if (e.debug != 0) continue;
     T* dst = out + orow * e.ldc + nb;
     if (nb + 16 <= s.N) {
-      store_row16(dst, w, (reinterpret_cast<uintptr_t>(dst) & 31u) == 0);
+      store_row16(dst, w);
     } else {
       __stcs(reinterpret_cast<uint4*>(dst), make_uint4(w[0], w[1], w[2], w[3]));   // 8-column tail
     }
   }
 }
-}
-
-// Same arithmetic as the generic path of gemm_epilogue_drain, but the finished 16-bit tile leaves through shared
-// memory and TMA: each warp packs 32 rows x 64 columns into its own 4 KB staging buffer (128B-swizzled rows, so the
-// 16-byte st.shared of the 32 lanes are conflict free) and one lane issues a single bulk tensor store for it — whole
-// 128-byte lines per request instead of one 32-byte sector per thread.  Only for identity-mapped outputs (row m of the
-// tile grid is row m of `out`); rows/columns beyond M/N are clipped by the tensor map.
-//   stg: this warp's staging buffer (shared::cta address, 1024-byte aligned);  out_row0: output row of lane 0
-//   NCH: 32-column chunks owned by this warp (even).
-template <typename T, int NCH, typename Release>
-__device__ __forceinline__ void gemm_epilogue_drain_tma(const GemmShape& s, const GemmEpi& e, uint32_t t_row, int n_half0,
-                                                        bool row_ok, long long rrow, int batch, uint32_t stg,
-                                                        const CUtensorMap* tm_out, int out_row0, bool evict_first,
-                                                        Release release_acc) {
-  using H16 = Half16<T>;
-  static_assert(NCH % 2 == 0, "TMA-store epilogue works on 64-column chunks");
-  // the output is consumed by a later kernel, the operand tiles by this one: without the hint the 400 MB of C lines
-  // of a large GEMM push A/W out of L2 (ncu: hit rate 91 % -> 83 %, DRAM reads 459 -> 738 MB per launch)
-  const uint64_t policy = l2_policy_evict_first();
-  const T* bias = reinterpret_cast<const T*>(e.bias);
-  const T* gate = reinterpret_cast<const T*>(e.gate);
-  const T* res = reinterpret_cast<const T*>(e.res);
-  const int lane = threadIdx.x & 31;
-  const uint32_t my_row = stg + lane * 128;
-#pragma unroll 1
-  for (int c64 = 0; c64 < NCH / 2; ++c64) {
-    const int n64 = n_half0 + c64 * 64;
-    // the previous store out of this buffer must have finished reading it
-    if (lane == 0) tma_store_wait_read();
-    __syncwarp();
-#pragma unroll
-    for (int hlf = 0; hlf < 2; ++hlf) {
-      uint32_t r[32];
-      tmem_ld_32x32(t_row + c64 * 64 + hlf * 32, r);
-      tmem_ld_wait();
-      if (c64 == NCH / 2 - 1 && hlf == 1) release_acc();
-      const int n0 = n64 + hlf * 32;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int n = n0 + j * 8;
-        float v[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[j * 8 + i]);
-        if (row_ok && n < s.N && e.debug < 2) {
-          if (bias != nullptr) {
-            const uint4 b4 = *reinterpret_cast<const uint4*>(bias + n);
-            const uint32_t bw[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 f = H16::unpack(bw[i]);
-              v[2 * i] += f.x;
-              v[2 * i + 1] += f.y;
-            }
-          }
-          if (e.act == DK_ACT_GELU_ERF) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = gelu_erf(v[i]);
-          } else if (e.act == DK_ACT_SILU) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = silu_f(v[i]);
-          } else if (e.act == DK_ACT_QUICK_GELU) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = quick_gelu_f(v[i]);
-          }
-          if (gate != nullptr) {
-            const uint4 g4 = *reinterpret_cast<const uint4*>(gate + static_cast<long long>(batch) * e.gate_ld + n);
-            const uint32_t gw[4] = {g4.x, g4.y, g4.z, g4.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 f = H16::unpack(gw[i]);
-              v[2 * i] *= f.x;
-              v[2 * i + 1] *= f.y;
-            }
-          }
-          if (res != nullptr) {
-            const uint4 r4 = *reinterpret_cast<const uint4*>(res + rrow * e.ldres + n);
-            const uint32_t rw[4] = {r4.x, r4.y, r4.z, r4.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 f = H16::unpack(rw[i]);
-              v[2 * i] += f.x;
-              v[2 * i + 1] += f.y;
-            }
-          }
-        }
-        const int ch = hlf * 4 + j;   // 16-byte chunk inside the 128-byte row
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(my_row + ((ch ^ (lane & 7)) << 4)),
-                     "r"(H16::pack(v[0], v[1])), "r"(H16::pack(v[2], v[3])), "r"(H16::pack(v[4], v[5])),
-                     "r"(H16::pack(v[6], v[7]))
-                     : "memory");
-      }
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0 && e.debug == 0 && n64 < s.N) {
-      if (evict_first)
-        tma_store_2d_hint(tm_out, stg, n64, out_row0, policy);
-      else
-        tma_store_2d(tm_out, stg, n64, out_row0);
-      tma_store_commit();
-    }
-  }
 }
 
 }  // namespace dk

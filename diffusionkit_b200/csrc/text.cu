@@ -1,5 +1,5 @@
 // Kernels of the text-encoder path (SURVEY.md §8 row f2): CLIP-L/G and the T5-XXL encoder.  The projections and MLPs
-// run on the tcgen05 GEMM (gemm.cu / gemm2.cu); this file holds what sits between them: embedding lookup, LayerNorm
+// run on the wgmma GEMM (gemm.cu); this file holds what sits between them: embedding lookup, LayerNorm
 // with affine, T5's RMSNorm over the fp32 residual stream, the gated-GELU product, and attention for short sequences
 // (S <= 512, head dim 64) with CLIP's causal mask or T5's relative-position bias.  All are small next to the denoise
 // path (T5-XXL at 512 tokens: 4.3 GFLOP of attention per layer against 0.6 TFLOP of GEMM).

@@ -1,11 +1,11 @@
-"""MMDiT (SD3 dual-stream / FLUX dual + single-stream) forward on B200.
+"""MMDiT (SD3 dual-stream / FLUX dual + single-stream) forward on H100.
 
 Host-side mirror of the reference module (python/src/diffusionkit/mlx/mmdit.py:22-266): same public methods
 (`cache_modulation_params`, `__call__(latent_image_embeddings, token_level_text_embeddings, timestep)`,
-`clear_modulation_params_cache`), same parameter names.  Every FLOP runs in hand-written sm_100a kernels reached
+`clear_modulation_params_cache`), same parameter names.  Every FLOP runs in hand-written sm_90a kernels reached
 through the C ABI (ops.py -> libdkb200.so); torch tensors are only the HBM containers.
 
-B200 layout decisions (vs. the reference's per-module MLX graph):
+H100 layout decisions (vs. the reference's per-module MLX graph):
   * q/k/v projections of a stream are ONE GEMM (packed [3h, h] weight; k has no bias — quirk Q3) whose epilogue applies
     the per-head QK-RMSNorm and RoPE (FLUX) and scatters rows straight into the joint [text|image] (FLUX) /
     [image|text] (SD3) sequence buffer — no norm / rope / concat kernels.

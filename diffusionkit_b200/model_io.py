@@ -301,9 +301,8 @@ def preadjusted_checkpoint_to_params(sd: Dict[str, Tensor], prefix: str = "") ->
 
 def dequantize_q4_params(sd: Dict[str, Tensor], device, dtype: torch.dtype, group_size: int = 64) -> Dict[str, Tensor]:
     """MLX QuantizedLinear triples (`X.weight` uint32 [N, K/8], `X.scales`, `X.biases` [N, K/64]) -> dense 16-bit
-    `X.weight` [N, K] on `device` (dk_dequant_q4).  On B200 the denoise GEMMs are tensor-pipe bound at M >= 1024 rows
-    and the dense FLUX weights are 13 % of HBM, so the 4-bit form is expanded once at load instead of inside every GEMM
-    (DESIGN.md §7).  Every other tensor is passed through (cast to `dtype` like the reference, :736-738)."""
+    `X.weight` [N, K] on `device` (dk_dequant_q4).  The denoise GEMMs are tensor-pipe bound at M >= 1024 rows and the dense
+    FLUX weights (23.8 GB) fit HBM, so the 4-bit form is expanded once at load instead of inside every GEMM.  Every other tensor is passed through (cast to `dtype` like the reference, :736-738)."""
     from . import ops
 
     out: Dict[str, Tensor] = {}

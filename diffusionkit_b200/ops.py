@@ -1,6 +1,6 @@
 """Typed Python wrappers over the C ABI (torch tensors are only the device-memory containers).
 
-Every function launches hand-written sm_100a kernels from libdkb200.so asynchronously on the current
+Every function launches hand-written sm_90a kernels from libdkb200.so asynchronously on the current
 torch CUDA stream.  Nothing here has a torch / CPU fallback.
 """
 from __future__ import annotations

@@ -1,5 +1,5 @@
 """DiffusionPipeline / FluxPipeline — the reference's Python surface (python/src/diffusionkit/mlx/__init__.py:64-788)
-over the B200 engine.  Same constructor arguments, method names, defaults and return structures; the denoise loop and
+over the H100 engine.  Same constructor arguments, method names, defaults and return structures; the denoise loop and
 the decode run entirely in the CUDA kernels of libdkb200.so.
 
 Differences that are deliberate (documented in DESIGN.md):
@@ -160,7 +160,7 @@ class DiffusionPipeline:
         self.mmdit_ckpt = MMDIT_CKPT[model_version]                          # KeyError on unknown model (:81)
         if not (w16 and a16):
             raise NotImplementedError(
-                "the B200 engine computes in 16-bit only: pass w16=True, a16=True (what the reference CLI forces, "
+                "the H100 engine computes in 16-bit only: pass w16=True, a16=True (what the reference CLI forces, "
                 "scripts/generate_images.py:117-118)")
         self._local_ckpt = local_ckpt
         self.dtype = self.float16_dtype
@@ -170,7 +170,7 @@ class DiffusionPipeline:
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else None
         if device is None:
-            raise DkError("no CUDA device: diffusionkit_b200 runs on B200 only; there is no CPU fallback")
+            raise DkError("no CUDA device: diffusionkit_b200 runs on H100 only; there is no CPU fallback")
         self.device = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
         self.config = mmdit_config if mmdit_config is not None else MODEL_CONFIGS[model_version]
         self._weight_seed = weight_seed

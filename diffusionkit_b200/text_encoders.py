@@ -1,7 +1,7 @@
-"""Text encoders on B200 (SURVEY.md §8 row f2) — host-side mirrors of the reference CLIPTextModel
+"""Text encoders on H100 (SURVEY.md §8 row f2) — host-side mirrors of the reference CLIPTextModel
 (python/src/diffusionkit/mlx/clip.py:27-120) and SD3T5Encoder (mlx/t5.py:198-243, 316-325).
 
-Same parameter names as the reference module trees.  Kernels: every projection / MLP on the tcgen05 GEMM (packed QKV,
+Same parameter names as the reference module trees.  Kernels: every projection / MLP on the wgmma GEMM (packed QKV,
 bias / quick-GELU / GELU / residual fused in the epilogue); embedding lookup, LayerNorm, T5 RMSNorm over the fp32
 residual stream, gated-GELU product and the short-sequence attention (causal mask or relative-position bias) in
 csrc/text.cu.

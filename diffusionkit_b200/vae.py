@@ -1,14 +1,14 @@
-"""VAE decoder and encoder on B200 — host-side mirrors of the reference VAEDecoder / VAEEncoder
+"""VAE decoder and encoder on H100 — host-side mirrors of the reference VAEDecoder / VAEEncoder
 (python/src/diffusionkit/mlx/vae.py:336-401 and :404-467; ResnetBlock2D :60-101, Attention :28-57,
 upsample_nearest :20-25, EncoderDecoderBlock2D :103-148).
 
 Same parameter names as the reference module tree (SURVEY.md App. C).  Kernels (csrc/):
-  conv 3x3        : tcgen05 implicit GEMM, the 9 taps are shifted 4-D TMA boxes (zero fill = padding), bias and the
+  conv 3x3        : wgmma implicit GEMM, the 9 taps are shifted 4-D TMA boxes (zero fill = padding), bias and the
                     ResNet skip fused in the epilogue
   GroupNorm(32)   : two-stage fp32 statistics + fused normalise/affine/SiLU
   conv 3x3 / 2    : same kernel, the TMA box walks the input with element stride 2 (zero fill = the reference's
                     bottom/right pad, vae.py:142-144)
-  mid attention   : q/k/v/out projections and both S=HW x HW matmuls on the tcgen05 GEMM (scores materialised like the
+  mid attention   : q/k/v/out projections and both S=HW x HW matmuls on the wgmma GEMM (scores materialised like the
                     reference, vae.py:49-52; V consumed as an MN-major operand), fp32 row softmax; 1/sqrt(C) is folded
                     into the query projection once at load (the reference scales q before q k^T, :49: the unscaled
                     product would reach the fp16 limit 22x earlier)
@@ -152,10 +152,8 @@ class VAEDecoder(_VAEBlocks):
         # where GroupNorm-apply + SiLU runs on the fused path: "1" (default) = inside the convolution, on the staged halo
         # tile (no normalised tensor in HBM; every halo element is transformed once per CTA that stages it: 2x for the
         # two halo rows of a 2-row tile, times Cout/128 n-tiles); "0" = one HBM pass of the apply kernel in front of the
-        # fused convolution (which still folds bias / skip / upsample / the next statistics).  Whole 1024^2 decode, same
-        # box (profiles/r02_vae_norm_mode.txt): 42.1 / 43.6 ms inside vs 41.9 / 40.3 ms separate at batch 4, 10.75 vs
-        # 10.24 ms at batch 1 — a 2-5 % difference for 33 % more launches and ~2 GB more HBM traffic per image, so
-        # the in-kernel form stays the default.
+        # fused convolution (which still folds bias / skip / upsample / the next statistics), at the price of more
+        # launches and a normalised tensor in HBM.
         self.norm_in_conv = os.environ.get("DK_VAE_NORM_IN_CONV", "1") != "0"
         self.use_cuda_graphs = os.environ.get("DK_CUDA_GRAPHS", "1") != "0"
         self._shapes: "OrderedDict[tuple, tuple]" = OrderedDict()     # input shape -> (graph, static in, static out, launches)

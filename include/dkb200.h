@@ -1,4 +1,4 @@
-/* dkb200 — C ABI of the B200-native denoise + decode engine behind DiffusionKit's
+/* dkb200 — C ABI of the H100-native denoise + decode engine behind DiffusionKit's
  * `diffusionkit.mlx` DiffusionPipeline / FluxPipeline API.
  *
  * The reference (argmaxinc/DiffusionKit @ 498e5dba) has no FFI boundary: its hot path sits behind a
@@ -61,7 +61,7 @@ void dk_ctx_destroy(dk_ctx* ctx);
 long long dk_ctx_launch_count(dk_ctx* ctx);
 
 /* ---------------------------------------------------------------------------------------------
- * K1  tcgen05 GEMM with fused epilogue — replaces every nn.Linear on the path
+ * K1  wgmma GEMM with fused epilogue — replaces every nn.Linear on the path
  *     (mmdit.py:471-473 q/k/v, :532 o_proj, :830-835 FFN, :430-435 adaLN, :56-59 context_embedder,
  *      :357-361/:372-376 embedders, :771-774 final linear; vae.py:36-39 attention projections).
  *     out[row(m), n] = res[rrow(m), n] + gate[m / rows_per_batch, n] * act(sum_k A[m,k] W[n,k] + bias[n])
@@ -130,12 +130,6 @@ int dk_qk_norm_rope(dk_ctx* ctx, int dtype, void* qkv, int rows, int S, int head
  * ------------------------------------------------------------------------------------------- */
 int dk_attention_fwd(dk_ctx* ctx, int dtype, const void* qkv, int B, int S, int heads, int d, float scale, int split,
                      void* out0, long long ld0, void* out1, long long ld1, void* stream);
-/* Tuning hook for same-process A/B measurements of the K3 variants (no reference counterpart): split P publication
- * (0/1), exponentials per four evaluated on the FMA pipe (0..2), streamed exponential pass (0/1; 2 / 3 select the 64-key
- * double-buffered kernel of attention_v6.cu with two threads / one thread per row); a negative value
- * restores the built-in default / environment setting.  Results are bit-identical for every setting of split and
- * stream; poly changes P below its 16-bit rounding. */
-int dk_attention_tuning(int split, int poly, int stream);
 
 /* ---------------------------------------------------------------------------------------------
  * elementwise / layout kernels on the MMDiT path
@@ -224,7 +218,7 @@ int dk_groupnorm_stats(dk_ctx* ctx, int dtype, const void* x, float* stats, floa
 int dk_groupnorm_apply(dk_ctx* ctx, int dtype, const void* x, void* y, const float* stats, const void* gamma,
                        const void* beta, int B, int HW, int C, int G, int silu, void* stream);
 /* K7  conv 3x3, stride 1, zero pad 1, NHWC, as an im2col-free implicit GEMM: the 9 taps are 9 shifted TMA
- *     boxes of the input (out-of-bounds = zero fill = the padding), accumulated in TMEM.
+ *     boxes of the input (out-of-bounds = zero fill = the padding), accumulated in registers (wgmma).
  *     x [B,H,W,Cin] (Cin % 64 == 0), w [Cout,3,3,Cin] (Cout % 8 == 0), bias [Cout], res NHWC [B,H,W,Cout] or NULL
  *     (the ResnetBlock2D skip, vae.py:99).  replaces nn.Conv2d 3x3 (vae.py:73-81,134-136,349-351,384) */
 int dk_conv3x3(dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias, const void* res, void* out,

@@ -1,4 +1,4 @@
-"""GPU checks of the individual sm_100a kernels against plain fp32 torch references of the same op.
+"""GPU checks of the individual sm_90a kernels against plain fp32 torch references of the same op.
 
 Each check_* function is self-contained (used by tests/test_kernels_gpu.py and by tools/run_gpu_checks.py, which
 runs every check in its own process so that one trapped kernel cannot poison the others).
@@ -114,7 +114,7 @@ def check_gemm_shapes():
 
 def check_gemm_persistent_large():
     _setup()
-    # more tiles than SMs: exercises the persistent loop, both TMEM accumulators and the smem ring wrap-around
+    # more tiles than SMs: exercises more than one wave of CTAs and the smem ring wrap-around
     return {"err": _gemm_case(4096, 4608, 1024, torch.bfloat16, bias=True, name="gemm_4096x4608x1024")}
 
 
@@ -366,8 +366,7 @@ def check_attention_d64():
 
 
 def check_attention_v3_explicit():
-    """the round-1 form of v3 (DK_ATTENTION_IMPL=3p: one P publication per step, every exponential on MUFU)"""
-    os.environ["DK_ATTENTION_IMPL"] = "3p"
+    """split outputs with a ragged tail at d = 64 (fp16 and bf16), two batches at d = 128, rescale"""
     _setup()
     out = {"d64_S1178_split": _attention_case(2, 1178, 2, 64, torch.float16, split=1024, name="att3_d64_S1178"),
            "d64_S333": _attention_case(1, 333, 2, 64, torch.bfloat16, name="att3_d64_S333"),
@@ -377,40 +376,24 @@ def check_attention_v3_explicit():
 
 
 def check_attention_v3_variants():
-    """every (split, streamed pass, poly share) setting of v3 through the in-process tuning hook: each against the fp32
-    reference; the streamed pass is bit-identical to the two-round pass with the same poly share (the split publication
-    alone changes the order in which the PV MMAs accumulate, so it is only compared with the reference)"""
+    """long ragged sequences at both head dims against the fp32 reference, and the kernel is deterministic: a second
+    launch on the same input is bit-identical to the first (the K/V steps and the quad reductions run in a fixed order)"""
     _setup()
-    from diffusionkit_b200 import _lib
-    lib = _lib.load()
     out = {}
-    try:
-        for d, dt, S in ((128, torch.bfloat16, 1300), (64, torch.float16, 1178)):
-            qkv = _rand((2 * S, 3 * 2 * d), dt)
-            for poly in (0, 1, 2):
-                base = None
-                for split, stream in ((0, 0), (1, 0), (1, 1)):
-                    lib.dk_attention_tuning(split, poly, stream)
-                    name = f"att3_d{d}_split{split}_stream{stream}_poly{poly}"
-                    out[name] = _attention_case(2, S, 2, d, dt, split=1024, name=name)
-                    o = torch.zeros((2 * S, 2 * d), dtype=dt, device=DEV)
-                    ops.attention(qkv, 2, S, 2, d, o)
-                    if split and base is None:
-                        base = o
-                    elif split:
-                        assert torch.equal(o, base), f"{name}: not bit-identical to the two-round pass"
-    finally:
-        lib.dk_attention_tuning(-1, -1, -1)
+    for d, dt, S in ((128, torch.bfloat16, 1300), (64, torch.float16, 1178)):
+        name = f"att_d{d}_S{S}"
+        out[name] = _attention_case(2, S, 2, d, dt, split=1024, name=name)
+        qkv = _rand((2 * S, 3 * 2 * d), dt)
+        o1 = torch.zeros((2 * S, 2 * d), dtype=dt, device=DEV)
+        o2 = torch.zeros((2 * S, 2 * d), dtype=dt, device=DEV)
+        ops.attention(qkv, 2, S, 2, d, o1)
+        ops.attention(qkv, 2, S, 2, d, o2)
+        assert torch.equal(o1, o2), f"{name}: two launches on the same input differ"
     return out
 
 
 def check_attention_v3s_kernel():
-    """v3 with the split P publication but the two-round exponential pass (DK_ATT_STREAM=0): the PV MMAs of the first 32
-    keys of every thread are issued while the exponentials of the other 32 are still running"""
-    os.environ["DK_ATTENTION_IMPL"] = "3"
-    os.environ["DK_ATT_SPLIT"] = "1"
-    os.environ["DK_ATT_STREAM"] = "0"
-    os.environ["DK_ATT_POLY"] = "1"
+    """one full K/V tile, ragged tails, split outputs at both head dims, a one-token sequence, rescale"""
     _setup()
     out = {"d128_S128": _attention_case(1, 128, 1, 128, torch.bfloat16, name="att3s_d128_S128"),
            "d128_S300": _attention_case(2, 300, 2, 128, torch.bfloat16, name="att3s_d128_S300"),
@@ -422,9 +405,7 @@ def check_attention_v3s_kernel():
 
 
 def check_attention_v5_kernel():
-    """persistent kernel with register-resident scores and speculative exponentials (DK_ATTENTION_IMPL=5): one and many
-    work items per CTA (items > SMs), odd/even K/V tile counts, tails, both head dims, split outputs, lazy rescale"""
-    os.environ["DK_ATTENTION_IMPL"] = "5"
+    """more CTAs than SMs, odd/even K/V tile counts, tails, both head dims, split outputs, rescale"""
     _setup()
     out = {"d128_S128": _attention_case(1, 128, 1, 128, torch.bfloat16, name="att5_d128_S128"),
            "d128_S256": _attention_case(1, 256, 2, 128, torch.bfloat16, name="att5_d128_S256"),
@@ -440,10 +421,8 @@ def check_attention_v5_kernel():
 
 
 def check_attention_v6_kernel():
-    """64-key steps with double-buffered score accumulators (DK_ATTENTION_IMPL=6): one and many steps, odd / even step
-    counts, ragged tails (incl. a fully masked 32-key half), both head dims, split outputs, poly share, lazy rescale
-    (which has to wait for the previous PV here)"""
-    os.environ["DK_ATTENTION_IMPL"] = "6"
+    """one and many K/V steps, odd / even step counts, ragged tails (incl. tiles with a fully masked half), both head
+    dims, split outputs, rescale"""
     _setup()
     out = {"d128_S64": _attention_case(1, 64, 1, 128, torch.bfloat16, name="att6_d128_S64"),
            "d128_S128": _attention_case(1, 128, 1, 128, torch.bfloat16, name="att6_d128_S128"),
@@ -527,16 +506,15 @@ def check_qk_norm_rope():
 
 
 def check_gemm_pair_kernel():
-    """the CTA-pair (cta_group::2, 256x256 tile) GEMM forced for every legal shape (DK_GEMM_PAIR=2): ragged M/N/K,
-    every epilogue, multi-wave persistence"""
-    os.environ["DK_GEMM_PAIR"] = "2"
+    """large and ragged shapes (256- and 128-wide tiles): ragged M/N/K, every epilogue, more tiles than SMs, strided
+    output windows, in-place residual, the fused QK epilogue"""
     _setup()
     out = {}
     for (M, N, K) in [(256, 256, 64), (256, 512, 512), (300, 264, 200), (77, 64, 64), (1000, 3072, 1536),
                       (4352, 768, 3072), (20, 1024, 3072)]:
         out[f"{M}x{N}x{K}"] = _gemm_case(M, N, K, torch.bfloat16, name=f"pair_{M}x{N}x{K}")
     out["large"] = _gemm_case(8192, 4608, 1024, torch.bfloat16, bias=True, name="pair_8192x4608x1024")
-    out["bn192"] = _gemm_case(4096, 3072, 512, torch.bfloat16, bias=True, name="pair_4096x3072x512")      # re-tiled 192
+    out["n3072"] = _gemm_case(4096, 3072, 512, torch.bfloat16, bias=True, name="pair_4096x3072x512")
     out["bn128"] = _gemm_case(1024, 1152, 256, torch.bfloat16, bias=True, gate=True, res=True, name="pair_1024x1152")
     out["gelu"] = _gemm_case(384, 512, 256, torch.bfloat16, bias=True, act=ACT_GELU_ERF, name="pair_gelu")
     out["remap"] = _gemm_case(600, 512, 256, torch.bfloat16, bias=True, gate=True, res=True, remap=True,
@@ -548,7 +526,7 @@ def check_gemm_pair_kernel():
 
 
 def _pair_store_cases():
-    """outputs the TMA-store epilogue has to get right: a strided column window of a wider buffer (the FLUX single-block
+    """outputs the GEMM epilogue has to get right: a strided column window of a wider buffer (the FLUX single-block
     concat buffer), rows/columns that are not tile multiples next to data that must survive, in-place residual"""
     out = {}
     M, N, K, ld, c0 = 1000, 520, 256, 1024, 256
@@ -568,9 +546,8 @@ def _pair_store_cases():
 
 
 def check_gemm_pair_legacy_store():
-    """the register -> global store path of the pair kernel (DK_GEMM_TMA_STORE=0) stays correct"""
-    os.environ["DK_GEMM_PAIR"] = "2"
-    os.environ["DK_GEMM_TMA_STORE"] = "0"
+    """the epilogue's register -> global stores with bias, gate and in-place-able residual on a multi-tile problem and a
+    ragged one, plus the output-window cases"""
     _setup()
     out = {"large": _gemm_case(2048, 1536, 512, torch.bfloat16, bias=True, gate=True, res=True, name="pairleg_large"),
            "ragged": _gemm_case(300, 264, 200, torch.bfloat16, name="pairleg_ragged")}
@@ -844,7 +821,7 @@ def check_fullsize_conv_fused():
 
 # ------------------------------------------------------------------------------------------------ BASELINE shapes
 # Parity at the shapes bench.py times (BASELINE.json C3/C4/C5): every kernel against fp32 torch at full size, with a
-# per-block error map on top of the global rel-L2 so that ONE wrong output tile (a scheduler wrap, a TMEM phase slip,
+# per-block error map on top of the global rel-L2 so that ONE wrong output tile (a tile-index decode slip, a barrier phase slip,
 # a tail tile) cannot hide in the average.
 def _assert_close_blocks(name, got, ref, tol, block_tol, br=128, bc=128):
     """global rel-L2 <= tol AND every br x bc block's rel-L2 (vs the block's own reference norm) <= block_tol"""
@@ -1035,24 +1012,5 @@ ALL_CHECKS = [
     check_softmax_image_post, check_edge_cases, check_error_paths,
 ] + FULLSIZE_CHECKS
 
-# kernels behind an environment knob that have not been measured / validated on hardware yet: not part of the pytest
-# suite; `python tools/run_gpu_checks.py +experimental <name>` runs them
-def check_attention_v6_one_thread_per_row():
-    """the 320-thread form of v6 (one thread per row; in-process selection: dk_attention_tuning stream = 3).  Run on
-    hardware in round 2 (profiles/r02_att_v6_one_call34.txt); outside the pytest suite because it is not a default."""
-    _setup()
-    from diffusionkit_b200 import _lib
-    lib = _lib.load()
-    lib.dk_attention_tuning(-1, -1, 3)
-    try:
-        return {"d128_S64": _attention_case(1, 64, 1, 128, torch.bfloat16, name="att7_d128_S64"),
-                "d128_S300": _attention_case(2, 300, 2, 128, torch.bfloat16, name="att7_d128_S300"),
-                "d128_S1280_split": _attention_case(1, 1280, 3, 128, torch.bfloat16, split=256, name="att7_d128_S1280"),
-                "d64_S1178_split": _attention_case(2, 1178, 2, 64, torch.float16, split=1024, name="att7_d64_S1178"),
-                "rescale": check_attention_large_scores()["err"]}
-    finally:
-        lib.dk_attention_tuning(-1, -1, -1)
-
-
-EXPERIMENTAL_CHECKS = [check_attention_v6_one_thread_per_row]
+EXPERIMENTAL_CHECKS = []
 

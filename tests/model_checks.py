@@ -577,8 +577,7 @@ def check_product_vs_reference_source():
     torch-backed stand-in for the MLX primitives, tests/golden/make_reference_mlx_golden.py — with no oracle in between:
     FLUX and SD3 MMDiT forward through the modulation cache, VAE decoder (raw output and clipped image) and VAE encoder
     (uint8 image in, read_image scaling fused) at their real widths.  16-bit product vs fp32 reference source; bounds =
-    the 16-bit-vs-fp32 tolerances of this file.  Measured on B200: FLUX rel-L2 8.1e-3 / 54.3 dB, SD3 9.1e-4 / 73.5 dB,
-    decoder 1.5e-2 (image 47.1 dB), encoder 1.4e-2."""
+    the 16-bit-vs-fp32 tolerances of this file."""
     from tests.golden import make_reference_mlx_golden as mk
 
     out = {}

@@ -1,5 +1,4 @@
 """-m gpu: every hand-written kernel against an fp32 torch reference of the same op (through the C ABI)."""
-import json
 import os
 import subprocess
 import sys
@@ -11,11 +10,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, HERE)
 
-# checks that select a non-default kernel through an environment variable the library latches on first use:
-# they need a process of their own
-ISOLATED = {"check_gemm_pair_kernel", "check_gemm_pair_legacy_store", "check_attention_v3_explicit",
-            "check_attention_v3s_kernel", "check_attention_v5_kernel", "check_attention_v6_kernel"}
-
 
 def pytest_generate_tests(metafunc):
     if "check" in metafunc.fixturenames:
@@ -25,13 +19,6 @@ def pytest_generate_tests(metafunc):
 
 
 def test_kernel(cuda, check):
-    if check.__name__ in ISOLATED:
-        p = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "run_gpu_checks.py"), "--one", check.__name__],
-                           capture_output=True, text=True, timeout=600)
-        lines = [l for l in p.stdout.splitlines() if l.startswith("RESULT ")]
-        assert p.returncode == 0 and lines, (p.stdout + p.stderr)[-2000:]
-        assert json.loads(lines[-1][7:])["ok"]
-        return
     res = check()
     assert isinstance(res, dict)
 
