@@ -77,12 +77,26 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// The same wait with a call-free watchdog (trap without the report), for kernels that wait while wgmma groups are in
+// flight: a function call anywhere in such a kernel makes ptxas serialise all of its wgmma instructions.
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins == DK_WATCHDOG_SPINS) asm volatile("trap;");
+  }
+}
 
 // Whole-warp wait with a single polling lane: lane 0 spins (hardware-suspended try_wait), the other 31 lanes park at
 // the warp barrier instead of burning issue slots and power on their own polls.
 __device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
   if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity);
   __syncwarp();
+}
+
+// 32-bit store to shared memory through its shared-window address: unlike a store through a generic pointer, it does
+// not keep the compiler from moving global loads above it
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v));
 }
 
 // generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
@@ -92,6 +106,29 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// --------------------------------------------------------------------------------------------
+// thread-block clusters
+// --------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; orders barrier initialisation / remote shared-memory traffic
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (which may be this CTA).  Plain
+// arrive: a .release.cluster arrive after every k-block made the GEMM mainloop markedly slower (measured on H100).
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
+      "r"(cta)
+      : "memory");
 }
 
 // --------------------------------------------------------------------------------------------
@@ -105,6 +142,16 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::
           "r"(smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+// The same box written to the same shared-memory offset of every CTA in cta_mask; each destination CTA's mbarrier at
+// bar's offset receives the transaction bytes.
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster "
+      "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,

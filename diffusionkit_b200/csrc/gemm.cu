@@ -1,20 +1,26 @@
-// K1 / K7 — warp-specialised wgmma GEMM for sm_90a, and its implicit-GEMM 3x3 convolution variant.
+// K1 / K7 — warp-specialised, persistent wgmma GEMM for sm_90a, and its implicit-GEMM 3x3 convolution variant.
 //
 //   out = epilogue( A[M,K] * W[N,K]^T )        (nn.Linear — reference mlx/mmdit.py:471-473,532,830-835, ...)
 //   out = epilogue( conv3x3(x NHWC, w OHWI) )  (nn.Conv2d — reference mlx/vae.py:73-81,134-136,349-351,384)
 //
-// Structure (one 128 x BN output tile per CTA, 384 threads):
-//   warpgroup 0 (warp 0): TMA producer — streams 128x64 A tiles and BNx64 W tiles (128B swizzle) through a
-//                         STAGES-deep mbarrier ring.  For the convolution the A tile of tap (dy,dx) is a shifted 4-D
-//                         TMA box of the NHWC input; out-of-bounds elements are zero-filled by the TMA unit, which
-//                         *is* the zero padding — no im2col buffer exists anywhere.
+// Structure (2-CTA clusters along M, 384 threads per CTA, as many CTAs as can be resident):
+//   schedule            : a cluster tile is (m-block pair, n-block); every cluster walks the cluster tiles with a static
+//                         stride, grouped 16 m-blocks per group so the resident clusters share A bands and W column
+//                         blocks in L2.  The two CTAs of a cluster take the two m-blocks of the pair.
+//   warpgroup 0 (warp 0): TMA producer — streams its 128x64 A tile and half of the BNx64 W tile (128B swizzle) through
+//                         a STAGES-deep mbarrier ring; the W half is multicast to both CTAs, so each CTA fetches
+//                         A + W/2 per k-block.  Ring stage and phase carry over from tile to tile, so the next tile's
+//                         loads start while the consumers are still in the epilogue.  For the convolution the A tile of
+//                         tap (dy,dx) is a shifted 4-D TMA box of the NHWC input; out-of-bounds elements are zero-filled
+//                         by the TMA unit, which *is* the zero padding — no im2col buffer exists anywhere.
 //   warpgroups 1, 2     : MMA consumers — each owns 64 rows of the tile: wgmma m64nBNk16 from shared memory into
-//                         register accumulators, one k-block group in flight while the next is issued.
-//   epilogue            : the accumulators go through an fp32 staging tile in the (then idle) pipeline buffers, so
-//                         that each thread owns one tile row: fused bias / GELU-erf / adaLN gate / residual, or
-//                         QK-RMSNorm + RoPE on the q/k thirds of a packed QKV projection; 128-bit stores straight to
-//                         the destination row (row remap = joint-sequence scatter).
-#include <stdlib.h>
+//                         register accumulators, one k-block group in flight while the next is issued.  A stage is
+//                         released to the producers of both CTAs (it may be refilled only when both have read it).
+//   epilogue            : on the accumulator fragments in registers (gemm_epilogue_tile): fused bias / GELU-erf /
+//                         adaLN gate / residual, or QK-RMSNorm + RoPE on the q/k thirds of a packed QKV projection;
+//                         16-bit results go through a dedicated shared-memory tile to 16-byte row stores (row remap =
+//                         joint-sequence scatter).
+#include <algorithm>
 
 #include "common.cuh"
 #include "gemm_epilogue.cuh"
@@ -25,6 +31,7 @@ namespace dk {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int GEMM_THREADS = 384;
+constexpr int CLUSTER = 2;
 
 template <int BN>
 struct GemmCfg {
@@ -32,14 +39,30 @@ struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int PIPE_BYTES = STAGES * (A_BYTES + B_BYTES);
-  static constexpr int STAGE_LD = BN + 4;   // fp32 staging row stride (floats): +4 spreads the rows over the banks
-  static_assert(PIPE_BYTES >= BM * STAGE_LD * 4, "the epilogue staging tile reuses the pipeline buffers");
+  static constexpr int EPI_BYTES = BM * (BN < 128 ? BN : 128) * 2;   // 16-bit output staging, one column pass
+  static constexpr int RSTD_BYTES = BM * 2 * 4;                       // QK-RMSNorm: 1/rms per (row, head of a pass)
   static constexpr int BAR_BYTES = 256;
-  static constexpr int SMEM_BYTES = PIPE_BYTES + BAR_BYTES + 1024;  // +1024: manual alignment slack
+  static constexpr int SMEM_BYTES = PIPE_BYTES + EPI_BYTES + RSTD_BYTES + BAR_BYTES + 1024;  // +1024: alignment slack
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 };
+
+// Cluster tile ct -> this CTA's (m-block, n-block).  When num_m is odd the partner of the last m-block gets
+// m_blk == num_m: its loads are zero-filled and its epilogue stores nothing.
+__device__ __forceinline__ void cluster_tile(int ct, const GemmShape& s, uint32_t rank, int& m_blk, int& n_blk) {
+  constexpr int GC = 8;  // m-block pairs per rasterisation group (16 m-blocks)
+  const int num_cm = (s.num_m + 1) >> 1;
+  const int group_size = GC * s.num_n;
+  const int group = ct / group_size;
+  const int first = group * GC;
+  const int gsz = min(num_cm - first, GC);
+  const int in_group = ct - group * group_size;
+  m_blk = 2 * (first + in_group % gsz) + static_cast<int>(rank);
+  n_blk = in_group / gsz;
+}
 
 // MODE 0: plain GEMM.  MODE 1: conv3x3 implicit GEMM (A via 4-D TMA boxes).
 // B_MN: W operand given as [K, N] row-major (MN-major wgmma operand, transposed B).
+// Launched in clusters of 2 along x with an even grid of at most (resident clusters) x 2 CTAs.
 template <typename T, int BN, bool B_MN, int MODE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape s,
@@ -50,168 +73,138 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr int B_BYTES = Cfg::B_BYTES;
 
   extern __shared__ uint8_t smem_raw[];
-  // 128B-swizzled tiles need 1024-byte aligned bases.
+  // 128B-swizzled tiles need 1024-byte aligned bases.  The multicast writes the partner's shared memory at the same
+  // offsets, so the layout must be identical in both CTAs (same kernel, same dynamic size, same base alignment).
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::PIPE_BYTES);
+  uint8_t* stg = smem + Cfg::PIPE_BYTES;
+  float* rstd = reinterpret_cast<float*>(stg + Cfg::EPI_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg + Cfg::EPI_BYTES + Cfg::RSTD_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
+  const uint32_t rank = cluster_ctarank();
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp
+      mbar_init(&empty_bar[i], 8 * CLUSTER);  // one arrive per consumer warp of each CTA of the cluster
     }
     fence_barrier_init();
   }
-  __syncthreads();
+  // the partner's multicast loads and stage releases target this CTA's barriers: both must be initialised first
+  cluster_sync();
 
-  // Grouped rasterisation: consecutive tile ids walk GM m-blocks for one n-block, so the CTAs resident at a time
-  // share a band of A rows and a handful of W column blocks (L2 reuse).
-  constexpr int GM = 16;
-  int m_blk, n_blk;
-  {
-    const int tile = blockIdx.x;
-    const int group_size = GM * s.num_n;
-    const int group = tile / group_size;
-    const int first_m = group * GM;
-    const int gsz = min(s.num_m - first_m, GM);
-    const int in_group = tile - group * group_size;
-    m_blk = first_m + in_group % gsz;
-    n_blk = in_group / gsz;
-  }
+  const int num_ctiles = ((s.num_m + 1) >> 1) * s.num_n;
+  const int first_ct = blockIdx.x / CLUSTER;
+  const int ct_stride = gridDim.x / CLUSTER;
 
   if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer, converged warp
-    if (warp != 0) return;
-    int img = 0, y0 = 0, x0 = 0;
-    if (MODE == 1) {
-      const int per_img = g.tiles_x * g.tiles_y;
-      img = m_blk / per_img;
-      const int t = m_blk - img * per_img;
-      y0 = (t / g.tiles_x) * g.TH;
-      x0 = (t % g.tiles_x) * g.TW;
-    }
-    uint32_t stage = 0, phase = 0;
-    for (int kb = 0; kb < s.num_k; ++kb) {
-      mbar_wait_warp(&empty_bar[stage], phase ^ 1);
-      if (elect_one_sync()) {
-        mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
-        uint8_t* a_dst = sA + stage * A_BYTES;
-        uint8_t* b_dst = sB + stage * B_BYTES;
-        if (MODE == 0) {
-          tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
-        } else {
-          const int tap = kb / g.cblocks;
-          const int c0 = (kb - tap * g.cblocks) * BK;
-          const int dy = tap / 3, dx = tap - dy * 3;
-          tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, x0 * g.stride + dx - g.pad, y0 * g.stride + dy - g.pad, img);
+    setmaxnreg_dec<40>();
+    if (warp == 0) {
+      uint32_t stage = 0, phase = 0;
+      for (int ct = first_ct; ct < num_ctiles; ct += ct_stride) {
+        int m_blk, n_blk;
+        cluster_tile(ct, s, rank, m_blk, n_blk);
+        int img = 0, y0 = 0, x0 = 0;
+        if (MODE == 1) {
+          const int per_img = g.tiles_x * g.tiles_y;
+          img = m_blk / per_img;
+          const int t = m_blk - img * per_img;
+          y0 = (t / g.tiles_x) * g.TH;
+          x0 = (t % g.tiles_x) * g.TW;
         }
-        if (!B_MN) {
-          tma_load_2d(b_dst, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
-        } else {
+        for (int kb = 0; kb < s.num_k; ++kb) {
+          if (lane == 0) mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
+          __syncwarp();
+          if (elect_one_sync()) {
+            // A (own) + the whole W tile: this CTA's half and the partner's multicast half
+            mbar_arrive_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);
+            uint8_t* a_dst = sA + stage * A_BYTES;
+            uint8_t* b_dst = sB + stage * B_BYTES;
+            if (MODE == 0) {
+              tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
+            } else {
+              const int tap = kb / g.cblocks;
+              const int c0 = (kb - tap * g.cblocks) * BK;
+              const int dy = tap / 3, dx = tap - dy * 3;
+              tma_load_4d(a_dst, &tmA, &full_bar[stage], c0, x0 * g.stride + dx - g.pad, y0 * g.stride + dy - g.pad,
+                          img);
+            }
+            if (!B_MN) {
+              // rows [rank*BN/2, (rank+1)*BN/2) of the W tile
+              tma_load_2d_multicast(b_dst + rank * (B_BYTES / 2), &tmB, &full_bar[stage], kb * BK,
+                                    n_blk * BN + static_cast<int>(rank) * (BN / 2), 0x3);
+            } else {
 #pragma unroll
-          for (int j = 0; j < BN / 64; ++j)
-            tma_load_2d(b_dst + j * (BK * 128), &tmB, &full_bar[stage], n_blk * BN + j * 64, kb * BK);
+              for (int j = 0; j < BN / 64; ++j)
+                if (j % CLUSTER == static_cast<int>(rank))
+                  tma_load_2d_multicast(b_dst + j * (BK * 128), &tmB, &full_bar[stage], n_blk * BN + j * 64, kb * BK,
+                                        0x3);
+            }
+          }
+          __syncwarp();
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
         }
       }
-      __syncwarp();
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
     }
-    return;
-  }
-
-  // -------------------------------------------------------------------- MMA consumers: rows 64*cw .. 64*cw+63
-  const int cw = wg - 1;
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  {
-    uint32_t stage = 0, phase = 0, prev = 0;
-    for (int kb = 0; kb < s.num_k; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t a_base = smem_u32(sA + stage * A_BYTES) + cw * 64 * 128;
-      const uint32_t b_base = smem_u32(sB + stage * B_BYTES);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {
-        const uint64_t da = make_smem_desc_sw128(a_base + k * 32, 16, 1024);
-        const uint64_t db = B_MN ? make_smem_desc_sw128(b_base + k * 16 * 128, BK * 128, 1024)
-                                 : make_smem_desc_sw128(b_base + k * 32, 16, 1024);
-        Wgmma<BN, Half16<T>::is_bf16, B_MN ? 1 : 0>::ss(acc, da, db, (kb | k) != 0 ? 1u : 0u);
-      }
-      wgmma_commit();
-      // the previous k-block's MMAs have retired: its stage can be refilled
-      wgmma_wait<1>();
-      if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
-    wgmma_wait<0>();
-    reg_fence(acc);
-  }
-
-  // ------------------------------------------------------------------ epilogue (256 threads, thread = tile row)
-  // every TMA load has landed and every MMA has retired once both warpgroups pass this barrier: the pipeline buffers
-  // become the fp32 staging tile
-  float* stg = reinterpret_cast<float*>(smem);
-  named_bar_sync(1, 256);
-  stage_acc_rows<BN>(stg, Cfg::STAGE_LD, cw * 64, acc);
-  named_bar_sync(1, 256);
-
-  const int ew = warp - 4;               // 0..7
-  const int quarter = ew & 3;            // rows 32*quarter .. 32*quarter+31
-  const int half = ew >> 2;              // which half of the tile's columns this warp drains
-  constexpr int NCH = BN / 64;           // 32-column chunks per thread
-  const int r_in_tile = quarter * 32 + lane;
-
-  // destination rows
-  bool row_ok;
-  long long orow, rrow;
-  int batch, pos = 0;
-  if (MODE == 0) {
-    const int m = m_blk * BM + r_in_tile;
-    row_ok = m < s.M;
-    batch = m / e.rpb;
-    const int in_b = m - batch * e.rpb;
-    pos = e.out_row_off + in_b;  // position in the joint sequence (RoPE)
-    orow = static_cast<long long>(batch) * e.out_batch_rows + e.out_row_off + in_b;
-    rrow = static_cast<long long>(batch) * e.res_batch_rows + e.res_row_off + in_b;
   } else {
-    const int per_img = g.tiles_x * g.tiles_y;
-    const int img = m_blk / per_img;
-    const int t = m_blk - img * per_img;
-    const int y = (t / g.tiles_x) * g.TH + r_in_tile / g.TW;
-    const int x = (t % g.tiles_x) * g.TW + r_in_tile % g.TW;
-    row_ok = (y < g.H) && (x < g.W);
-    batch = img;
-    orow = (static_cast<long long>(img) * g.H + y) * g.W + x;
-    rrow = orow;
-  }
-  const float* srow = stg + r_in_tile * Cfg::STAGE_LD + half * (BN / 2);
-  auto load32 = [&](int c, uint32_t (&r)[32]) {
+    // ------------------------------------------------------------------ MMA consumers: rows 64*cw .. 64*cw+63
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;
+    float acc[BN / 2];
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const float4 v = *reinterpret_cast<const float4*>(srow + c + 4 * q);
-      r[4 * q] = __float_as_uint(v.x);
-      r[4 * q + 1] = __float_as_uint(v.y);
-      r[4 * q + 2] = __float_as_uint(v.z);
-      r[4 * q + 3] = __float_as_uint(v.w);
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    uint32_t stage = 0, phase = 0;
+    for (int ct = first_ct; ct < num_ctiles; ct += ct_stride) {
+      int m_blk, n_blk;
+      cluster_tile(ct, s, rank, m_blk, n_blk);
+      uint32_t prev = 0;
+      for (int kb = 0; kb < s.num_k; ++kb) {
+        mbar_wait_nocall(&full_bar[stage], phase);
+        const uint32_t a_base = smem_u32(sA + stage * A_BYTES) + cw * 64 * 128;
+        const uint32_t b_base = smem_u32(sB + stage * B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t da = make_smem_desc_sw128(a_base + k * 32, 16, 1024);
+          const uint64_t db = B_MN ? make_smem_desc_sw128(b_base + k * 16 * 128, BK * 128, 1024)
+                                   : make_smem_desc_sw128(b_base + k * 32, 16, 1024);
+          Wgmma<BN, Half16<T>::is_bf16, B_MN ? 1 : 0>::ss(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        // the previous k-block's MMAs have retired: its stage can be refilled, in both CTAs of the cluster
+        wgmma_wait<1>();
+        if (kb > 0 && lane == 0) {
+          mbar_arrive_cluster(&empty_bar[prev], 0);
+          mbar_arrive_cluster(&empty_bar[prev], 1);
+        }
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (lane == 0) {
+        mbar_arrive_cluster(&empty_bar[prev], 0);
+        mbar_arrive_cluster(&empty_bar[prev], 1);
+      }
+      gemm_epilogue_tile<T, BN, MODE>(acc, s, e, g, m_blk, n_blk, cw, stg + cw * (Cfg::EPI_BYTES / 2), rstd + cw * 128);
     }
-  };
-  gemm_epilogue_drain<T, NCH, MODE>(s, e, load32, n_blk * BN + half * (BN / 2), row_ok, orow, rrow, batch, pos);
+  }
+  // no CTA may leave while its partner can still multicast into its shared memory or arrive on its barriers
+  cluster_sync();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -222,12 +215,30 @@ static int launch_gemm_inst(dk_ctx* ctx, const CUtensorMap& tmA, const CUtensorM
                             const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
   auto kern = gemm_wgmma_kernel<T, BN, B_MN, MODE>;
-  static bool configured = false;
-  if (!configured) {
+  cudaLaunchAttribute cluster;
+  cluster.id = cudaLaunchAttributeClusterDimension;
+  cluster.val.clusterDim.x = CLUSTER;
+  cluster.val.clusterDim.y = 1;
+  cluster.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(CLUSTER);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+  cfg.stream = stream;
+  cfg.attrs = &cluster;
+  cfg.numAttrs = 1;
+  // resident clusters: a GPC whose SM count is odd leaves one SM without a partner
+  static int max_clusters = 0;
+  if (max_clusters == 0) {
     DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    configured = true;
+    int n = 0;
+    DK_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+    DK_REQUIRE(n > 0, "dk_gemm: no 2-CTA cluster of the GEMM kernel fits on the device");
+    max_clusters = n;
   }
-  kern<<<s.num_m * s.num_n, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, s, e, g);
+  const int cluster_tiles = dk_ceil_div(s.num_m, CLUSTER) * s.num_n;
+  cfg.gridDim = dim3(CLUSTER * std::min(cluster_tiles, max_clusters));
+  DK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, s, e, g));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
@@ -294,10 +305,6 @@ extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
   e.res_batch_rows = a->rows_per_batch > 0 ? a->res_batch_rows : a->M;
   e.res_row_off = a->res_row_off;
   e.act = a->act;
-  {
-    static const int dbg = [] { const char* v = getenv("DK_GEMM_EPI_DEBUG"); return v ? atoi(v) : 0; }();
-    e.debug = dbg;
-  }
   e.qk_qw = a->qk_q_weight;
   e.qk_kw = a->qk_k_weight;
   e.qk_rope = a->qk_rope;
@@ -323,7 +330,7 @@ extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
   if (!a->w_n_major) {
     const uint64_t dims[2] = {static_cast<uint64_t>(a->K), static_cast<uint64_t>(a->N)};
     const uint64_t strides[1] = {static_cast<uint64_t>(a->ldw) * 2};
-    const uint32_t box[2] = {BK, static_cast<uint32_t>(bn)};
+    const uint32_t box[2] = {BK, static_cast<uint32_t>(bn / CLUSTER)};   // each CTA of a cluster loads half the tile
     if (int rc = dk_make_tmap_16b(ctx, &tmB, a->W, 2, dims, strides, box)) return rc;
   } else {
     const uint64_t dims[2] = {static_cast<uint64_t>(a->N), static_cast<uint64_t>(a->K)};
@@ -406,7 +413,7 @@ static int conv3x3_impl(dk_ctx* ctx, int dtype, const void* x, const void* w, co
   {
     const uint64_t dims[2] = {static_cast<uint64_t>(9 * Cin), static_cast<uint64_t>(Cout)};
     const uint64_t strides[1] = {static_cast<uint64_t>(9 * Cin) * 2};
-    const uint32_t box[2] = {BK, static_cast<uint32_t>(bn)};
+    const uint32_t box[2] = {BK, static_cast<uint32_t>(bn / CLUSTER)};
     if (int rc = dk_make_tmap_16b(ctx, &tmB, w, 2, dims, strides, box)) return rc;
   }
   if (dtype == DK_BF16) return launch_gemm_bn<__nv_bfloat16, false, 1>(ctx, bn, tmA, tmB, s, e, g, stream);
