@@ -20,8 +20,6 @@ H100 layout decisions (vs. the reference's per-module MLX graph):
 from __future__ import annotations
 
 import math
-import os
-from collections import OrderedDict
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -29,6 +27,7 @@ import torch
 from . import ops
 from ._lib import ACT_GELU_ERF, ACT_NONE, ACT_SILU, DkError
 from .config import MMDiTConfig, PositionalEncoding
+from .graphs import ShapeCache, default_settings
 
 
 class _Stream:
@@ -62,13 +61,10 @@ class MMDiT:
         self._mod_all: Optional[torch.Tensor] = None
         self._mod_cur: Optional[torch.Tensor] = None
         self._mod_batch = 0
-        # Everything a captured forward bakes device pointers of — workspace, RoPE table, cropped positional embedding —
-        # is owned PER SHAPE KEY together with the graph that uses it, so a graph can never outlive its buffers when one
-        # model serves several resolutions / text lengths (LRU-bounded: evicting a shape drops its graph with it).
-        self._shapes: "OrderedDict[tuple, dict]" = OrderedDict()
-        self.max_cached_shapes = int(os.environ.get("DK_MAX_CACHED_SHAPES", "4"))
-        # CUDA-graph replay of the (timestep-invariant) forward: one captured graph per input shape
-        self.use_cuda_graphs = os.environ.get("DK_CUDA_GRAPHS", "1") != "0"
+        # workspace, RoPE table and cropped positional embedding live per input shape, next to the CUDA graph of the
+        # (timestep-invariant) forward that bakes in their pointers
+        self._shapes = ShapeCache()
+        self.use_cuda_graphs, self.max_cached_shapes = default_settings()
 
     # ------------------------------------------------------------------------------------------ weight packing
     def _pack(self, P: Dict[str, torch.Tensor]):
@@ -174,8 +170,7 @@ class MMDiT:
         if self._mod_cur is None or self._mod_batch != B:
             # persistent buffer: captured graphs read the current step's modulation rows from this address
             self._mod_cur = torch.empty((B, self.mod_total), dtype=self.dtype, device=self.device)
-            for st in self._shapes.values():
-                st["graph"] = None
+            self._shapes.drop_graphs()
         self._mod_batch = B
         self._mod_index = {}
         for i, t in enumerate(ts):
@@ -200,19 +195,8 @@ class MMDiT:
         return self._mod_cur[:, s_off + k * self.h: s_off + (k + 1) * self.h]
 
     # ------------------------------------------------------------------------------------------ workspace
-    def _shape_state(self, key: tuple) -> dict:
-        st = self._shapes.get(key)
-        if st is None:
-            while len(self._shapes) >= max(1, self.max_cached_shapes):
-                self._shapes.popitem(last=False)            # least recently used shape: buffers AND graph go together
-            st = {"ws": None, "rope": None, "pos": None, "graph": None}
-            self._shapes[key] = st
-        else:
-            self._shapes.move_to_end(key)
-        return st
-
     def _workspace(self, st: dict, B: int, N: int, T: int):
-        if st["ws"] is not None:
+        if "ws" in st:
             return st["ws"]
         h, dt, dev = self.h, self.dtype, self.device
         S = N + T
@@ -239,7 +223,7 @@ class MMDiT:
     def _rope_table(self, st: dict, T: int, hp: int, wp: int) -> torch.Tensor:
         """(S, d/2, 2) fp32 cos/sin; text tokens at position (0,0,0), image token (r, c) at (0, r, c)
         (reference mmdit.py:865-911).  Cached across calls like the reference (:916-932)."""
-        if st["rope"] is not None:
+        if "rope" in st:
             return st["rope"]
         axes = self.config.rope_axes_dim
         S = T + hp * wp
@@ -306,26 +290,9 @@ class MMDiT:
                 self.select_timestep(tval)
         if self._mod_cur is None or self._mod_batch != B:
             raise DkError(f"modulation cache holds batch {self._mod_batch}, forward got batch {B}")
-        state = self._shape_state((B, H, W, Cl, T))
-        if not self.use_cuda_graphs:
-            return self._forward_impl(state, x, text, B, H, W, Cl, T)
-        entry = state["graph"]
-        if entry is None:
-            sx, stx = x.clone(), text.clone()
-            self._forward_impl(state, sx, stx, B, H, W, Cl, T)    # eager warm-up: workspaces, tables, func attributes
-            torch.cuda.current_stream().synchronize()
-            n0 = ops.launch_count()
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                so = self._forward_impl(state, sx, stx, B, H, W, Cl, T)
-            entry = (graph, sx, stx, so, ops.launch_count() - n0)
-            state["graph"] = entry
-        graph, sx, stx, so, n_launch = entry
-        sx.copy_(x)
-        stx.copy_(text)
-        graph.replay()
-        ops.note_graph_launches(n_launch)
-        return so
+        state = self._shapes.state((B, H, W, Cl, T), self.max_cached_shapes)
+        return self._shapes.run(state, self.use_cuda_graphs,
+                                lambda xx, tt: self._forward_impl(state, xx, tt, B, H, W, Cl, T), x, text)
 
     def _forward_impl(self, state, x, text, B, H, W, Cl, T):
         c = self.config
@@ -343,7 +310,7 @@ class MMDiT:
             ops.gemm(ws["rows_in"], self.w_x, out=img, bias=self.b_x)
         else:
             ops.patchify(x, 1, out=ws["rows_in"])
-            if state["pos"] is None:
+            if "pos" not in state:
                 state["pos"] = ops.pos_embed_crop(self.pos_table, c.max_latent_resolution, hp, wp)
             ops.gemm(ws["rows_in"], self.w_x, out=img, bias=self.b_x, res=state["pos"], rows_per_batch=N,
                      out_batch_rows=N, res_batch_rows=0)

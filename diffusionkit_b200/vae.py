@@ -12,24 +12,24 @@ Same parameter names as the reference module tree (SURVEY.md App. C).  Kernels (
                     reference, vae.py:49-52; V consumed as an MN-major operand), fp32 row softmax; 1/sqrt(C) is folded
                     into the query projection once at load (the reference scales q before q k^T, :49: the unscaled
                     product would reach the fp16 limit 22x earlier)
-  fused ResNet path (decoder, wherever the shape allows — rows of >= 128 pixels): csrc/conv_fused.cu, ONE kernel per
-                    convolution = GroupNorm-apply + SiLU on the staged halo tile -> [nearest 2x by sub-pixel phases]
-                    -> conv 3x3 -> bias / skip -> output + the NEXT GroupNorm's partial statistics.  No normalised
-                    tensor, no upsampled tensor and no separate statistics pass ever touch HBM.
-  The whole decode is captured in a CUDA graph per input shape (buffers owned by the graph entry, LRU-bounded).
+  fused convolution (decoder, wherever dk_conv_fused_supported accepts the shape — rows of >= 128 pixels, Cin <= 512):
+                    csrc/conv_fused.cu, ONE kernel per convolution = GroupNorm-apply + SiLU on the staged halo tile ->
+                    [nearest 2x by sub-pixel phases] -> conv 3x3 -> bias / skip -> output + the NEXT GroupNorm's partial
+                    statistics.  No normalised tensor, no upsampled tensor and no separate statistics pass touch HBM.
+                    Other shapes, and the whole encoder, run the three unfused kernels above.
+  The whole decode is captured in a CUDA graph per input shape (graphs.py).
 """
 from __future__ import annotations
 
 import math
-import os
-from collections import OrderedDict
-from typing import Dict, Optional
+from typing import Dict
 
 import torch
 
 from . import ops
 from ._lib import DkError
 from .config import VAEDecoderConfig, VAEEncoderConfig
+from .graphs import ShapeCache, default_settings
 
 
 def _pad_dim(t: torch.Tensor, dim: int, to: int) -> torch.Tensor:
@@ -43,6 +43,8 @@ def _pad_dim(t: torch.Tensor, dim: int, to: int) -> torch.Tensor:
 class _VAEBlocks:
     """Parameter handling and the building blocks the decoder and the encoder share."""
 
+    fuse = True                                       # take the fused convolution wherever the shape allows
+
     def __init__(self, params: Dict[str, torch.Tensor], config, device=None):
         who = type(self).__name__
         any_p = next(iter(params.values()))
@@ -55,7 +57,6 @@ class _VAEBlocks:
         self.config = config
         self.groups = config.resnet_groups
         self.p = {k: v.to(device=self.device, dtype=self.dtype).contiguous() for k, v in params.items()}
-        self._gn_ws = None
         # attention scale 1/sqrt(C) folded into the query projection (fp32 product, rounded once): the reference computes
         # (q * scale) @ k^T (vae.py:49); scaling after the product would overflow fp16 22x earlier
         for k in [k for k in self.p if k.endswith("query_proj.weight")]:
@@ -65,36 +66,46 @@ class _VAEBlocks:
             self.p[kb] = (self.p[kb].float() * sc).to(self.dtype)
 
     # ------------------------------------------------------------------ building blocks
-    def _gn(self, x, name, silu):
-        B = x.shape[0]
-        n_ws = ops.ctx(self.device.index).lib.dk_groupnorm_ws_floats(B, self.groups)
-        if self._gn_ws is None or self._gn_ws.numel() < n_ws:
-            self._gn_ws = torch.empty(n_ws, dtype=torch.float32, device=self.device)
-        stats = ops.groupnorm_stats(x, self.groups, 1e-5, ws=self._gn_ws)
-        return ops.groupnorm_apply(x, stats, self.p[name + ".weight"], self.p[name + ".bias"], self.groups, silu)
-
-    def _conv(self, x, name, res=None):
-        return ops.conv3x3(x, self.p[name + ".weight"], self.p[name + ".bias"], res=res)
+    def _conv(self, x, conv, norm=None, st=None, res=None, up=False):
+        """[GroupNorm(norm) + SiLU] -> [nearest 2x] -> conv3x3 (+ bias, + res) -> (y, statistics of y).  One halo-tiled
+        kernel where the module fuses and the shape allows, else GroupNorm-apply, upsample and implicit-GEMM conv."""
+        w, b = self.p[conv + ".weight"], self.p[conv + ".bias"]
+        B, H, W, C = x.shape
+        Cout = w.shape[0]
+        gn = None if norm is None else (st.get(), self.p[norm + ".weight"], self.p[norm + ".bias"], self.groups)
+        if self.fuse and ops.conv_fused_supported(H, W, C, Cout):
+            part = None
+            if Cout % 128 == 0:                           # a narrow output tile (conv_out) writes no statistics
+                part = torch.empty((B, (4 if up else 1) * H * W // 128, self.groups, 2), dtype=torch.float32,
+                                   device=self.device)
+            y = ops.conv3x3_fused(x, self.up_w[conv] if up else w, bias=b, res=res, up=up, gn=gn, silu=gn is not None,
+                                  out_partial=part, out_G=self.groups)
+            return y, _Stats(y, self.groups, part)
+        if gn is not None:
+            x = ops.groupnorm_apply(x, *gn, True)
+        if up:
+            x = ops.upsample_nearest2x(x)
+        y = ops.conv3x3(x, w, b, res=res)
+        return y, _Stats(y, self.groups)
 
     def _lin(self, x2d, name, res=None):
         return ops.gemm(x2d, self.p[name + ".weight"], bias=self.p[name + ".bias"], res=res)
 
-    def _resnet(self, x, name):
+    def _resnet(self, x, st, name):
         """ResnetBlock2D.__call__ (vae.py:86-101)"""
-        y = self._gn(x, name + ".norm1", True)
-        y = self._conv(y, name + ".conv1")
-        y = self._gn(y, name + ".norm2", True)
+        y, st = self._conv(x, name + ".conv1", name + ".norm1", st)
         skip = x
         if (name + ".conv_shortcut.weight") in self.p:
             B, H, W, C = x.shape
             skip = self._lin(x.reshape(B * H * W, C), name + ".conv_shortcut").reshape(B, H, W, -1)
-        return self._conv(y, name + ".conv2", res=skip)
+        return self._conv(y, name + ".conv2", name + ".norm2", st, res=skip)
 
-    def _attention(self, x, name):
+    def _attention(self, x, st, name):
         """Attention.__call__ (vae.py:40-57): single head over the H*W positions."""
         B, H, W, C = x.shape
         S = H * W
-        y = self._gn(x, name + ".group_norm", False).reshape(B * S, C)
+        y = ops.groupnorm_apply(x, st.get(), self.p[name + ".group_norm.weight"], self.p[name + ".group_norm.bias"],
+                                self.groups, False).reshape(B * S, C)
         q = self._lin(y, name + ".query_proj")
         k = self._lin(y, name + ".key_proj")
         v = self._lin(y, name + ".value_proj")
@@ -105,8 +116,8 @@ class _VAEBlocks:
             ops.gemm(q[sl], k[sl], out=scores)                       # (scale q) k^T: the scale lives in query_proj
             ops.softmax_rows(scores, 1.0)
             ops.gemm(scores, v[sl], out=o[sl], w_n_major=True)        # P v   (v is [S, C] = [K, N] row-major)
-        out = self._lin(o, name + ".out_proj", res=x.reshape(B * S, C))
-        return out.reshape(B, H, W, C)
+        out = self._lin(o, name + ".out_proj", res=x.reshape(B * S, C)).reshape(B, H, W, C)
+        return out, _Stats(out, self.groups)
 
     def _pad_channels(self, x, to):
         B, H, W, C = x.shape
@@ -116,23 +127,20 @@ class _VAEBlocks:
 
 
 class _Stats:
-    """GroupNorm statistics of a tensor, produced lazily: either the partial sums the producing convolution wrote in its
-    epilogue (folded by dk_groupnorm_finalize) or, for tensors that did not come out of the fused kernel, the standalone
-    two-stage kernel."""
+    """GroupNorm statistics of a tensor, produced on first use: folded from the partial sums the producing fused
+    convolution wrote in its epilogue (dk_groupnorm_finalize), or, without them, by the standalone two-stage kernel."""
 
-    def __init__(self, owner, x, partial=None):
-        self.owner, self.x, self.partial, self._stats = owner, x, partial, None
+    def __init__(self, x, groups, partial=None):
+        self.x, self.groups, self.partial, self._stats = x, groups, partial, None
 
     def get(self):
         if self._stats is None:
             B, H, W, C = self.x.shape
-            G = self.owner.groups
+            G = self.groups
             if self.partial is not None:
                 self._stats = ops.groupnorm_finalize(self.partial, B, G, H * W // 128, float(H * W * (C // G)), 1e-5)
             else:
-                n_ws = ops.ctx(self.owner.device.index).lib.dk_groupnorm_ws_floats(B, G)
-                ws = torch.empty(n_ws, dtype=torch.float32, device=self.owner.device)
-                self._stats = ops.groupnorm_stats(self.x, G, 1e-5, ws=ws)
+                self._stats = ops.groupnorm_stats(self.x, G, 1e-5)
         return self._stats
 
 
@@ -148,140 +156,32 @@ class VAEDecoder(_VAEBlocks):
         # sub-pixel phase weights of conv3x3(nearest2x(.)) for the upsample stages (dk_conv_up_weights)
         self.up_w = {k[:-len(".weight")]: ops.conv_up_weights(v) for k, v in self.p.items()
                      if k.endswith(".upsample.weight")}
-        self.use_fused = os.environ.get("DK_VAE_FUSED", "1") != "0"
-        # where GroupNorm-apply + SiLU runs on the fused path: "1" (default) = inside the convolution, on the staged halo
-        # tile (no normalised tensor in HBM; every halo element is transformed once per CTA that stages it: 2x for the
-        # two halo rows of a 2-row tile, times Cout/128 n-tiles); "0" = one HBM pass of the apply kernel in front of the
-        # fused convolution (which still folds bias / skip / upsample / the next statistics), at the price of more
-        # launches and a normalised tensor in HBM.
-        self.norm_in_conv = os.environ.get("DK_VAE_NORM_IN_CONV", "1") != "0"
-        self.use_cuda_graphs = os.environ.get("DK_CUDA_GRAPHS", "1") != "0"
-        self._shapes: "OrderedDict[tuple, tuple]" = OrderedDict()     # input shape -> (graph, static in, static out, launches)
-        self.max_cached_shapes = int(os.environ.get("DK_MAX_CACHED_SHAPES", "4"))
+        self._shapes = ShapeCache()
+        self.use_cuda_graphs, self.max_cached_shapes = default_settings()
 
-    # ------------------------------------------------------------------ fused building blocks
-    def _fused_ok(self, x, cout):
-        B, H, W, C = x.shape
-        return self.use_fused and ops.conv_fused_supported(H, W, C, cout)
-
-    def _norm_conv(self, x, st: _Stats, norm, conv, res=None):
-        """conv(silu(GroupNorm(x))) (+ res) -> (y, statistics holder of y)"""
-        w, b = self.p[conv + ".weight"], self.p[conv + ".bias"]
-        B, H, W, C = x.shape
-        if self._fused_ok(x, w.shape[0]):
-            part = torch.empty((B, H * W // 128, self.groups, 2), dtype=torch.float32, device=self.device)
-            if self.norm_in_conv:
-                y = ops.conv3x3_fused(x, w, bias=b, res=res, gn=(st.get(), self.p[norm + ".weight"],
-                                                                 self.p[norm + ".bias"], self.groups), silu=True,
-                                      out_partial=part, out_G=self.groups)
-            else:
-                xn = ops.groupnorm_apply(x, st.get(), self.p[norm + ".weight"], self.p[norm + ".bias"], self.groups, True)
-                y = ops.conv3x3_fused(xn, w, bias=b, res=res, out_partial=part, out_G=self.groups)
-            return y, _Stats(self, y, part)
-        xn = ops.groupnorm_apply(x, st.get(), self.p[norm + ".weight"], self.p[norm + ".bias"], self.groups, True)
-        y = ops.conv3x3(xn, w, b, res=res)
-        return y, _Stats(self, y)
-
-    def _resnet_f(self, x, st: _Stats, name):
-        """ResnetBlock2D.__call__ (vae.py:86-101) on the fused path"""
-        y, st1 = self._norm_conv(x, st, name + ".norm1", name + ".conv1")
-        skip = x
-        if (name + ".conv_shortcut.weight") in self.p:
-            B, H, W, C = x.shape
-            skip = self._lin(x.reshape(B * H * W, C), name + ".conv_shortcut").reshape(B, H, W, -1)
-        return self._norm_conv(y, st1, name + ".norm2", name + ".conv2", res=skip)
-
-    def _upsample_conv(self, x, name):
-        """upsample_nearest + conv (vae.py:20-25,146-147)"""
-        w, b = self.p[name + ".weight"], self.p[name + ".bias"]
-        B, H, W, C = x.shape
-        if self._fused_ok(x, w.shape[0]):
-            part = torch.empty((B, 4 * H * W // 128, self.groups, 2), dtype=torch.float32, device=self.device)
-            y = ops.conv3x3_fused(x, self.up_w[name], bias=b, up=True, out_partial=part, out_G=self.groups)
-            return y, _Stats(self, y, part)
-        y = ops.conv3x3(ops.upsample_nearest2x(x), w, b)
-        return y, _Stats(self, y)
-
-    def _attention_f(self, x, st: _Stats, name):
-        B, H, W, C = x.shape
-        S = H * W
-        y = ops.groupnorm_apply(x, st.get(), self.p[name + ".group_norm.weight"], self.p[name + ".group_norm.bias"],
-                                self.groups, False).reshape(B * S, C)
-        q = self._lin(y, name + ".query_proj")
-        k = self._lin(y, name + ".key_proj")
-        v = self._lin(y, name + ".value_proj")
-        o = torch.empty((B * S, C), dtype=self.dtype, device=self.device)
-        scores = torch.empty((S, S), dtype=self.dtype, device=self.device)
-        for b in range(B):
-            sl = slice(b * S, (b + 1) * S)
-            ops.gemm(q[sl], k[sl], out=scores)
-            ops.softmax_rows(scores, 1.0)
-            ops.gemm(scores, v[sl], out=o[sl], w_n_major=True)
-        out = self._lin(o, name + ".out_proj", res=x.reshape(B * S, C)).reshape(B, H, W, C)
-        return out, _Stats(self, out)
-
-    # ------------------------------------------------------------------ forward
-    def _decode_impl(self, x: torch.Tensor) -> torch.Tensor:
-        xin = self._pad_channels(x, self.cin_pad)
-        w_in = self.p["conv_in.weight"]
-        B, H, W, _ = xin.shape
-        if self._fused_ok(xin, w_in.shape[0]):
-            part = torch.empty((B, H * W // 128, self.groups, 2), dtype=torch.float32, device=self.device)
-            h = ops.conv3x3_fused(xin, w_in, bias=self.p["conv_in.bias"], out_partial=part, out_G=self.groups)
-            st = _Stats(self, h, part)
-        else:
-            h = self._conv(xin, "conv_in")
-            st = _Stats(self, h)
-        h, st = self._resnet_f(h, st, "mid_blocks.0")
-        h, st = self._attention_f(h, st, "mid_blocks.1")
-        h, st = self._resnet_f(h, st, "mid_blocks.2")
+    def _decode(self, x: torch.Tensor) -> torch.Tensor:
+        h, st = self._conv(self._pad_channels(x, self.cin_pad), "conv_in")
+        h, st = self._resnet(h, st, "mid_blocks.0")
+        h, st = self._attention(h, st, "mid_blocks.1")
+        h, st = self._resnet(h, st, "mid_blocks.2")
         n = len(self.config.block_out_channels)
         for j in reversed(range(n)):                                  # reversed(self.up_blocks) (vae.py:393)
             for l in range(self.config.layers_per_block):
-                h, st = self._resnet_f(h, st, f"up_blocks.{j}.resnets.{l}")
+                h, st = self._resnet(h, st, f"up_blocks.{j}.resnets.{l}")
             if f"up_blocks.{j}.upsample.weight" in self.p:
-                h, st = self._upsample_conv(h, f"up_blocks.{j}.upsample")             # vae.py:146-147
-        w_out = self.p["conv_out.weight"]                             # 3 real output channels padded to 8
-        if self._fused_ok(h, w_out.shape[0]) and self.norm_in_conv:
-            # conv_norm_out + SiLU + conv_out in the halo-tiled kernel (one narrow 8-channel output tile): the input
-            # crosses L2 -> SM once instead of nine times (the nine-box implicit GEMM ran this layer at 0.9 TB/s)
-            return ops.conv3x3_fused(h, w_out, bias=self.p["conv_out.bias"],
-                                     gn=(st.get(), self.p["conv_norm_out.weight"], self.p["conv_norm_out.bias"],
-                                         self.groups), silu=True)
-        hn = ops.groupnorm_apply(h, st.get(), self.p["conv_norm_out.weight"], self.p["conv_norm_out.bias"], self.groups,
-                                 True)
-        if self._fused_ok(hn, w_out.shape[0]):
-            return ops.conv3x3_fused(hn, w_out, bias=self.p["conv_out.bias"])
-        return self._conv(hn, "conv_out")                             # (B, 8H, 8W, 8) — 3 real channels
+                h, st = self._conv(h, f"up_blocks.{j}.upsample", up=True)             # vae.py:146-147
+        # conv_norm_out + SiLU + conv_out, 3 real output channels padded to 8.  Fused, this is one narrow output tile:
+        # the input crosses L2 -> SM once instead of nine times (the nine-box implicit GEMM ran it at 0.9 TB/s)
+        return self._conv(h, "conv_out", "conv_norm_out", st)[0]
 
     def __call__(self, x: torch.Tensor) -> torch.Tensor:
         """x (B, H, W, 16) NHWC -> (B, 8H, 8W, 3) NHWC view (channel stride 1, pixel stride 8)."""
         if x.dim() != 4:
             raise ValueError(f"VAEDecoder expects NHWC rank-4 input, got rank {x.dim()}")
         x = x.to(device=self.device, dtype=self.dtype).contiguous()
-        if not self.use_cuda_graphs:
-            return self._decode_impl(x)[..., : self.config.out_channels]
-        key = tuple(x.shape)
-        entry = self._shapes.get(key)
-        if entry is None:
-            while len(self._shapes) >= max(1, self.max_cached_shapes):
-                self._shapes.popitem(last=False)
-            sx = x.clone()
-            self._decode_impl(sx)                                     # eager warm-up (function attributes, allocator)
-            torch.cuda.current_stream(self.device).synchronize()
-            n0 = ops.launch_count()
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                so = self._decode_impl(sx)
-            entry = (graph, sx, so, ops.launch_count() - n0)
-            self._shapes[key] = entry
-        else:
-            self._shapes.move_to_end(key)
-        graph, sx, so, n_launch = entry
-        sx.copy_(x)
-        graph.replay()
-        ops.note_graph_launches(n_launch)
-        return so[..., : self.config.out_channels]
+        st = self._shapes.state(tuple(x.shape), self.max_cached_shapes)
+        y = self._shapes.run(st, self.use_cuda_graphs, self._decode, x)
+        return y[..., : self.config.out_channels]
 
 
 class VAEEncoder(_VAEBlocks):
@@ -290,6 +190,8 @@ class VAEEncoder(_VAEBlocks):
     (load_vae_encoder(float16=False), __init__.py:116); here it runs in the pipeline's 16-bit activation type with fp32
     accumulation (DESIGN.md §7)."""
 
+    fuse = False            # the fused convolution would change the encoder's outputs: it keeps the unfused kernels
+
     def __init__(self, params: Dict[str, torch.Tensor], config: VAEEncoderConfig = VAEEncoderConfig(), device=None):
         super().__init__(params, config, device)
         self.cin_pad = 64
@@ -297,19 +199,19 @@ class VAEEncoder(_VAEBlocks):
 
     def encode_hidden(self, x16: torch.Tensor) -> torch.Tensor:
         """x16 (B, H, W, cin_pad) 16-bit NHWC in [-1, 1] -> hidden (B, H/8, W/8, 32) = (mean | logvar)"""
-        h = self._conv(x16, "conv_in")
+        h, st = self._conv(x16, "conv_in")
         n = len(self.config.block_out_channels)
         for i in range(n):
             for l in range(self.config.layers_per_block):
-                h = self._resnet(h, f"down_blocks.{i}.resnets.{l}")
+                h, st = self._resnet(h, st, f"down_blocks.{i}.resnets.{l}")
             if f"down_blocks.{i}.downsample.weight" in self.p:        # pad (0,1),(0,1) + stride 2 (vae.py:142-144)
                 h = ops.conv3x3_s2(h, self.p[f"down_blocks.{i}.downsample.weight"],
                                    self.p[f"down_blocks.{i}.downsample.bias"])
-        h = self._resnet(h, "mid_blocks.0")
-        h = self._attention(h, "mid_blocks.1")
-        h = self._resnet(h, "mid_blocks.2")
-        h = self._gn(h, "conv_norm_out", True)
-        return self._conv(h, "conv_out")
+                st = _Stats(h, self.groups)
+        h, st = self._resnet(h, st, "mid_blocks.0")
+        h, st = self._attention(h, st, "mid_blocks.1")
+        h, st = self._resnet(h, st, "mid_blocks.2")
+        return self._conv(h, "conv_out", "conv_norm_out", st)[0]
 
     def __call__(self, image: torch.Tensor) -> torch.Tensor:
         """image: uint8 NHWC (B, H, W, >=3) on the device, or a 16/32-bit float NHWC (B, H, W, 3) already in [-1, 1]."""

@@ -718,16 +718,6 @@ def check_vae_decode_512_vs_oracle():
     return _vae_case(torch.bfloat16, 1, (64, 64), 35.0)
 
 
-def check_vae_decode_512_norm_pass():
-    """the same 512 x 512 decode with GroupNorm-apply + SiLU as one HBM pass in front of each fused convolution
-    (DK_VAE_NORM_IN_CONV=0; the default runs them inside the convolutions, on the staged halo tiles)"""
-    os.environ["DK_VAE_NORM_IN_CONV"] = "0"
-    try:
-        return _vae_case(torch.bfloat16, 1, (64, 64), 35.0)
-    finally:
-        os.environ.pop("DK_VAE_NORM_IN_CONV", None)
-
-
 def check_vae_decode_1024_vs_oracle():
     """the BASELINE decode: 1024 x 1024 (latent 128^2, mid attention over S = 16384) against the fp32 oracle"""
     return _vae_case(torch.bfloat16, 1, (128, 128), 35.0)
@@ -775,4 +765,4 @@ ALL_CHECKS = [check_mmdit_flux_tiny, check_mmdit_sd3_tiny, check_product_vs_refe
               check_pipeline_img2img, check_pipeline_flux_tiny, check_pipeline_sd3_cfg_tiny,
               check_pipeline_errors, check_pipeline_local_ckpt, check_full_size_flux_properties, check_full_size_vae_properties,
               check_fullwidth_flux_vs_oracle, check_fullwidth_flux_dev_len_vs_oracle, check_fullwidth_sd3_vs_oracle,
-              check_vae_decode_512_vs_oracle, check_vae_decode_512_norm_pass, check_vae_decode_1024_vs_oracle]
+              check_vae_decode_512_vs_oracle, check_vae_decode_1024_vs_oracle]
