@@ -1,7 +1,8 @@
 """GPU checks of the individual sm_90a kernels against plain fp32 torch references of the same op.
 
 Each check_* function is self-contained (used by tests/test_kernels_gpu.py and by tools/run_gpu_checks.py, which
-runs every check in its own process so that one trapped kernel cannot poison the others).
+runs every check in its own process so that one trapped kernel cannot poison the others).  A check runs a table of
+cases; every case of an op, small or full-size, is compared with that op's one ref_* function.
 Tolerances: 16-bit outputs, fp32 accumulation -> relative L2 error <= 4e-3 (bf16 epsilon is 3.9e-3 per element,
 the L2 over many elements averages to ~2e-3); attention <= 1e-2.
 """
@@ -12,9 +13,10 @@ import numpy as np
 import torch
 
 from diffusionkit_b200 import ops
-from diffusionkit_b200._lib import ACT_GELU_ERF, ACT_NONE, ACT_SILU
+from diffusionkit_b200._lib import ACT_GELU_ERF, ACT_NONE, ACT_QUICK_GELU, ACT_SILU
 
 DEV = "cuda:0"
+bf16, fp16 = torch.bfloat16, torch.float16
 
 
 def _setup():
@@ -50,140 +52,225 @@ def _rand(shape, dtype, scale=1.0):
     return (torch.randn(shape, device=DEV, dtype=torch.float32) * scale).to(dtype)
 
 
-# ------------------------------------------------------------------------------------------------ GEMM
-def _gemm_case(M, N, K, dtype, bias=False, act=ACT_NONE, gate=False, res=False, remap=False, name=""):
-    A = _rand((M, K), dtype)
-    W = _rand((N, K), dtype, 1.0 / math.sqrt(K))
-    b = _rand((N,), dtype, 0.5) if bias else None
-    ref = A.float() @ W.float().t()
-    if bias:
-        ref = ref + b.float()
+# ------------------------------------------------------------------------------------------------ fp32 references
+def ref_gemm(A, W, bias=None, act=ACT_NONE, gate=None, res=None):
+    """res + gate * act(A @ W^T + bias) in fp32.  W is [N, K]; gate is [G, N], row g gating the g-th of G equal row
+    batches.  The product runs in row chunks: the fp32 copy of a 16384 x 12288 output alone is 805 MB."""
+    Wt = W.float().t().contiguous()
+    y = torch.cat([A[i:i + 4096].float() @ Wt for i in range(0, A.shape[0], 4096)], 0)
+    if bias is not None:
+        y += bias.float()
     if act == ACT_GELU_ERF:
-        ref = torch.nn.functional.gelu(ref)
+        y = torch.nn.functional.gelu(y)
     elif act == ACT_SILU:
-        ref = torch.nn.functional.silu(ref)
-    kw = {}
-    out = None
-    if remap:
-        # M = Bt * rpb rows scattered into a [Bt * out_rows, N] buffer at row offset off
-        Bt = 2
-        assert M % Bt == 0
-        rpb = M // Bt
-        out_rows, off = rpb + 40, 24
-        out = torch.zeros((Bt * out_rows, N), dtype=dtype, device=DEV)
-        kw.update(rows_per_batch=rpb, out_batch_rows=out_rows, out_row_off=off)
-        g = _rand((Bt, N), dtype) if gate else None
-        r = _rand((Bt * rpb, N), dtype) if res else None
-        if gate:
-            ref = ref * g.float().repeat_interleave(rpb, 0)
-        if res:
-            ref = ref + r.float()
-        got = ops.gemm(A, W, out=out, bias=b, act=act, gate=g, res=r, **kw)
-        got_rows = torch.cat([got[i * out_rows + off:i * out_rows + off + rpb] for i in range(Bt)], 0)
-        untouched = torch.cat([got[i * out_rows:i * out_rows + off] for i in range(Bt)], 0)
-        assert float(untouched.float().abs().max()) == 0.0, f"{name}: rows outside the remap window were written"
-        return _assert_close(name, got_rows, ref, 4e-3)
-    g = _rand((1, N), dtype) if gate else None
-    r = _rand((M, N), dtype) if res else None
-    if gate:
-        ref = ref * g.float()
-    if res:
-        ref = ref + r.float()
-    got = ops.gemm(A, W, bias=b, act=act, gate=g, res=r)
+        y = torch.nn.functional.silu(y)
+    elif act == ACT_QUICK_GELU:
+        y = y * torch.sigmoid(1.702 * y)
+    if gate is not None:
+        y = (y.reshape(gate.shape[0], -1, y.shape[1]) * gate.float()[:, None]).reshape(y.shape)
+    if res is not None:
+        y += res.float()
+    return y
+
+
+def ref_qk_norm_rope(y, pos, heads, d, q_w, k_w, rope, round_to=None, eps=1e-6):
+    """QK-RMSNorm + RoPE in fp32 on the q and k thirds of a packed [rows, 3 * heads * d] y; v passes through.
+    q_w / k_w: [d] or per-row [rows, 1, d] norm weights, None skips the norm.  rope[pos[row]]: the row's (cos, sin)
+    pairs, None skips the rotation.  round_to: the 16-bit type the unfused dk_qk_norm_rope stores the normalised value
+    in before it rotates it; the fused GEMM epilogue rotates it unrounded (None)."""
+    h = heads * d
+    y = y.float()
+    ref = y.clone()
+    for which, w in enumerate([q_w, k_w]):
+        t = y[:, which * h:(which + 1) * h].reshape(-1, heads, d)
+        if w is not None:
+            t = t * torch.rsqrt((t * t).mean(-1, keepdim=True) + eps) * w.float()
+            if round_to is not None:
+                t = t.to(round_to).float()
+        if rope is not None:
+            c, sn = rope[pos][:, None, :, 0], rope[pos][:, None, :, 1]
+            x0, x1 = t[..., 0::2], t[..., 1::2]
+            t = torch.stack([x0 * c - x1 * sn, x0 * sn + x1 * c], dim=-1).reshape(-1, heads, d)
+        ref[:, which * h:(which + 1) * h] = t.reshape(-1, h)
+    return ref
+
+
+def ref_attention(qkv, B, S, heads, d):
+    """softmax(q k^T / sqrt(d)) v in fp32 for a packed [B * S, 3 * heads * d] qkv -> [B * S, heads * d], one head at a
+    time (a 4685^2 fp32 score matrix is 88 MB)"""
+    h = heads * d
+    x = qkv.reshape(B, S, 3, heads, d)
+    ref = torch.empty((B, S, h), dtype=torch.float32, device=qkv.device)
+    for b in range(B):
+        for hd in range(heads):
+            q, k, v = x[b, :, 0, hd].float(), x[b, :, 1, hd].float(), x[b, :, 2, hd].float()
+            ref[b, :, hd * d:(hd + 1) * d] = torch.softmax(q @ k.t() / math.sqrt(d), dim=-1) @ v
+    return ref.reshape(B * S, h)
+
+
+def ref_conv3x3(x, w, b, res=None):
+    """3x3 convolution, zero padding 1, of NHWC x with w [Cout, 3, 3, Cin] + b (+ res) in fp32.  It runs in horizontal
+    bands with a one-row halo, so a full-size image needs little fp32 scratch."""
+    B, H, W, Cin = x.shape
+    Cout = w.shape[0]
+    wf = w.float().permute(0, 3, 1, 2).contiguous()
+    ref = torch.empty((B, H, W, Cout), dtype=torch.float32, device=x.device)
+    rows = max(8, (1 << 24) // (W * max(Cin, Cout)))
+    for i in range(B):
+        for y0 in range(0, H, rows):
+            y1 = min(H, y0 + rows)
+            xin = x[i, max(0, y0 - 1):min(H, y1 + 1)].float().permute(2, 0, 1)[None]
+            xin = torch.nn.functional.pad(xin, (1, 1, 1 if y0 == 0 else 0, 1 if y1 == H else 0))
+            ref[i, y0:y1] = torch.nn.functional.conv2d(xin, wf, b.float())[0].permute(1, 2, 0)
+    if res is not None:
+        ref += res.float()
+    return ref
+
+
+def ref_groupnorm_silu(x, gamma, beta, G=32, eps=1e-5):
+    """GroupNorm(G) + SiLU of NHWC x, one image at a time, with float64 statistics.  The normalised, affine value is
+    rounded to x's 16-bit type before the SiLU, as dk_groupnorm_apply and the fused convolution round it.
+    Returns (y fp32, mean [B, G], rstd [B, G])."""
+    B, Cc = x.shape[0], x.shape[-1]
+    y = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    mean = torch.empty((B, G), dtype=torch.float64, device=x.device)
+    var = torch.empty_like(mean)
+    for i in range(B):
+        xg = x[i].reshape(-1, G, Cc // G)
+        xd = xg.double()
+        mean[i], var[i] = xd.mean(dim=(0, 2)), xd.var(dim=(0, 2), unbiased=False)
+        del xd
+        xn = (xg.float() - mean[i].float()[None, :, None]) * torch.rsqrt(var[i] + eps).float()[None, :, None]
+        y[i] = torch.nn.functional.silu((xn.reshape(x[i].shape) * gamma.float() + beta.float()).to(x.dtype).float())
+    return y, mean.float(), torch.rsqrt(var + eps).float()
+
+
+# ------------------------------------------------------------------------------------------------ GEMM
+def _gemm_case(M, N, K, dtype, epi="", block_tol=None):
+    """dk_gemm vs ref_gemm.  epi lists the epilogue terms: bias, gelu | silu | quick_gelu, gate, res (out of place),
+    inplace (residual read from and written to the output), remap (two batches of M / 2 rows scattered at row offset
+    24 into 40-row-padded batches), window (a column window of a wider buffer, the FLUX single-block concat buffer),
+    n_major (W given as [K, N]).  Bytes of a remap / window buffer outside the output must keep their sentinel."""
+    e = set(epi.split())
+    act = (ACT_GELU_ERF if "gelu" in e else ACT_SILU if "silu" in e else ACT_QUICK_GELU if "quick_gelu" in e
+           else ACT_NONE)
+    Bt = 2 if "remap" in e else 1
+    A = _rand((M, K), dtype)
+    W = _rand((K, N) if "n_major" in e else (N, K), dtype, 1 / math.sqrt(K))
+    b = _rand((N,), dtype, 0.5) if "bias" in e else None
+    g = _rand((Bt, N), dtype) if "gate" in e else None
+    r = _rand((M, N), dtype) if e & {"res", "inplace"} else None
+    ref = ref_gemm(A, W.t() if "n_major" in e else W, b, act, g, r)
+    name = f"gemm_{M}x{N}x{K}_{str(dtype)[6:]}_{'_'.join(epi.split()) or 'plain'}"
+    out, buf, kw = (r if "inplace" in e else None), None, {}
+    if "remap" in e:
+        rpb, out_rows, off = M // Bt, M // Bt + 40, 24
+        buf = out = torch.full((Bt * out_rows, N), 7.0, dtype=dtype, device=DEV)
+        rows = torch.cat([torch.arange(i * out_rows + off, i * out_rows + off + rpb) for i in range(Bt)]).to(DEV)
+        window = (rows, slice(0, N))
+        kw = dict(rows_per_batch=rpb, out_batch_rows=out_rows, out_row_off=off)
+    elif "window" in e:
+        buf = torch.full((M + 8, 1024), 7.0, dtype=dtype, device=DEV)
+        window = (slice(0, M), slice(256, 256 + N))
+        out = buf[window]
+    got = ops.gemm(A, W, out=out, bias=b, act=act, gate=g, res=r, w_n_major="n_major" in e, **kw)
+    if buf is not None:
+        got = buf[window]
+        outside = torch.ones(buf.shape, dtype=torch.bool, device=DEV)
+        outside[window] = False
+        assert bool((buf[outside] == 7.0).all()), f"{name}: bytes outside the output window were written"
+    if block_tol is not None:
+        return _assert_close_blocks(name, got, ref, 4e-3, block_tol)
     return _assert_close(name, got, ref, 4e-3)
+
+
+def _gemm_table(cases):
+    _setup()
+    return {f"{M}x{N}x{K}_{epi}": _gemm_case(M, N, K, dt, epi) for (M, N, K, dt, epi) in cases}
 
 
 def check_gemm_single_tile():
     _setup()
-    return {"err": _gemm_case(128, 256, 64, torch.bfloat16, name="gemm_128x256x64")}
+    return {"err": _gemm_case(128, 256, 64, bf16)}
 
 
 def check_gemm_multi_k():
     _setup()
-    return {"err": _gemm_case(128, 256, 512, torch.bfloat16, name="gemm_128x256x512")}
+    return {"err": _gemm_case(128, 256, 512, bf16)}
+
+
+def check_gemm_one_m_pair():
+    """M = 256: one m-block pair, so both CTAs of a cluster own rows and share the W tile; one and several K steps"""
+    return _gemm_table([(256, 256, 64, bf16, ""), (256, 512, 512, bf16, "")])
 
 
 def check_gemm_shapes():
-    _setup()
-    out = {}
-    for (M, N, K) in [(256, 512, 256), (300, 264, 200), (77, 64, 64), (1000, 3072, 1536), (20, 1024, 3072),
-                      (4352, 768, 3072), (128, 128, 128)]:
-        out[f"{M}x{N}x{K}"] = _gemm_case(M, N, K, torch.bfloat16, name=f"gemm_{M}x{N}x{K}")
-    return out
+    """ragged M / N / K, tiny and tall problems"""
+    return _gemm_table([(256, 512, 256, bf16, ""), (300, 264, 200, bf16, ""), (77, 64, 64, bf16, ""),
+                        (1000, 3072, 1536, bf16, ""), (20, 1024, 3072, bf16, ""), (4352, 768, 3072, bf16, ""),
+                        (128, 128, 128, bf16, "")])
 
 
 def check_gemm_persistent_large():
-    _setup()
-    # more tiles than SMs: exercises more than one wave of CTAs and the smem ring wrap-around
-    return {"err": _gemm_case(4096, 4608, 1024, torch.bfloat16, bias=True, name="gemm_4096x4608x1024")}
+    """more tiles than SMs: more than one wave of clusters and the smem ring wrap-around"""
+    return _gemm_table([(4096, 4608, 1024, bf16, "bias"), (8192, 4608, 1024, bf16, "bias"),
+                        (4096, 3072, 512, bf16, "bias")])
 
 
 def check_gemm_epilogues():
-    _setup()
-    out = {}
-    out["bias"] = _gemm_case(384, 512, 256, torch.bfloat16, bias=True, name="gemm_bias")
-    out["gelu"] = _gemm_case(384, 512, 256, torch.bfloat16, bias=True, act=ACT_GELU_ERF, name="gemm_gelu")
-    out["silu"] = _gemm_case(384, 512, 256, torch.bfloat16, bias=True, act=ACT_SILU, name="gemm_silu")
-    out["gate_res"] = _gemm_case(384, 512, 256, torch.bfloat16, bias=True, gate=True, res=True, name="gemm_gate_res")
-    out["remap"] = _gemm_case(600, 512, 256, torch.bfloat16, bias=True, gate=True, res=True, remap=True,
-                              name="gemm_remap")
-    return out
+    return _gemm_table([(384, 512, 256, bf16, "bias"), (384, 512, 256, bf16, "bias gelu"),
+                        (384, 512, 256, bf16, "bias silu"), (384, 512, 256, bf16, "bias gate res"),
+                        (600, 512, 256, bf16, "bias gate res remap"), (77, 512, 256, bf16, "bias quick_gelu")])
+
+
+def check_gemm_gate_residual():
+    """bias + gate + residual on multi-tile problems, one with N = 1152 (not a multiple of the 256-wide tile)"""
+    return _gemm_table([(1024, 1152, 256, bf16, "bias gate res"), (2048, 1536, 512, bf16, "bias gate res")])
+
+
+def check_gemm_output_window():
+    """GELU output into a column window of a wider buffer (the FLUX single-block concat buffer), M and N not tile
+    multiples: every byte left, right and below the window keeps its sentinel"""
+    return _gemm_table([(1000, 520, 256, bf16, "gelu window")])
 
 
 def check_gemm_fp16():
-    _setup()
-    return {"err": _gemm_case(300, 512, 320, torch.float16, bias=True, act=ACT_GELU_ERF, name="gemm_fp16")}
+    return _gemm_table([(300, 512, 320, fp16, "bias gelu"), (300, 512, 320, fp16, "bias")])
 
 
 def check_gemm_inplace_residual():
-    _setup()
-    M, N, K = 256, 256, 128
-    A = _rand((M, K), torch.bfloat16)
-    W = _rand((N, K), torch.bfloat16, 1 / math.sqrt(K))
-    x = _rand((M, N), torch.bfloat16)
-    ref = x.float() + A.float() @ W.float().t()
-    got = ops.gemm(A, W, out=x, res=x)
-    return {"err": _assert_close("gemm_inplace", got, ref, 4e-3)}
+    return _gemm_table([(256, 256, 128, bf16, "inplace"), (1000, 520, 256, bf16, "gate inplace")])
 
 
 def check_gemm_w_n_major():
-    _setup()
-    out = {}
-    for (M, N, K) in [(128, 128, 64), (256, 384, 256), (200, 136, 72)]:
-        A = _rand((M, K), torch.bfloat16)
-        Wt = _rand((K, N), torch.bfloat16, 1 / math.sqrt(K))  # [K, N] row-major
-        ref = A.float() @ Wt.float()
-        got = ops.gemm(A, Wt, w_n_major=True)
-        out[f"{M}x{N}x{K}"] = _assert_close(f"gemm_nmajor_{M}x{N}x{K}", got, ref, 4e-3)
-    return out
+    return _gemm_table([(128, 128, 64, bf16, "n_major"), (256, 384, 256, bf16, "n_major"),
+                        (200, 136, 72, bf16, "n_major")])
 
 
 # ------------------------------------------------------------------------------------------------ conv
-def _conv_case(B, H, W, Cin, Cout, dtype, bias=True, res=False, name=""):
+def _conv_case(B, H, W, Cin, Cout, dtype, res=False, block_tol=None):
     x = _rand((B, H, W, Cin), dtype)
     w = _rand((Cout, 3, 3, Cin), dtype, 1 / math.sqrt(9 * Cin))
-    b = _rand((Cout,), dtype, 0.5) if bias else None
+    b = _rand((Cout,), dtype, 0.5)
     r = _rand((B, H, W, Cout), dtype) if res else None
-    ref = torch.nn.functional.conv2d(x.float().permute(0, 3, 1, 2), w.float().permute(0, 3, 1, 2),
-                                     b.float() if bias else None, padding=1).permute(0, 2, 3, 1)
-    if res:
-        ref = ref + r.float()
+    ref = ref_conv3x3(x, w, b, r)
     got = ops.conv3x3(x, w, bias=b, res=r)
+    name = f"conv_{B}x{H}x{W}_{Cin}to{Cout}_{str(dtype)[6:]}" + ("_res" if res else "")
+    if block_tol is not None:
+        return _assert_close_blocks(name, got.reshape(-1, Cout), ref.reshape(-1, Cout), 4e-3, block_tol,
+                                    bc=min(128, Cout))
     return _assert_close(name, got, ref, 4e-3)
 
 
 def check_conv3x3():
     _setup()
-    out = {}
-    out["16x16"] = _conv_case(2, 16, 16, 64, 64, torch.bfloat16, name="conv_16x16")
-    out["8x32_res"] = _conv_case(1, 8, 32, 128, 128, torch.bfloat16, res=True, name="conv_8x32")
-    out["12x20_ragged"] = _conv_case(2, 12, 20, 64, 72, torch.bfloat16, name="conv_12x20")
-    out["64x256"] = _conv_case(1, 64, 256, 128, 256, torch.bfloat16, res=True, name="conv_64x256")
-    out["fp16"] = _conv_case(1, 32, 32, 64, 16, torch.float16, name="conv_fp16")
-    return out
+    return {f"{B}x{H}x{W}_{Cin}to{Cout}": _conv_case(B, H, W, Cin, Cout, dt, res)
+            for (B, H, W, Cin, Cout, dt, res) in [(2, 16, 16, 64, 64, bf16, False), (1, 8, 32, 128, 128, bf16, True),
+                                                  (2, 12, 20, 64, 72, bf16, False), (1, 64, 256, 128, 256, bf16, True),
+                                                  (1, 32, 32, 64, 16, fp16, False)]}
 
 
-def _conv_s2_case(B, H, W, Cin, Cout, dtype, name=""):
+def _conv_s2_case(B, H, W, Cin, Cout, dtype):
     x = _rand((B, H, W, Cin), dtype)
     w = _rand((Cout, 3, 3, Cin), dtype, 1 / math.sqrt(9 * Cin))
     b = _rand((Cout,), dtype, 0.5)
@@ -192,19 +279,18 @@ def _conv_s2_case(B, H, W, Cin, Cout, dtype, name=""):
     ref = torch.nn.functional.conv2d(xp, w.float().permute(0, 3, 1, 2), b.float(), stride=2).permute(0, 2, 3, 1)
     got = ops.conv3x3_s2(x, w, bias=b)
     assert got.shape == (B, H // 2, W // 2, Cout)
-    return _assert_close(name, got, ref, 4e-3)
+    return _assert_close(f"convs2_{B}x{H}x{W}_{Cin}to{Cout}_{str(dtype)[6:]}", got, ref, 4e-3)
 
 
 def check_conv3x3_s2():
     """the encoder's stride-2 downsample: same implicit-GEMM kernel, TMA box with element stride 2"""
     _setup()
-    out = {}
-    out["32x32"] = _conv_s2_case(2, 32, 32, 64, 64, torch.bfloat16, name="convs2_32x32")          # TW=16, TH=8
-    out["16x64"] = _conv_s2_case(1, 16, 64, 128, 128, torch.bfloat16, name="convs2_16x64")        # TW=32, TH=4
-    out["24x40_ragged"] = _conv_s2_case(2, 24, 40, 64, 72, torch.bfloat16, name="convs2_24x40")   # TW=128 ragged
-    out["64x512"] = _conv_s2_case(1, 64, 512, 128, 128, torch.bfloat16, name="convs2_64x512")     # box 256 wide
-    out["fp16"] = _conv_s2_case(1, 32, 32, 64, 16, torch.float16, name="convs2_fp16")
-    return out
+    return {f"{B}x{H}x{W}_{Cin}to{Cout}": _conv_s2_case(B, H, W, Cin, Cout, dt)
+            for (B, H, W, Cin, Cout, dt) in [(2, 32, 32, 64, 64, bf16),        # TW=16, TH=8
+                                             (1, 16, 64, 128, 128, bf16),      # TW=32, TH=4
+                                             (2, 24, 40, 64, 72, bf16),        # TW=128 ragged
+                                             (1, 64, 512, 128, 128, bf16),     # box 256 wide
+                                             (1, 32, 32, 64, 16, fp16)]}
 
 
 def check_img2img_kernels():
@@ -255,9 +341,8 @@ def check_dequant_q4():
 
 
 def check_text_kernels():
-    """csrc/text.cu: embedding, LayerNorm(affine), T5 RMSNorm over fp32, fp32 += 16-bit, gated GELU, quick-GELU epilogue"""
-    from diffusionkit_b200._lib import ACT_QUICK_GELU
-
+    """csrc/text.cu: embedding, LayerNorm(affine), T5 RMSNorm over fp32, fp32 += 16-bit, gated GELU (the quick-GELU GEMM
+    epilogue is a row of check_gemm_epilogues)"""
     _setup()
     out = {}
     for dt in (torch.bfloat16, torch.float16):
@@ -281,11 +366,6 @@ def check_text_kernels():
     hgl = _rand((33, 2 * 512), torch.bfloat16, 2.0)
     ref = torch.nn.functional.gelu(hgl.float()[:, :512]) * hgl.float()[:, 512:]
     out["glu"] = _assert_close("glu_gelu", ops.glu_gelu(hgl), ref, 4e-3)
-    a, wq = _rand((77, 256), torch.bfloat16), _rand((512, 256), torch.bfloat16, 1 / 16)
-    bq = _rand((512,), torch.bfloat16, 0.5)
-    z = a.float() @ wq.float().t() + bq.float()
-    out["quick_gelu"] = _assert_close("gemm_quick_gelu", ops.gemm(a, wq, bias=bq, act=ACT_QUICK_GELU),
-                                      z * torch.sigmoid(1.702 * z), 4e-3)
     return out
 
 
@@ -325,115 +405,72 @@ def check_attention_small():
 
 
 # ------------------------------------------------------------------------------------------------ attention
-def _attention_case(B, S, heads, d, dtype, split=None, name=""):
+def _attention_case(B, S, heads, d, dtype, split=None, out1_pad=64, block_tol=None, twice=False):
+    """dk_attention_fwd vs ref_attention.  With a split, rows >= split of each sequence go to out1, a view whose rows
+    are out1_pad elements longer than heads * d.  twice: a second launch on the same input must be bit-identical to
+    the first (the K/V steps and the quad reductions run in a fixed order)."""
     h = heads * d
     qkv = _rand((B * S, 3 * h), dtype)
-    q, k, v = [t.reshape(B, S, heads, d).permute(0, 2, 1, 3).float() for t in qkv.split(h, dim=1)]
-    ref = torch.softmax(q @ k.transpose(-1, -2) / math.sqrt(d), dim=-1) @ v
-    ref = ref.permute(0, 2, 1, 3).reshape(B, S, h)
-    if split is None:
-        out = torch.zeros((B * S, h), dtype=dtype, device=DEV)
-        ops.attention(qkv, B, S, heads, d, out)
-        got = out.reshape(B, S, h)
-    else:
+
+    def launch():
+        if split is None:
+            out = torch.zeros((B * S, h), dtype=dtype, device=DEV)
+            ops.attention(qkv, B, S, heads, d, out)
+            return out
         o0 = torch.zeros((B * split, h), dtype=dtype, device=DEV)
-        o1 = torch.zeros((B * (S - split), h + 64), dtype=dtype, device=DEV)[:, :h]  # non-trivial leading dim
+        o1 = torch.zeros((B * (S - split), h + out1_pad), dtype=dtype, device=DEV)[:, :h]
         ops.attention(qkv, B, S, heads, d, o0, split=split, out1=o1)
-        got = torch.cat([o0.reshape(B, split, h), o1.reshape(B, S - split, h)], dim=1)
+        return torch.cat([o0.reshape(B, split, h), o1.reshape(B, S - split, h)], dim=1).reshape(B * S, h)
+
+    name = f"att_d{d}_{B}x{S}x{heads}_{str(dtype)[6:]}" + (f"_split{split}" if split is not None else "")
+    got = launch()
+    if twice:
+        assert torch.equal(got, launch()), f"{name}: two launches on the same input differ"
+    ref = ref_attention(qkv, B, S, heads, d)
+    if block_tol is not None:
+        return _assert_close_blocks(name, got, ref, 1e-2, block_tol, bc=d)
     return _assert_close(name, got, ref, 1e-2)
+
+
+def _attention_table(cases):
+    _setup()
+    return {f"{B}x{S}x{heads}_split{split}": _attention_case(B, S, heads, d, dt, split)
+            for (B, S, heads, d, dt, split) in cases}
 
 
 def check_attention_d128_one_tile():
     _setup()
-    return {"err": _attention_case(1, 128, 1, 128, torch.bfloat16, name="att_d128_S128")}
+    return {"err": _attention_case(1, 128, 1, 128, bf16)}
 
 
 def check_attention_d128():
-    _setup()
-    out = {}
-    out["S300"] = _attention_case(2, 300, 2, 128, torch.bfloat16, name="att_d128_S300")
-    out["S1280_split"] = _attention_case(1, 1280, 3, 128, torch.bfloat16, split=256, name="att_d128_S1280")
-    return out
+    return _attention_table([(2, 300, 2, 128, bf16, None), (1, 1280, 3, 128, bf16, 256)])
 
 
 def check_attention_d64():
+    return _attention_table([(1, 128, 1, 64, fp16, None), (2, 1178, 2, 64, fp16, 1024), (1, 333, 2, 64, bf16, None)])
+
+
+def check_attention_short():
+    """a half-filled K/V tile and two full ones"""
+    return _attention_table([(1, 64, 1, 128, bf16, None), (1, 256, 2, 128, bf16, None)])
+
+
+def check_attention_long():
+    """many K/V steps with a ragged last tile, with and without split outputs"""
+    return _attention_table([(2, 1300, 2, 128, bf16, 1024), (1, 4400, 2, 128, bf16, None)])
+
+
+def check_attention_many_ctas():
+    """more (batch, head, query tile) work items than SMs, at both head dims"""
+    return _attention_table([(3, 700, 24, 128, bf16, 100), (2, 1500, 24, 64, fp16, 1024)])
+
+
+def check_attention_determinism():
+    """long ragged sequences at both head dims: a second launch on the same input is bit-identical to the first"""
     _setup()
-    out = {}
-    out["S128"] = _attention_case(1, 128, 1, 64, torch.float16, name="att_d64_S128")
-    out["S1178_split"] = _attention_case(2, 1178, 2, 64, torch.float16, split=1024, name="att_d64_S1178")
-    out["bf16_S333"] = _attention_case(1, 333, 2, 64, torch.bfloat16, name="att_d64_S333")
-    return out
-
-
-def check_attention_v3_explicit():
-    """split outputs with a ragged tail at d = 64 (fp16 and bf16), two batches at d = 128, rescale"""
-    _setup()
-    out = {"d64_S1178_split": _attention_case(2, 1178, 2, 64, torch.float16, split=1024, name="att3_d64_S1178"),
-           "d64_S333": _attention_case(1, 333, 2, 64, torch.bfloat16, name="att3_d64_S333"),
-           "d128_S300": _attention_case(2, 300, 2, 128, torch.bfloat16, name="att3_d128_S300")}
-    out["rescale"] = check_attention_large_scores()["err"]
-    return out
-
-
-def check_attention_v3_variants():
-    """long ragged sequences at both head dims against the fp32 reference, and the kernel is deterministic: a second
-    launch on the same input is bit-identical to the first (the K/V steps and the quad reductions run in a fixed order)"""
-    _setup()
-    out = {}
-    for d, dt, S in ((128, torch.bfloat16, 1300), (64, torch.float16, 1178)):
-        name = f"att_d{d}_S{S}"
-        out[name] = _attention_case(2, S, 2, d, dt, split=1024, name=name)
-        qkv = _rand((2 * S, 3 * 2 * d), dt)
-        o1 = torch.zeros((2 * S, 2 * d), dtype=dt, device=DEV)
-        o2 = torch.zeros((2 * S, 2 * d), dtype=dt, device=DEV)
-        ops.attention(qkv, 2, S, 2, d, o1)
-        ops.attention(qkv, 2, S, 2, d, o2)
-        assert torch.equal(o1, o2), f"{name}: two launches on the same input differ"
-    return out
-
-
-def check_attention_v3s_kernel():
-    """one full K/V tile, ragged tails, split outputs at both head dims, a one-token sequence, rescale"""
-    _setup()
-    out = {"d128_S128": _attention_case(1, 128, 1, 128, torch.bfloat16, name="att3s_d128_S128"),
-           "d128_S300": _attention_case(2, 300, 2, 128, torch.bfloat16, name="att3s_d128_S300"),
-           "d128_S1280_split": _attention_case(1, 1280, 3, 128, torch.bfloat16, split=256, name="att3s_d128_S1280"),
-           "d64_S1178_split": _attention_case(2, 1178, 2, 64, torch.float16, split=1024, name="att3s_d64_S1178"),
-           "S1": _attention_case(2, 1, 2, 128, torch.bfloat16, name="att3s_S1")}
-    out["rescale"] = check_attention_large_scores()["err"]
-    return out
-
-
-def check_attention_v5_kernel():
-    """more CTAs than SMs, odd/even K/V tile counts, tails, both head dims, split outputs, rescale"""
-    _setup()
-    out = {"d128_S128": _attention_case(1, 128, 1, 128, torch.bfloat16, name="att5_d128_S128"),
-           "d128_S256": _attention_case(1, 256, 2, 128, torch.bfloat16, name="att5_d128_S256"),
-           "d128_S300": _attention_case(2, 300, 2, 128, torch.bfloat16, name="att5_d128_S300"),
-           "d128_S1280_split": _attention_case(1, 1280, 3, 128, torch.bfloat16, split=256, name="att5_d128_S1280"),
-           "d64_S1178_split": _attention_case(2, 1178, 2, 64, torch.float16, split=1024, name="att5_d64_S1178"),
-           "d64_S333": _attention_case(1, 333, 2, 64, torch.bfloat16, name="att5_d64_S333"),
-           "S1": _attention_case(2, 1, 2, 128, torch.bfloat16, name="att5_S1"),
-           "many_items": _attention_case(3, 700, 24, 128, torch.bfloat16, split=100, name="att5_many"),     # 216 items
-           "many_items_d64": _attention_case(2, 1500, 24, 64, torch.float16, split=1024, name="att5_many64")}
-    out["rescale"] = check_attention_large_scores()["err"]
-    return out
-
-
-def check_attention_v6_kernel():
-    """one and many K/V steps, odd / even step counts, ragged tails (incl. tiles with a fully masked half), both head
-    dims, split outputs, rescale"""
-    _setup()
-    out = {"d128_S64": _attention_case(1, 64, 1, 128, torch.bfloat16, name="att6_d128_S64"),
-           "d128_S128": _attention_case(1, 128, 1, 128, torch.bfloat16, name="att6_d128_S128"),
-           "d128_S300": _attention_case(2, 300, 2, 128, torch.bfloat16, name="att6_d128_S300"),
-           "d128_S1280_split": _attention_case(1, 1280, 3, 128, torch.bfloat16, split=256, name="att6_d128_S1280"),
-           "d128_S4400": _attention_case(1, 4400, 2, 128, torch.bfloat16, name="att6_d128_S4400"),
-           "d64_S1178_split": _attention_case(2, 1178, 2, 64, torch.float16, split=1024, name="att6_d64_S1178"),
-           "d64_S333": _attention_case(1, 333, 2, 64, torch.bfloat16, name="att6_d64_S333"),
-           "S1": _attention_case(2, 1, 2, 128, torch.bfloat16, name="att6_S1")}
-    out["rescale"] = check_attention_large_scores()["err"]
-    return out
+    return {"d128_S1300": _attention_case(2, 1300, 2, 128, bf16, twice=True),
+            "d64_S1178": _attention_case(2, 1178, 2, 64, fp16, twice=True)}
 
 
 def check_attention_large_scores():
@@ -447,11 +484,9 @@ def check_attention_large_scores():
     base = _rand((1, d), torch.bfloat16).float()
     qkv[:, :h] = (base * 2.0 + 0.3 * qkv[:, :h].float()).to(torch.bfloat16)
     qkv[:, h:2 * h] = (base * ramp + 0.3 * qkv[:, h:2 * h].float()).to(torch.bfloat16)
-    q, k, v = [t.reshape(B, S, heads, d).permute(0, 2, 1, 3).float() for t in qkv.split(h, dim=1)]
-    ref = (torch.softmax(q @ k.transpose(-1, -2) / math.sqrt(d), dim=-1) @ v).permute(0, 2, 1, 3).reshape(B * S, h)
     out = torch.zeros((B * S, h), dtype=torch.bfloat16, device=DEV)
     ops.attention(qkv, B, S, heads, d, out)
-    return {"err": _assert_close("att_rescale", out, ref, 1e-2)}
+    return {"err": _assert_close("att_rescale", out, ref_attention(qkv, B, S, heads, d), 1e-2)}
 
 
 # ------------------------------------------------------------------------------------------------ elementwise
@@ -476,82 +511,23 @@ def _rope_table(S, d, device):
 
 
 def check_qk_norm_rope():
+    """the unfused dk_qk_norm_rope: rows before split use the first pair of norm weights, the rest the second"""
     _setup()
     out = {}
     for (B, S, heads, d, dt, use_norm, use_rope) in [(2, 50, 3, 128, torch.bfloat16, True, True),
                                                      (1, 33, 2, 64, torch.float16, True, False),
                                                      (1, 40, 2, 128, torch.bfloat16, False, True)]:
-        h = heads * d
-        qkv = _rand((B * S, 3 * h), dt)
+        qkv = _rand((B * S, 3 * heads * d), dt)
         split = S // 3
         ws = [(_rand((d,), dt, 0.1) + 1.0) for _ in range(4)] if use_norm else [None] * 4
         rope = _rope_table(S, d, DEV) if use_rope else None
-        ref = qkv.float().clone()
         pos = torch.arange(B * S, device=DEV) % S
-        for which, (w1, w2) in enumerate([(ws[0], ws[2]), (ws[1], ws[3])]):
-            t = ref[:, which * h:(which + 1) * h].reshape(B * S, heads, d)
-            if use_norm:
-                w = torch.where((pos < split)[:, None, None], w1.float()[None, None], w2.float()[None, None])
-                t = t * torch.rsqrt((t * t).mean(-1, keepdim=True) + 1e-6) * w
-                t = t.to(dt).float()
-            if use_rope:
-                c = rope[pos][:, None, :, 0]
-                s = rope[pos][:, None, :, 1]
-                x0, x1 = t[..., 0::2], t[..., 1::2]
-                t = torch.stack([x0 * c - x1 * s, x0 * s + x1 * c], dim=-1).reshape(B * S, heads, d)
-            ref[:, which * h:(which + 1) * h] = t.reshape(B * S, h)
+        first = (pos < split)[:, None, None]
+        qw, kw = ([torch.where(first, w1.float(), w2.float()) for w1, w2 in ((ws[0], ws[2]), (ws[1], ws[3]))]
+                  if use_norm else (None, None))
+        ref = ref_qk_norm_rope(qkv, pos, heads, d, qw, kw, rope, round_to=dt)
         got = ops.qk_norm_rope(qkv.clone(), S, heads, d, split, ws[0], ws[1], ws[2], ws[3], rope)
         out[f"d{d}_{use_norm}_{use_rope}"] = _assert_close(f"qknr_{d}", got, ref, 4e-3)
-    return out
-
-
-def check_gemm_pair_kernel():
-    """large and ragged shapes (256- and 128-wide tiles): ragged M/N/K, every epilogue, more tiles than SMs, strided
-    output windows, in-place residual, the fused QK epilogue"""
-    _setup()
-    out = {}
-    for (M, N, K) in [(256, 256, 64), (256, 512, 512), (300, 264, 200), (77, 64, 64), (1000, 3072, 1536),
-                      (4352, 768, 3072), (20, 1024, 3072)]:
-        out[f"{M}x{N}x{K}"] = _gemm_case(M, N, K, torch.bfloat16, name=f"pair_{M}x{N}x{K}")
-    out["large"] = _gemm_case(8192, 4608, 1024, torch.bfloat16, bias=True, name="pair_8192x4608x1024")
-    out["n3072"] = _gemm_case(4096, 3072, 512, torch.bfloat16, bias=True, name="pair_4096x3072x512")
-    out["bn128"] = _gemm_case(1024, 1152, 256, torch.bfloat16, bias=True, gate=True, res=True, name="pair_1024x1152")
-    out["gelu"] = _gemm_case(384, 512, 256, torch.bfloat16, bias=True, act=ACT_GELU_ERF, name="pair_gelu")
-    out["remap"] = _gemm_case(600, 512, 256, torch.bfloat16, bias=True, gate=True, res=True, remap=True,
-                              name="pair_remap")
-    out["fp16"] = _gemm_case(300, 512, 320, torch.float16, bias=True, name="pair_fp16")
-    out.update(_pair_store_cases())
-    out.update({"qk_" + k: v for k, v in check_gemm_fused_qk_norm_rope().items()})
-    return out
-
-
-def _pair_store_cases():
-    """outputs the GEMM epilogue has to get right: a strided column window of a wider buffer (the FLUX single-block
-    concat buffer), rows/columns that are not tile multiples next to data that must survive, in-place residual"""
-    out = {}
-    M, N, K, ld, c0 = 1000, 520, 256, 1024, 256
-    A, W = _rand((M, K), torch.bfloat16), _rand((N, K), torch.bfloat16, 1 / math.sqrt(K))
-    buf = torch.full((M + 8, ld), 7.0, dtype=torch.bfloat16, device=DEV)
-    view = buf[:M, c0:c0 + N]
-    ops.gemm(A, W, out=view, act=ACT_GELU_ERF)
-    out["window"] = _assert_close("pair_window", view, torch.nn.functional.gelu(A.float() @ W.float().t()), 4e-3)
-    keep = buf.clone()
-    keep[:M, c0:c0 + N] = 7.0
-    assert bool((keep == 7.0).all()), "pair_window: bytes outside the output window were written"
-    x = _rand((M, N), torch.bfloat16)
-    g = _rand((1, N), torch.bfloat16)
-    ref = x.float() + g.float() * (A.float() @ W.float().t())
-    out["inplace"] = _assert_close("pair_inplace", ops.gemm(A, W, out=x, res=x, gate=g), ref, 4e-3)
-    return out
-
-
-def check_gemm_pair_legacy_store():
-    """the epilogue's register -> global stores with bias, gate and in-place-able residual on a multi-tile problem and a
-    ragged one, plus the output-window cases"""
-    _setup()
-    out = {"large": _gemm_case(2048, 1536, 512, torch.bfloat16, bias=True, gate=True, res=True, name="pairleg_large"),
-           "ragged": _gemm_case(300, 264, 200, torch.bfloat16, name="pairleg_ragged")}
-    out.update(_pair_store_cases())
     return out
 
 
@@ -583,19 +559,8 @@ def check_gemm_fused_qk_norm_rope():
         other[rows] = False
         if bool(other.any()):
             assert float(fused[other].float().abs().max()) == 0.0, "rows outside the scatter window were written"
-        # fp32 reference
-        y = (A.float() @ W.float().t() + bias.float())
         pos = (torch.arange(Bt * Ss, device=DEV) % Ss) + off
-        ref = y.clone()
-        for which, w in enumerate([qw, kw]):
-            t = y[:, which * h:(which + 1) * h].reshape(-1, heads, d)
-            if use_norm:
-                t = t * torch.rsqrt((t * t).mean(-1, keepdim=True) + 1e-6) * w.float()
-            if use_rope:
-                c, sn = rope[pos][:, None, :, 0], rope[pos][:, None, :, 1]
-                x0, x1 = t[..., 0::2], t[..., 1::2]
-                t = torch.stack([x0 * c - x1 * sn, x0 * sn + x1 * c], dim=-1).reshape(-1, heads, d)
-            ref[:, which * h:(which + 1) * h] = t.reshape(-1, h)
+        ref = ref_qk_norm_rope(ref_gemm(A, W, bias), pos, heads, d, qw, kw, rope)
         out[f"vs_fp32_d{d}_{use_norm}"] = _assert_close(f"fusedqk_ref_{d}", fused[rows], ref, 6e-3)
     return out
 
@@ -665,25 +630,26 @@ def check_sampler_kernels():
     return out
 
 
+def _groupnorm_case(B, H, W, Cc, dt):
+    """dk_groupnorm_stats and dk_groupnorm_apply (+ SiLU) vs ref_groupnorm_silu, each image compared on its own"""
+    x = _rand((B, H, W, Cc), dt, 1.5) + 0.7
+    gamma = _rand((Cc,), dt, 0.1) + 1.0
+    beta = _rand((Cc,), dt, 0.1)
+    ref, mean, rstd = ref_groupnorm_silu(x, gamma, beta, 32, 1e-5)
+    stats = ops.groupnorm_stats(x, 32, 1e-5)
+    name = f"gn_{B}x{H}x{W}x{Cc}_{str(dt)[6:]}"
+    out = {"mean": _assert_close(name + "_mean", stats[..., 0], mean, 1e-4),
+           "rstd": _assert_close(name + "_rstd", stats[..., 1], rstd, 1e-4)}
+    got = ops.groupnorm_apply(x, stats, gamma, beta, 32, True)
+    for i in range(B):
+        out[f"apply_{i}"] = _assert_close(f"{name}_apply_{i}", got[i], ref[i], 4e-3)
+    return out
+
+
 def check_groupnorm():
     _setup()
-    out = {}
-    for (B, H, W, Cc, dt) in [(2, 16, 16, 128, torch.bfloat16), (1, 9, 7, 512, torch.bfloat16),
-                              (1, 32, 32, 256, torch.float16)]:
-        x = _rand((B, H, W, Cc), dt, 1.5) + 0.7
-        gamma = _rand((Cc,), dt, 0.1) + 1.0
-        beta = _rand((Cc,), dt, 0.1)
-        stats = ops.groupnorm_stats(x, 32, 1e-5)
-        xf = x.float().reshape(B, H * W, 32, Cc // 32)
-        mean = xf.mean(dim=(1, 3))
-        var = xf.var(dim=(1, 3), unbiased=False)
-        out[f"stats_{Cc}"] = _assert_close("gn_mean", stats[..., 0], mean, 1e-4)
-        _assert_close("gn_rstd", stats[..., 1], torch.rsqrt(var + 1e-5), 1e-4)
-        ref = torch.nn.functional.group_norm(x.float().permute(0, 3, 1, 2), 32, gamma.float(), beta.float(), 1e-5)
-        ref = torch.nn.functional.silu(ref.permute(0, 2, 3, 1).to(dt).float())
-        got = ops.groupnorm_apply(x, stats, gamma, beta, 32, True)
-        out[f"apply_{Cc}"] = _assert_close("gn_apply", got, ref, 4e-3)
-    return out
+    return {f"{B}x{H}x{W}x{Cc}": _groupnorm_case(B, H, W, Cc, dt)
+            for (B, H, W, Cc, dt) in [(2, 16, 16, 128, bf16), (1, 9, 7, 512, bf16), (1, 32, 32, 256, fp16)]}
 
 
 def check_softmax_image_post():
@@ -705,13 +671,13 @@ def check_edge_cases():
     """smallest / most ragged shapes every kernel accepts"""
     _setup()
     out = {}
-    out["gemm_1x8x8"] = _gemm_case(1, 8, 8, torch.bfloat16, bias=True, name="gemm_1x8x8")
-    out["gemm_129x72x24"] = _gemm_case(129, 72, 24, torch.float16, bias=True, act=ACT_SILU, name="gemm_129x72x24")
-    out["att_S1"] = _attention_case(2, 1, 2, 128, torch.bfloat16, name="att_S1")
-    out["att_S129"] = _attention_case(1, 129, 1, 64, torch.float16, name="att_S129")
-    out["att_S257_split1"] = _attention_case(1, 257, 2, 128, torch.bfloat16, split=1, name="att_S257")
-    out["conv_1x1"] = _conv_case(1, 1, 1, 64, 8, torch.bfloat16, name="conv_1x1")
-    out["conv_3x5"] = _conv_case(2, 3, 5, 64, 24, torch.bfloat16, res=True, name="conv_3x5")
+    out["gemm_1x8x8"] = _gemm_case(1, 8, 8, torch.bfloat16, "bias")
+    out["gemm_129x72x24"] = _gemm_case(129, 72, 24, torch.float16, "bias silu")
+    out["att_S1"] = _attention_case(2, 1, 2, 128, torch.bfloat16)
+    out["att_S129"] = _attention_case(1, 129, 1, 64, torch.float16)
+    out["att_S257_split1"] = _attention_case(1, 257, 2, 128, torch.bfloat16, split=1)
+    out["conv_1x1"] = _conv_case(1, 1, 1, 64, 8, torch.bfloat16)
+    out["conv_3x5"] = _conv_case(2, 3, 5, 64, 24, torch.bfloat16, res=True)
     x = _rand((3, 64), torch.bfloat16, 2.0)
     mod = _rand((3, 128), torch.bfloat16, 0.3)
     ref = torch.nn.functional.layer_norm(x.float(), (64,), eps=1e-6) * (1 + mod[:, 64:].float()) + mod[:, :64].float()
@@ -749,12 +715,12 @@ def check_error_paths():
             continue
         raise AssertionError(f"{name}: accepted")
     # the context is still healthy afterwards
-    return {"after": _gemm_case(128, 128, 64, torch.bfloat16, name="gemm_after_errors")}
+    return {"after": _gemm_case(128, 128, 64, torch.bfloat16)}
 
 
 # ------------------------------------------------------------------------------------------------ fused VAE conv (K7f)
-def _conv_fused_case(B, H, W, Cin, Cout, dtype, norm, up, res, want_stats, name, tol=4e-3):
-    """[GroupNorm+SiLU] -> [nearest 2x] -> conv3x3 (+bias, +skip) in one kernel vs the same chain in fp32 torch
+def _conv_fused_case(B, H, W, Cin, Cout, dtype, norm, up, res, want_stats, tol):
+    """[GroupNorm+SiLU] -> [nearest 2x] -> conv3x3 (+bias, +skip) in one kernel vs the same chain of fp32 references
     (reference mlx/vae.py:60-101 ResnetBlock2D, :20-25/:146-147 upsample stage)"""
     G = 32
     x = _rand((B, H, W, Cin), dtype, 1.5) + 0.3
@@ -762,24 +728,20 @@ def _conv_fused_case(B, H, W, Cin, Cout, dtype, norm, up, res, want_stats, name,
     b = _rand((Cout,), dtype, 0.5)
     Ho, Wo = (2 * H, 2 * W) if up else (H, W)
     r = _rand((B, Ho, Wo, Cout), dtype) if res else None
-    xin = x.float()
-    gn = None
+    xin, gn = x, None
     if norm:
         gamma, beta = _rand((Cin,), dtype, 0.1) + 1.0, _rand((Cin,), dtype, 0.1)
-        stats = ops.groupnorm_stats(x, G, 1e-5)
-        gn = (stats, gamma, beta, G)
-        xn = torch.nn.functional.group_norm(xin.permute(0, 3, 1, 2), G, gamma.float(), beta.float(), 1e-5)
-        xin = torch.nn.functional.silu(xn.permute(0, 2, 3, 1).to(dtype).float()).to(dtype).float()
+        gn = (ops.groupnorm_stats(x, G, 1e-5), gamma, beta, G)
+        xin = ref_groupnorm_silu(x, gamma, beta, G, 1e-5)[0].to(dtype)     # the conv reads the activation in 16 bits
     if up:
         xin = xin.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
-    ref = torch.nn.functional.conv2d(xin.permute(0, 3, 1, 2), w.float().permute(0, 3, 1, 2), b.float(),
-                                     padding=1).permute(0, 2, 3, 1)
-    if res:
-        ref = ref + r.float()
+    ref = ref_conv3x3(xin, w, b, r)
     wk = ops.conv_up_weights(w) if up else w
     slots = Ho * Wo // 128
     part = torch.full((B, slots, G, 2), float("nan"), dtype=torch.float32, device=DEV) if want_stats else None
     got = ops.conv3x3_fused(x, wk, bias=b, res=r, up=up, gn=gn, silu=norm, out_partial=part, out_G=G)
+    name = f"cf_{B}x{H}x{W}_{Cin}to{Cout}_{str(dtype)[6:]}" + "".join(
+        f"_{k}" for k, v in (("norm", norm), ("up", up), ("res", res)) if v)
     out = {"rel_l2": _assert_close(name, got, ref, tol)}
     if want_stats:
         st = ops.groupnorm_finalize(part, B, G, slots, float(Ho * Wo * (Cout // G)), 1e-5)
@@ -790,33 +752,34 @@ def _conv_fused_case(B, H, W, Cin, Cout, dtype, norm, up, res, want_stats, name,
     return out
 
 
-def check_conv_fused():
+def _conv_fused_table(cases):
     _setup()
     out = {}
-    bf = torch.bfloat16
-    out["plain_64to128"] = _conv_fused_case(1, 8, 128, 64, 128, bf, False, False, False, False, "cf_plain")
-    out["plain_res_256"] = _conv_fused_case(2, 16, 256, 128, 256, bf, False, False, True, True, "cf_res256")
-    out["norm_silu"] = _conv_fused_case(2, 8, 128, 128, 128, bf, True, False, False, True, "cf_norm", tol=6e-3)
-    out["norm_silu_res_512to256"] = _conv_fused_case(1, 12, 256, 512, 256, bf, True, False, True, True, "cf_norm512",
-                                                     tol=6e-3)
-    out["up_256"] = _conv_fused_case(1, 8, 128, 256, 256, bf, False, True, False, True, "cf_up", tol=6e-3)
-    out["up_b2_512"] = _conv_fused_case(2, 4, 256, 512, 512, bf, False, True, False, False, "cf_up512", tol=6e-3)
-    out["fp16_norm"] = _conv_fused_case(1, 8, 128, 64, 128, torch.float16, True, False, True, True, "cf_fp16")
-    # narrow output tile (conv_out: 3 real channels padded to 8; weight rows beyond Cout zero-filled by TMA)
-    out["narrow_norm_128to8"] = _conv_fused_case(2, 8, 256, 128, 8, bf, True, False, False, False, "cf_narrow8", tol=6e-3)
-    out["narrow_plain_64to64"] = _conv_fused_case(1, 4, 128, 64, 64, bf, False, False, True, False, "cf_narrow64")
+    for (B, H, W, Cin, Cout, dt, norm, up, res, want_stats, tol) in cases:
+        key = f"{B}x{H}x{W}_{Cin}to{Cout}_norm{norm:d}_up{up:d}_res{res:d}"
+        out[key] = _conv_fused_case(B, H, W, Cin, Cout, dt, norm, up, res, want_stats, tol)
     return out
+
+
+def check_conv_fused():
+    # (B, H, W, Cin, Cout, dtype, norm, up, res, want_stats, tol); the 128 -> 8 case is the narrow output tile of
+    # conv_out (3 real channels padded to 8; weight rows beyond Cout zero-filled by TMA)
+    return _conv_fused_table([(1, 8, 128, 64, 128, bf16, False, False, False, False, 4e-3),
+                              (2, 16, 256, 128, 256, bf16, False, False, True, True, 4e-3),
+                              (2, 8, 128, 128, 128, bf16, True, False, False, True, 6e-3),
+                              (1, 12, 256, 512, 256, bf16, True, False, True, True, 6e-3),
+                              (1, 8, 128, 256, 256, bf16, False, True, False, True, 6e-3),
+                              (2, 4, 256, 512, 512, bf16, False, True, False, False, 6e-3),
+                              (1, 8, 128, 64, 128, fp16, True, False, True, True, 4e-3),
+                              (2, 8, 256, 128, 8, bf16, True, False, False, False, 6e-3),
+                              (1, 4, 128, 64, 64, bf16, False, False, True, False, 4e-3)])
 
 
 def check_fullsize_conv_fused():
     """the fused ResNet-path convolution at the 1024^2 decode's real extents"""
-    _setup()
-    bf = torch.bfloat16
-    return {"1024_128_norm_res": _conv_fused_case(1, 1024, 1024, 128, 128, bf, True, False, True, True, "cf_full_1024",
-                                                  tol=6e-3),
-            "512_256_norm": _conv_fused_case(2, 512, 512, 256, 256, bf, True, False, False, True, "cf_full_512", tol=6e-3),
-            "up_512to1024_256": _conv_fused_case(1, 512, 512, 256, 256, bf, False, True, False, True, "cf_full_up",
-                                                 tol=6e-3)}
+    return _conv_fused_table([(1, 1024, 1024, 128, 128, bf16, True, False, True, True, 6e-3),
+                              (2, 512, 512, 256, 256, bf16, True, False, False, True, 6e-3),
+                              (1, 512, 512, 256, 256, bf16, False, True, False, True, 6e-3)])
 
 
 # ------------------------------------------------------------------------------------------------ BASELINE shapes
@@ -847,20 +810,10 @@ def _assert_close_blocks(name, got, ref, tol, block_tol, br=128, bc=128):
     return {"rel_l2": err, "worst_block": worst}
 
 
-def _ref_matmul(A, W):
-    """fp32 reference product in row chunks (the fp32 copy of a 16384 x 12288 output alone is 805 MB)"""
-    Wt = W.float().t().contiguous()
-    return torch.cat([A[i:i + 4096].float() @ Wt for i in range(0, A.shape[0], 4096)], 0)
-
-
 def check_fullsize_gemm_fc1():
     """FLUX fc1 at the C4 bench shape: 16384 x 12288 x 3072, bias + GELU-erf (reference mlx/mmdit.py:827-835)"""
     _setup()
-    M, N, K = 16384, 12288, 3072
-    A, W, b = _rand((M, K), torch.bfloat16), _rand((N, K), torch.bfloat16, 1 / math.sqrt(K)), _rand((N,), torch.bfloat16, 0.5)
-    ref = torch.nn.functional.gelu(_ref_matmul(A, W) + b.float())
-    got = ops.gemm(A, W, bias=b, act=ACT_GELU_ERF)
-    return _assert_close_blocks("full_fc1", got, ref, 4e-3, 1.2e-2)
+    return _gemm_case(16384, 12288, 3072, bf16, "bias gelu", block_tol=1.2e-2)
 
 
 def check_fullsize_gemm_single_out():
@@ -871,23 +824,9 @@ def check_fullsize_gemm_single_out():
     M = B * S
     A, W, b = _rand((M, K), torch.bfloat16), _rand((N, K), torch.bfloat16, 1 / math.sqrt(K)), _rand((N,), torch.bfloat16, 0.5)
     x, g = _rand((M, N), torch.bfloat16), _rand((B, N), torch.bfloat16)
-    ref = x.float() + g.float().repeat_interleave(S, 0) * (_ref_matmul(A, W) + b.float())
+    ref = ref_gemm(A, W, b, gate=g, res=x)
     got = ops.gemm(A, W, out=x, bias=b, gate=g, res=x, rows_per_batch=S, out_batch_rows=S)
     return _assert_close_blocks("full_single_out", got, ref, 4e-3, 1.2e-2)
-
-
-def _ref_qk_norm_rope(y, pos, h, heads, d, qw, kw, rope):
-    ref = y.clone()
-    for which, w in enumerate([qw, kw]):
-        t = y[:, which * h:(which + 1) * h].reshape(-1, heads, d)
-        if w is not None:
-            t = t * torch.rsqrt((t * t).mean(-1, keepdim=True) + 1e-6) * w.float()
-        if rope is not None:
-            c, sn = rope[pos][:, None, :, 0], rope[pos][:, None, :, 1]
-            x0, x1 = t[..., 0::2], t[..., 1::2]
-            t = torch.stack([x0 * c - x1 * sn, x0 * sn + x1 * c], dim=-1).reshape(-1, heads, d)
-        ref[:, which * h:(which + 1) * h] = t.reshape(-1, h)
-    return ref
 
 
 def check_fullsize_gemm_qkv_fused():
@@ -903,30 +842,12 @@ def check_fullsize_gemm_qkv_fused():
     ops.gemm(A, W, out=fused, bias=bias, rows_per_batch=Ss, out_batch_rows=S, out_row_off=off,
              qk=(heads, d, qw, kw, rope, 1e-6))
     rows = torch.cat([torch.arange(b * S + off, b * S + off + Ss) for b in range(Bt)]).to(DEV)
-    y = _ref_matmul(A, W) + bias.float()
     pos = (torch.arange(Bt * Ss, device=DEV) % Ss) + off
-    ref = _ref_qk_norm_rope(y, pos, h, heads, d, qw, kw, rope)
+    ref = ref_qk_norm_rope(ref_gemm(A, W, bias), pos, heads, d, qw, kw, rope)
     other = torch.ones(Bt * S, dtype=torch.bool, device=DEV)
     other[rows] = False
     assert float(fused[other].float().abs().max()) == 0.0, "rows outside the scatter window were written"
     return _assert_close_blocks("full_qkv_fused", fused[rows], ref, 6e-3, 1.5e-2)
-
-
-def _attention_full_case(B, S, heads, d, dtype, split, name):
-    """fp32 reference one head at a time (a 4685^2 fp32 score matrix is 88 MB)"""
-    h = heads * d
-    qkv = _rand((B * S, 3 * h), dtype)
-    o0 = torch.zeros((B * split, h), dtype=dtype, device=DEV)
-    o1 = torch.zeros((B * (S - split), h), dtype=dtype, device=DEV)
-    ops.attention(qkv, B, S, heads, d, o0, split=split, out1=o1)
-    got = torch.cat([o0.reshape(B, split, h), o1.reshape(B, S - split, h)], dim=1)
-    ref = torch.empty((B, S, h), dtype=torch.float32, device=DEV)
-    x = qkv.reshape(B, S, 3, heads, d)
-    for b in range(B):
-        for hd in range(heads):
-            q, k, v = x[b, :, 0, hd].float(), x[b, :, 1, hd].float(), x[b, :, 2, hd].float()
-            ref[b, :, hd * d:(hd + 1) * d] = torch.softmax(q @ k.t() / math.sqrt(d), dim=-1) @ v
-    return _assert_close_blocks(name, got.reshape(B * S, h), ref.reshape(B * S, h), 1e-2, 3e-2, br=128, bc=d)
 
 
 def check_fullsize_attention():
@@ -934,66 +855,25 @@ def check_fullsize_attention():
     S=4608 (C5), SD3 d=64 fp16 S=4685 (C3: ragged tail), outputs split at the text/image boundary as the model does
     (reference mlx/mmdit.py:594-657)"""
     _setup()
-    return {"flux_S4352": _attention_full_case(2, 4352, 24, 128, torch.bfloat16, 256, "full_att_4352"),
-            "flux_S4608": _attention_full_case(1, 4608, 24, 128, torch.bfloat16, 512, "full_att_4608"),
-            "sd3_S4685": _attention_full_case(2, 4685, 24, 64, torch.float16, 4096, "full_att_4685")}
-
-
-def _conv_full_case(B, H, W, Cin, Cout, dtype, res, name):
-    x = _rand((B, H, W, Cin), dtype)
-    w = _rand((Cout, 3, 3, Cin), dtype, 1 / math.sqrt(9 * Cin))
-    b = _rand((Cout,), dtype, 0.5)
-    r = _rand((B, H, W, Cout), dtype) if res else None
-    got = ops.conv3x3(x, w, bias=b, res=r)
-    wf = w.float().permute(0, 3, 1, 2).contiguous()
-    ref = torch.empty((B, H, W, Cout), dtype=torch.float32, device=DEV)
-    rows = max(8, (1 << 24) // (W * max(Cin, Cout)))       # reference in horizontal bands with a one-row halo
-    for b_ in range(B):
-        for y0 in range(0, H, rows):
-            y1 = min(H, y0 + rows)
-            ya, yb = max(0, y0 - 1), min(H, y1 + 1)
-            xin = x[b_, ya:yb].float().permute(2, 0, 1)[None]
-            xin = torch.nn.functional.pad(xin, (1, 1, 1 if y0 == 0 else 0, 1 if y1 == H else 0))
-            o = torch.nn.functional.conv2d(xin, wf, b.float())[0].permute(1, 2, 0)
-            ref[b_, y0:y1] = o
-    if res:
-        ref += r.float()
-    return _assert_close_blocks(name, got.reshape(-1, Cout), ref.reshape(-1, Cout), 4e-3, 1.2e-2, br=128, bc=min(128, Cout))
+    return {"flux_S4352": _attention_case(2, 4352, 24, 128, bf16, 256, out1_pad=0, block_tol=3e-2),
+            "flux_S4608": _attention_case(1, 4608, 24, 128, bf16, 512, out1_pad=0, block_tol=3e-2),
+            "sd3_S4685": _attention_case(2, 4685, 24, 64, fp16, 4096, out1_pad=0, block_tol=3e-2)}
 
 
 def check_fullsize_conv():
     """VAE decoder convs at the 1024^2 decode's real extents (reference mlx/vae.py:60-101,146-149):
     1024 x 1024 x 128 -> 128 (+ skip), 512 x 512 x 256 -> 256, and the 512 -> 256 channel change at 512^2"""
     _setup()
-    return {"1024_128": _conv_full_case(1, 1024, 1024, 128, 128, torch.bfloat16, True, "full_conv_1024"),
-            "512_256": _conv_full_case(2, 512, 512, 256, 256, torch.bfloat16, False, "full_conv_512"),
-            "512_512to256": _conv_full_case(1, 512, 512, 512, 256, torch.bfloat16, False, "full_conv_512to256")}
+    return {"1024_128": _conv_case(1, 1024, 1024, 128, 128, bf16, True, block_tol=1.2e-2),
+            "512_256": _conv_case(2, 512, 512, 256, 256, bf16, False, block_tol=1.2e-2),
+            "512_512to256": _conv_case(1, 512, 512, 512, 256, bf16, False, block_tol=1.2e-2)}
 
 
 def check_fullsize_groupnorm():
     """GroupNorm(32) + SiLU at 1024 x 1024 x 128 and 512 x 512 x 256, batch 2 (reference mlx/vae.py:72-80)"""
     _setup()
-    out = {}
-    for (B, H, W, Cc) in [(2, 1024, 1024, 128), (2, 512, 512, 256)]:
-        dt = torch.bfloat16
-        x = _rand((B, H, W, Cc), dt, 1.5) + 0.7
-        gamma, beta = _rand((Cc,), dt, 0.1) + 1.0, _rand((Cc,), dt, 0.1)
-        stats = ops.groupnorm_stats(x, 32, 1e-5)
-        mean = torch.empty((B, 32), device=DEV, dtype=torch.float64)
-        var = torch.empty((B, 32), device=DEV, dtype=torch.float64)
-        for b_ in range(B):
-            xf = x[b_].reshape(H * W, 32, Cc // 32).double()
-            mean[b_] = xf.mean(dim=(0, 2))
-            var[b_] = xf.var(dim=(0, 2), unbiased=False)
-        out[f"mean_{Cc}"] = _assert_close("full_gn_mean", stats[..., 0], mean.float(), 1e-4)
-        out[f"rstd_{Cc}"] = _assert_close("full_gn_rstd", stats[..., 1], torch.rsqrt(var + 1e-5).float(), 1e-4)
-        got = ops.groupnorm_apply(x, stats, gamma, beta, 32, True)
-        for b_ in range(B):
-            xn = (x[b_].float().reshape(H * W, 32, Cc // 32) - mean[b_].float()[None, :, None]) * \
-                torch.rsqrt(var[b_] + 1e-5).float()[None, :, None]
-            ref = torch.nn.functional.silu((xn.reshape(H * W, Cc) * gamma.float() + beta.float()).to(dt).float())
-            out[f"apply_{Cc}_{b_}"] = _assert_close("full_gn_apply", got[b_].reshape(H * W, Cc), ref, 4e-3)
-    return out
+    return {f"{H}x{W}x{Cc}": _groupnorm_case(B, H, W, Cc, bf16) for (B, H, W, Cc) in [(2, 1024, 1024, 128),
+                                                                                     (2, 512, 512, 256)]}
 
 
 FULLSIZE_CHECKS = [check_fullsize_gemm_fc1, check_fullsize_gemm_single_out, check_fullsize_gemm_qkv_fused,
@@ -1001,16 +881,13 @@ FULLSIZE_CHECKS = [check_fullsize_gemm_fc1, check_fullsize_gemm_single_out, chec
 
 
 ALL_CHECKS = [
-    check_gemm_single_tile, check_gemm_multi_k, check_gemm_shapes, check_gemm_persistent_large, check_gemm_epilogues,
-    check_gemm_fp16, check_gemm_inplace_residual, check_gemm_w_n_major, check_gemm_fused_qk_norm_rope,
-    check_gemm_pair_kernel, check_gemm_pair_legacy_store, check_conv3x3, check_conv3x3_s2, check_img2img_kernels, check_dequant_q4,
-    check_text_kernels, check_attention_small,
-    check_attention_d128_one_tile, check_attention_d128, check_attention_d64, check_attention_large_scores,
-    check_attention_v3_explicit, check_attention_v3s_kernel, check_attention_v3_variants, check_attention_v5_kernel, check_attention_v6_kernel,
+    check_gemm_single_tile, check_gemm_multi_k, check_gemm_one_m_pair, check_gemm_shapes, check_gemm_persistent_large,
+    check_gemm_epilogues, check_gemm_gate_residual, check_gemm_output_window, check_gemm_fp16,
+    check_gemm_inplace_residual, check_gemm_w_n_major, check_gemm_fused_qk_norm_rope,
+    check_conv3x3, check_conv3x3_s2, check_img2img_kernels, check_dequant_q4, check_text_kernels, check_attention_small,
+    check_attention_d128_one_tile, check_attention_d128, check_attention_d64, check_attention_short,
+    check_attention_long, check_attention_many_ctas, check_attention_determinism, check_attention_large_scores,
     check_conv_fused,
     check_ln_modulate, check_qk_norm_rope, check_layout_kernels, check_sampler_kernels, check_groupnorm,
     check_softmax_image_post, check_edge_cases, check_error_paths,
 ] + FULLSIZE_CHECKS
-
-EXPERIMENTAL_CHECKS = []
-

@@ -11,6 +11,7 @@ import torch
 
 from diffusionkit_b200 import ops
 from diffusionkit_b200._lib import ACT_GELU_ERF
+from tests.kernel_checks import ref_conv3x3, rel_l2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -19,10 +20,6 @@ DEV = "cuda:0"
 def _rand(shape, dtype, scale=1.0, seed=0):
     g = torch.Generator(device=DEV).manual_seed(seed)
     return (torch.randn(shape, generator=g, device=DEV) * scale).to(dtype)
-
-
-def _rel_l2(a, b):
-    return float((a.float() - b.float()).norm() / (b.float().norm() + 1e-30))
 
 
 def _sentinel(shape, dtype):
@@ -80,7 +77,7 @@ def test_odd_num_m_sd3_text_rows_inplace_residual(cuda):
     ops.gemm(A, W, out=buf, bias=b, gate=gate, res=buf, rows_per_batch=rpb, out_batch_rows=rpb + pad, out_row_off=off,
              res_batch_rows=rpb + pad, res_row_off=off)
     ref = x0.float() + gate.float().repeat_interleave(rpb, 0) * (A.float() @ W.float().t() + b.float())
-    assert _rel_l2(buf[rows], ref) <= 4e-3
+    assert rel_l2(buf[rows], ref) <= 4e-3
     other = torch.ones(buf.shape[0], dtype=torch.bool, device=DEV)
     other[rows] = False
     assert _same_bits(buf[other], before[other])
@@ -97,7 +94,7 @@ def test_odd_num_m_cat_window(cuda, N):
     before = cat.clone()
     ops.gemm(A, W, out=cat[:M, left:left + N], bias=b, act=ACT_GELU_ERF)
     ref = torch.nn.functional.gelu(A.float() @ W.float().t() + b.float())
-    assert _rel_l2(cat[:M, left:left + N], ref) <= 4e-3
+    assert rel_l2(cat[:M, left:left + N], ref) <= 4e-3
     mask = torch.ones(cat.shape, dtype=torch.bool, device=DEV)
     mask[:M, left:left + N] = False
     assert _same_bits(cat[mask], before[mask])
@@ -117,7 +114,7 @@ def test_repeatable(cuda, dtype, N, M):
     assert _same_bits(one, two)
     if M == 256:
         ref = torch.nn.functional.gelu(A.float() @ W.float().t() + b.float())
-        assert _rel_l2(one, ref) <= 4e-3
+        assert rel_l2(one, ref) <= 4e-3
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(1, 101, 64, 128, 128), (1, 320, 320, 128, 256)],
@@ -131,9 +128,7 @@ def test_conv3x3_persistent(cuda, B, H, W, Cin, Cout):
     b = _rand((Cout,), dt, 0.5, seed=25)
     r = _rand((B, H, W, Cout), dt, seed=26)
     got = ops.conv3x3(x, w, bias=b, res=r)
-    ref = torch.nn.functional.conv2d(x.float().permute(0, 3, 1, 2), w.float().permute(0, 3, 1, 2), b.float(),
-                                     padding=1).permute(0, 2, 3, 1) + r.float()
-    assert _rel_l2(got, ref) <= 4e-3
+    assert rel_l2(got, ref_conv3x3(x, w, b, r)) <= 4e-3
     assert _same_bits(got, ops.conv3x3(x, w, bias=b, res=r))
 
 
@@ -143,5 +138,5 @@ def test_w_n_major_persistent(cuda):
     M, N, K, dt = 128 * 333 - 40, 384, 256, torch.bfloat16
     A, Wt = _rand((M, K), dt, seed=27), _rand((K, N), dt, 1 / math.sqrt(K), seed=28)
     got = ops.gemm(A, Wt, w_n_major=True)
-    assert _rel_l2(got, A.float() @ Wt.float()) <= 4e-3
+    assert rel_l2(got, A.float() @ Wt.float()) <= 4e-3
     assert _same_bits(got, ops.gemm(A, Wt, w_n_major=True))

@@ -29,9 +29,6 @@ def main():
 
     names = [c.__name__ for c in kc.ALL_CHECKS + mc.ALL_CHECKS]
     filt = sys.argv[1:]
-    if "+experimental" in filt:
-        filt.remove("+experimental")
-        names += [c.__name__ for c in kc.EXPERIMENTAL_CHECKS]
     if filt:
         names = [n for n in names if any(f in n for f in filt)]
     out_dir = os.path.join(ROOT, "gpurun_out")
