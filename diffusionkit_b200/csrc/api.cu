@@ -55,6 +55,15 @@ extern "C" void dk_ctx_destroy(dk_ctx* ctx) {
 
 extern "C" long long dk_ctx_launch_count(dk_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
+int dk_kernel_smem(dk_ctx* ctx, const void* func, int bytes) {
+  int& limit = ctx->smem_limit[func];
+  if (limit < bytes) {
+    DK_CHECK_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    limit = bytes;
+  }
+  return 0;
+}
+
 int dk_make_tmap_16b(dk_ctx* ctx, CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                      const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides) {
   cuuint64_t gdim[5];
@@ -114,8 +123,7 @@ extern "C" int dk_comm_unique_id(uint8_t id_host[128]) {
 }
 
 extern "C" int dk_comm_init(dk_ctx* ctx, int rank, int world, const uint8_t id_host[128]) {
-  DK_REQUIRE(ctx != nullptr, "dk_comm_init: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_REQUIRE(ctx->nccl_comm == nullptr, "dk_comm_init: communicator already initialised");
   void* lib = dk_open_nccl();
   DK_REQUIRE(lib != nullptr, "dk_comm_init: libnccl not found");
@@ -133,8 +141,8 @@ extern "C" int dk_comm_init(dk_ctx* ctx, int rank, int world, const uint8_t id_h
 }
 
 extern "C" int dk_comm_broadcast(dk_ctx* ctx, void* ptr, size_t bytes, int root, void* stream) {
-  DK_REQUIRE(ctx != nullptr && ctx->nccl_comm != nullptr, "dk_comm_broadcast: communicator not initialised");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
+  DK_REQUIRE(ctx->nccl_comm != nullptr, "dk_comm_broadcast: communicator not initialised");
   auto bcast = reinterpret_cast<nccl_bcast_fn>(dlsym(ctx->nccl_lib, "ncclBroadcast"));
   DK_REQUIRE(bcast != nullptr, "dk_comm_broadcast: ncclBroadcast missing");
   const int rc = bcast(ptr, ptr, bytes, /*ncclInt8*/ 0, root, ctx->nccl_comm, static_cast<cudaStream_t>(stream));

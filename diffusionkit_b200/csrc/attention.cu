@@ -10,11 +10,35 @@
 //                         on the S fragment (a row is spread over the four lanes of a quad), O = O * alpha + P V
 //                         (m64nD, P from registers: the S accumulator layout of 16 key columns IS the A fragment
 //                         layout of one k16 step), O / l -> global.
-#include "attention.cuh"
+#include "common.cuh"
+#include "host.h"
 
 namespace dk {
 
+constexpr int ATT_BQ = 128;
+constexpr int ATT_BKV = 128;
 constexpr int ATT_THREADS = 384;
+
+struct AttParams {
+  int B, S, heads, split;
+  float scale_log2;  // scale * log2(e)
+  void* out0;
+  long long ld0;
+  void* out1;
+  long long ld1;
+};
+
+// one 128-row Q tile per CTA, K / V ring of KS tiles of 128 keys
+template <int D>
+struct AttCfg {
+  static constexpr int KS = 2;
+  static constexpr int TILE_BYTES = 128 * D * 2;
+  static constexpr int OFF_Q = 0;
+  static constexpr int OFF_K = TILE_BYTES;
+  static constexpr int OFF_V = OFF_K + KS * TILE_BYTES;
+  static constexpr int OFF_BAR = OFF_V + KS * TILE_BYTES;
+  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+};
 
 template <typename T, int D>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
@@ -204,11 +228,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tm, const AttParams p) 
 template <typename T, int D>
 static int launch_attention(dk_ctx* ctx, const CUtensorMap& tm, const AttParams& p, cudaStream_t stream) {
   auto kern = attention_fwd_kernel<T, D>;
-  static bool configured = false;
-  if (!configured) {
-    DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<D>::SMEM_BYTES));
-    configured = true;
-  }
+  if (int rc = dk_kernel_smem(ctx, reinterpret_cast<const void*>(kern), AttCfg<D>::SMEM_BYTES)) return rc;
   dim3 grid(dk_ceil_div(p.S, ATT_BQ), p.heads, p.B);
   kern<<<grid, ATT_THREADS, AttCfg<D>::SMEM_BYTES, stream>>>(tm, p);
   DK_LAUNCH_CHECK(ctx);
@@ -221,17 +241,15 @@ using namespace dk;
 
 extern "C" int dk_attention_fwd(dk_ctx* ctx, int dtype, const void* qkv, int B, int S, int heads, int d, float scale,
                                 int split, void* out0, long long ld0, void* out1, long long ld1, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_attention_fwd: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
-  DK_REQUIRE(dtype == DK_BF16 || dtype == DK_FP16, "dk_attention_fwd: bad dtype %d", dtype);
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
   DK_REQUIRE(d == 64 || d == 128, "dk_attention_fwd: head dim %d unsupported (64 or 128)", d);
   DK_REQUIRE(B > 0 && S > 0 && heads > 0, "dk_attention_fwd: empty problem");
   DK_REQUIRE(split >= 0 && split <= S, "dk_attention_fwd: split %d outside [0, %d]", split, S);
   DK_REQUIRE(out0 != nullptr || split == 0, "dk_attention_fwd: out0 is NULL");
   DK_REQUIRE(out1 != nullptr || split == S, "dk_attention_fwd: out1 is NULL but split < S");
   DK_REQUIRE(ld0 % 8 == 0 && ld1 % 8 == 0, "dk_attention_fwd: output leading dims must be multiples of 8");
-  DK_REQUIRE((reinterpret_cast<uintptr_t>(qkv) & 15u) == 0 && (reinterpret_cast<uintptr_t>(out0) & 15u) == 0 &&
-                 (reinterpret_cast<uintptr_t>(out1) & 15u) == 0,
+  DK_REQUIRE(dk_aligned16(qkv) && dk_aligned16(out0) && dk_aligned16(out1),
              "dk_attention_fwd: buffers must be 16-byte aligned");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int h = heads * d;
@@ -250,10 +268,8 @@ extern "C" int dk_attention_fwd(dk_ctx* ctx, int dtype, const void* qkv, int B, 
   p.ld0 = ld0;
   p.out1 = out1;
   p.ld1 = ld1;
-  if (dtype == DK_BF16) {
-    if (d == 128) return launch_attention<__nv_bfloat16, 128>(ctx, tm, p, stream);
-    return launch_attention<__nv_bfloat16, 64>(ctx, tm, p, stream);
-  }
-  if (d == 128) return launch_attention<__half, 128>(ctx, tm, p, stream);
-  return launch_attention<__half, 64>(ctx, tm, p, stream);
+  DK_DISPATCH(dtype, {
+    if (d == 128) return launch_attention<T, 128>(ctx, tm, p, stream);
+    return launch_attention<T, 64>(ctx, tm, p, stream);
+  });
 }

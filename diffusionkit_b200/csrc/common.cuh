@@ -275,6 +275,32 @@ struct Half16<__half> {
   }
 };
 
+// 8 consecutive 16-bit values (one 16-byte aligned vector) <-> fp32
+template <typename T>
+__device__ __forceinline__ void load8(const T* p, float (&v)[8]) {
+  const uint4 u = *reinterpret_cast<const uint4*>(p);
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 f = Half16<T>::unpack(w[i]);
+    v[2 * i] = f.x;
+    v[2 * i + 1] = f.y;
+  }
+}
+template <typename T>
+__device__ __forceinline__ void store8(T* p, const float (&v)[8]) {
+  uint4 o;
+  o.x = Half16<T>::pack(v[0], v[1]);
+  o.y = Half16<T>::pack(v[2], v[3]);
+  o.z = Half16<T>::pack(v[4], v[5]);
+  o.w = Half16<T>::pack(v[6], v[7]);
+  *reinterpret_cast<uint4*>(p) = o;
+}
+template <typename T>
+__device__ __forceinline__ float round16(float v) {
+  return Half16<T>::to_f(Half16<T>::from_f(v));
+}
+
 __device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f)); }
 // x * sigmoid(x) with ex2.approx + rcp.approx (the IEEE divide made the GroupNorm-apply kernel issue-bound)
 __device__ __forceinline__ float silu_f(float v) {

@@ -491,8 +491,6 @@ __global__ void conv_up_weights_kernel(const T* __restrict__ w, T* __restrict__ 
 
 using namespace dk;
 
-static bool cf_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 extern "C" int dk_conv_fused_supported(int H, int W, int Cin, int Cout) {
   // Cout: whole 128-channel tiles, or ONE narrow tile of 8..120 channels (conv_out: the weight rows beyond Cout are
   // zero-filled by the TMA unit, the epilogue stores only the real channels)
@@ -501,18 +499,12 @@ extern "C" int dk_conv_fused_supported(int H, int W, int Cin, int Cout) {
 }
 
 extern "C" int dk_conv_up_weights(dk_ctx* ctx, int dtype, const void* w, void* wp, int Cout, int Cin, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_conv_up_weights: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
-  DK_REQUIRE(dtype == DK_BF16 || dtype == DK_FP16, "dk_conv_up_weights: bad dtype %d", dtype);
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
   DK_REQUIRE(w != nullptr && wp != nullptr && Cout > 0 && Cin > 0, "dk_conv_up_weights: bad arguments");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const long long total = 16LL * Cout * Cin;
-  const int grid = static_cast<int>((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096);
-  if (dtype == DK_BF16)
-    conv_up_weights_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(w),
-                                                                      static_cast<__nv_bfloat16*>(wp), Cout, Cin);
-  else
-    conv_up_weights_kernel<__half><<<grid, 256, 0, stream>>>(static_cast<const __half*>(w), static_cast<__half*>(wp), Cout, Cin);
+  DK_DISPATCH(dtype, (conv_up_weights_kernel<T><<<dk_grid_for(16LL * Cout * Cin, 256, ctx->sm_count), 256, 0, stream>>>(
+                         static_cast<const T*>(w), static_cast<T*>(wp), Cout, Cin)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
@@ -525,17 +517,16 @@ extern "C" int dk_conv3x3_fused(dk_ctx* ctx, int dtype, const void* x, const voi
                                 void* out, int B, int H, int W, int Cin, int Cout, int up, const float* gn_stats,
                                 const void* gamma, const void* beta, int G, int silu, float* out_partial, int out_G,
                                 void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_conv3x3_fused: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
-  DK_REQUIRE(dtype == DK_BF16 || dtype == DK_FP16, "dk_conv3x3_fused: bad dtype %d", dtype);
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
   DK_REQUIRE(B > 0 && dk_conv_fused_supported(H, W, Cin, Cout),
              "dk_conv3x3_fused: needs W %% 128 == 0, H %% 4 == 0, Cin %% 64 == 0 (<= 512), Cout %% 128 == 0 or a multiple "
              "of 8 below 128 (got %dx%d, %d -> %d)",
              H, W, Cin, Cout);
   DK_REQUIRE(Cout % CF_BN == 0 || (up == 0 && out_partial == nullptr),
              "dk_conv3x3_fused: a narrow output tile (Cout = %d) has no upsampling and no output statistics", Cout);
-  DK_REQUIRE(cf_aligned16(x) && cf_aligned16(w) && cf_aligned16(out) && (bias == nullptr || cf_aligned16(bias)) &&
-                 (res == nullptr || cf_aligned16(res)),
+  DK_REQUIRE(dk_aligned16(x) && dk_aligned16(w) && dk_aligned16(out) && (bias == nullptr || dk_aligned16(bias)) &&
+                 (res == nullptr || dk_aligned16(res)),
              "dk_conv3x3_fused: buffers must be 16-byte aligned");
   DK_REQUIRE(gn_stats == nullptr || (gamma != nullptr && beta != nullptr && G > 0 && Cin % G == 0),
              "dk_conv3x3_fused: GroupNorm needs gamma, beta and G dividing Cin");
@@ -582,23 +573,11 @@ extern "C" int dk_conv3x3_fused(dk_ctx* ctx, int dtype, const void* x, const voi
   }
   const long long items = static_cast<long long>(B) * p.tiles_y * p.tiles_x * (up ? 4 : 1) * p.n_tiles;
   DK_REQUIRE(items < (1LL << 31), "dk_conv3x3_fused: problem too large");
-  if (dtype == DK_BF16) {
-    auto kern = conv_fused_kernel<__nv_bfloat16>;
-    static bool configured = false;
-    if (!configured) {
-      DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CF_SMEM_BYTES));
-      configured = true;
-    }
+  DK_DISPATCH(dtype, {
+    auto kern = conv_fused_kernel<T>;
+    if (int rc = dk_kernel_smem(ctx, reinterpret_cast<const void*>(kern), CF_SMEM_BYTES)) return rc;
     kern<<<static_cast<int>(items), CF_THREADS, CF_SMEM_BYTES, stream>>>(tmX, tmW, p);
-  } else {
-    auto kern = conv_fused_kernel<__half>;
-    static bool configured = false;
-    if (!configured) {
-      DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, CF_SMEM_BYTES));
-      configured = true;
-    }
-    kern<<<static_cast<int>(items), CF_THREADS, CF_SMEM_BYTES, stream>>>(tmX, tmW, p);
-  }
+  });
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }

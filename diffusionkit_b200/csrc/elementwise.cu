@@ -5,31 +5,6 @@
 
 namespace dk {
 
-template <typename T>
-__device__ __forceinline__ void load8(const T* p, float (&v)[8]) {
-  const uint4 u = *reinterpret_cast<const uint4*>(p);
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 f = Half16<T>::unpack(w[i]);
-    v[2 * i] = f.x;
-    v[2 * i + 1] = f.y;
-  }
-}
-template <typename T>
-__device__ __forceinline__ void store8(T* p, const float (&v)[8]) {
-  uint4 o;
-  o.x = Half16<T>::pack(v[0], v[1]);
-  o.y = Half16<T>::pack(v[2], v[3]);
-  o.z = Half16<T>::pack(v[4], v[5]);
-  o.w = Half16<T>::pack(v[6], v[7]);
-  *reinterpret_cast<uint4*>(p) = o;
-}
-template <typename T>
-__device__ __forceinline__ float round16(float v) {
-  return Half16<T>::to_f(Half16<T>::from_f(v));
-}
-
 // block-wide sum for blockDim.x = NT (multiple of 32); every thread gets the result
 template <int NT>
 __device__ __forceinline__ float block_sum(float v, float* red) {
@@ -55,23 +30,23 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// K2: LayerNorm (no affine) + adaLN modulate.  One 128-thread block per row, row kept in registers.
-//     mlx.fast.layer_norm semantics: biased variance, fp32 accumulation, (x-mu)*rsqrt(var+eps)*w + b with
-//     w = 1 + scale, b = shift (reference mlx/mmdit.py:958-972).
+// K2: LayerNorm, mlx.fast.layer_norm semantics: biased variance, fp32 accumulation, (x-mu)*rsqrt(var+eps)*w + b.
+//   MODULATE: no affine of its own, adaLN modulate w = 1 + scale, b = shift of the row's batch
+//             (reference mlx/mmdit.py:958-972);
+//   otherwise the learned affine w = scale, b = shift of nn.LayerNorm, the same for every row (mlx/clip.py:32-33,78).
 // ------------------------------------------------------------------------------------------------
 constexpr int LN_WARPS = 4;     // rows per block
 constexpr int LN_MAXV = 16;     // h <= 32 lanes * 8 * 16 = 4096
 
 // One warp per row: the row lives in registers (<= 16 x 128-bit loads in flight per lane), statistics via warp
 // shuffles only — no shared memory, no block barriers.
-template <typename T, int NV>
+template <typename T, int NV, bool MODULATE>
 __global__ void __launch_bounds__(LN_WARPS * 32)
-ln_modulate_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ shift, const T* __restrict__ scale,
-                   long long mod_ld, int rows, int rows_per_batch, int h, float eps) {
+layernorm_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ shift, const T* __restrict__ scale,
+                 long long mod_ld, int rows, int rows_per_batch, int h, float eps) {
   const int row = blockIdx.x * LN_WARPS + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
-  const int b = row / rows_per_batch;
   const T* xr = x + static_cast<long long>(row) * h;
   T* yr = y + static_cast<long long>(row) * h;
   const int nvec = h / 8;
@@ -100,8 +75,13 @@ ln_modulate_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restri
     }
   }
   const float rstd = rsqrtf(warp_sum(q) / h + eps);
-  const T* sh = shift + static_cast<long long>(b) * mod_ld;
-  const T* sc = scale + static_cast<long long>(b) * mod_ld;
+  const T* sh = shift;
+  const T* sc = scale;
+  if (MODULATE) {
+    const int b = row / rows_per_batch;
+    sh += static_cast<long long>(b) * mod_ld;
+    sc += static_cast<long long>(b) * mod_ld;
+  }
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int vec = lane + i * 32;
@@ -110,10 +90,24 @@ ln_modulate_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restri
       load8(sc + vec * 8, a);
       load8(sh + vec * 8, c);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = (v[i][j] - mean) * rstd * (1.0f + a[j]) + c[j];
+      for (int j = 0; j < 8; ++j)
+        o[j] = MODULATE ? (v[i][j] - mean) * rstd * (1.0f + a[j]) + c[j] : (v[i][j] - mean) * rstd * a[j] + c[j];
       store8(yr + vec * 8, o);
     }
   }
+}
+
+template <typename T, bool MODULATE>
+static void launch_layernorm(const void* x, void* y, const void* shift, const void* scale, long long mod_ld, int rows,
+                             int rows_per_batch, int h, float eps, cudaStream_t stream) {
+  const int blocks = dk_ceil_div(rows, LN_WARPS);
+  const int nv = dk_ceil_div(h / 8, 32);   // vectors per lane
+  auto kern = nv <= 4 ? layernorm_kernel<T, 4, MODULATE>
+              : nv <= 8 ? layernorm_kernel<T, 8, MODULATE>
+              : nv <= 12 ? layernorm_kernel<T, 12, MODULATE>
+              : layernorm_kernel<T, 16, MODULATE>;
+  kern<<<blocks, LN_WARPS * 32, 0, stream>>>(static_cast<const T*>(x), static_cast<T*>(y), static_cast<const T*>(shift),
+                                             static_cast<const T*>(scale), mod_ld, rows, rows_per_batch, h, eps);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -702,56 +696,33 @@ __global__ void image_post_kernel(const T* __restrict__ x, int c_stride, float* 
   }
 }
 
-static inline int grid_for(long long work_items, int threads, int sm_count) {
-  long long blocks = (work_items + threads - 1) / threads;
-  const long long cap = static_cast<long long>(sm_count) * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<int>(blocks);
-}
-
 }  // namespace dk
 
 using namespace dk;
 
-#define DK_DTYPE_OK(dt) DK_REQUIRE((dt) == DK_BF16 || (dt) == DK_FP16, "%s: bad dtype %d", __func__, (dt))
-#define DK_DISPATCH(dt, ...)                      \
-  do {                                            \
-    if ((dt) == DK_BF16) {                        \
-      using T = __nv_bfloat16;                    \
-      __VA_ARGS__;                                \
-    } else {                                      \
-      using T = __half;                           \
-      __VA_ARGS__;                                \
-    }                                             \
-  } while (0)
-
 extern "C" int dk_ln_modulate(dk_ctx* ctx, int dtype, const void* x, void* y, const void* shift, const void* scale,
                               long long mod_ld, int rows, int rows_per_batch, int h, float eps, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_ln_modulate: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(rows > 0 && rows_per_batch > 0, "dk_ln_modulate: empty input");
   DK_REQUIRE(h % 8 == 0 && h <= 32 * 8 * LN_MAXV, "dk_ln_modulate: h=%d unsupported (multiple of 8, <= %d)", h,
              32 * 8 * LN_MAXV);
   DK_REQUIRE(mod_ld % 8 == 0, "dk_ln_modulate: mod_ld must be a multiple of 8");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const int blocks = (rows + LN_WARPS - 1) / LN_WARPS;
-  const int nv = (h / 8 + 31) / 32;   // vectors per lane
-  DK_DISPATCH(dtype, {
-    const T* xp = static_cast<const T*>(x);
-    T* yp = static_cast<T*>(y);
-    const T* shp = static_cast<const T*>(shift);
-    const T* scp = static_cast<const T*>(scale);
-    if (nv <= 4)
-      ln_modulate_kernel<T, 4><<<blocks, LN_WARPS * 32, 0, stream>>>(xp, yp, shp, scp, mod_ld, rows, rows_per_batch, h, eps);
-    else if (nv <= 8)
-      ln_modulate_kernel<T, 8><<<blocks, LN_WARPS * 32, 0, stream>>>(xp, yp, shp, scp, mod_ld, rows, rows_per_batch, h, eps);
-    else if (nv <= 12)
-      ln_modulate_kernel<T, 12><<<blocks, LN_WARPS * 32, 0, stream>>>(xp, yp, shp, scp, mod_ld, rows, rows_per_batch, h, eps);
-    else
-      ln_modulate_kernel<T, 16><<<blocks, LN_WARPS * 32, 0, stream>>>(xp, yp, shp, scp, mod_ld, rows, rows_per_batch, h, eps);
-  });
+  DK_DISPATCH(dtype, (launch_layernorm<T, true>(x, y, shift, scale, mod_ld, rows, rows_per_batch, h, eps, stream)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_layernorm(dk_ctx* ctx, int dtype, const void* x, void* y, const void* weight, const void* bias,
+                            int rows, int h, float eps, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(rows > 0 && h > 0 && h % 8 == 0 && h <= 32 * 8 * LN_MAXV,
+             "dk_layernorm: h (%d) must be a multiple of 8, <= %d", h, 32 * 8 * LN_MAXV);
+  DK_REQUIRE(weight != nullptr && bias != nullptr, "dk_layernorm: weight and bias are required");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (launch_layernorm<T, false>(x, y, bias, weight, 0, rows, rows, h, eps, stream)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
@@ -759,8 +730,7 @@ extern "C" int dk_ln_modulate(dk_ctx* ctx, int dtype, const void* x, void* y, co
 extern "C" int dk_qk_norm_rope(dk_ctx* ctx, int dtype, void* qkv, int rows, int S, int heads, int d, int split,
                                const void* q_w, const void* k_w, const void* q_w2, const void* k_w2, const float* rope,
                                float eps, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_qk_norm_rope: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(d == 64 || d == 128, "dk_qk_norm_rope: head dim %d unsupported (64 or 128)", d);
   DK_REQUIRE(rows > 0 && S > 0 && rows % S == 0, "dk_qk_norm_rope: rows %d must be a multiple of S %d", rows, S);
@@ -785,25 +755,23 @@ extern "C" int dk_qk_norm_rope(dk_ctx* ctx, int dtype, void* qkv, int rows, int 
 
 extern "C" int dk_silu_add(dk_ctx* ctx, int dtype, const void* y, const void* temb, void* c, int n_t, int B, int h,
                            void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_silu_add: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(h % 8 == 0, "dk_silu_add: h must be a multiple of 8");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const long long nvec = static_cast<long long>(n_t) * B * h / 8;
-  DK_DISPATCH(dtype, (silu_add_kernel<T><<<grid_for(nvec, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (silu_add_kernel<T><<<dk_grid_for(nvec, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(y), static_cast<const T*>(temb), static_cast<T*>(c), n_t, B, h)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
 
 extern "C" int dk_act(dk_ctx* ctx, int dtype, const void* x, void* y, long long n, int act, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_act: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(n % 8 == 0, "dk_act: n must be a multiple of 8");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (act_kernel<T><<<grid_for(n / 8, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (act_kernel<T><<<dk_grid_for(n / 8, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(x), static_cast<T*>(y), n, act)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
@@ -811,13 +779,12 @@ extern "C" int dk_act(dk_ctx* ctx, int dtype, const void* x, void* y, long long 
 
 extern "C" int dk_patchify(dk_ctx* ctx, int dtype, const void* latent, void* rows, int B, int H, int W, int C, int order,
                            void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_patchify: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(H % 2 == 0 && W % 2 == 0, "dk_patchify: latent size must be even (got %dx%d)", H, W);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const long long total = static_cast<long long>(B) * H * W * C;
-  DK_DISPATCH(dtype, (patchify_kernel<T><<<grid_for(total, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (patchify_kernel<T><<<dk_grid_for(total, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(latent), static_cast<T*>(rows), B, H, W, C, order)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
@@ -825,13 +792,12 @@ extern "C" int dk_patchify(dk_ctx* ctx, int dtype, const void* latent, void* row
 
 extern "C" int dk_unpatchify(dk_ctx* ctx, int dtype, const void* rows, void* latent, int B, int H, int W, int C,
                              int order, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_unpatchify: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(H % 2 == 0 && W % 2 == 0, "dk_unpatchify: latent size must be even (got %dx%d)", H, W);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const long long total = static_cast<long long>(B) * H * W * C;
-  DK_DISPATCH(dtype, (unpatchify_kernel<T><<<grid_for(total, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (unpatchify_kernel<T><<<dk_grid_for(total, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(rows), static_cast<T*>(latent), B, H, W, C, order)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
@@ -839,14 +805,13 @@ extern "C" int dk_unpatchify(dk_ctx* ctx, int dtype, const void* rows, void* lat
 
 extern "C" int dk_pos_embed_crop(dk_ctx* ctx, int dtype, const void* table, void* out, int max_hw, int hp, int wp, int h,
                                  void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_pos_embed_crop: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(hp <= max_hw && wp <= max_hw, "dk_pos_embed_crop: %dx%d exceeds the %d table", hp, wp, max_hw);
   DK_REQUIRE(h % 8 == 0, "dk_pos_embed_crop: h must be a multiple of 8");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const long long nvec = static_cast<long long>(hp) * wp * h / 8;
-  DK_DISPATCH(dtype, (pos_embed_crop_kernel<T><<<grid_for(nvec, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (pos_embed_crop_kernel<T><<<dk_grid_for(nvec, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(table), static_cast<T*>(out), max_hw, hp, wp, h)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
@@ -854,13 +819,12 @@ extern "C" int dk_pos_embed_crop(dk_ctx* ctx, int dtype, const void* table, void
 
 extern "C" int dk_copy_rows(dk_ctx* ctx, int dtype, const void* src, void* dst, int B, int rows, int h, int dst_rows,
                             int dst_off, int src_rows, int src_off, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_copy_rows: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(h % 8 == 0, "dk_copy_rows: h must be a multiple of 8");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const long long nvec = static_cast<long long>(B) * rows * h / 8;
-  DK_DISPATCH(dtype, (copy_rows_kernel<T><<<grid_for(nvec, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (copy_rows_kernel<T><<<dk_grid_for(nvec, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(src), static_cast<T*>(dst), B, rows, h, dst_rows, dst_off, src_rows,
                          src_off)));
   DK_LAUNCH_CHECK(ctx);
@@ -869,11 +833,10 @@ extern "C" int dk_copy_rows(dk_ctx* ctx, int dtype, const void* src, void* dst, 
 
 extern "C" int dk_sampler_prepare(dk_ctx* ctx, int dtype, const float* x, void* xin, long long n_per_rep, int reps,
                                   void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_sampler_prepare: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (sampler_prepare_kernel<T><<<grid_for(n_per_rep, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (sampler_prepare_kernel<T><<<dk_grid_for(n_per_rep, 256, ctx->sm_count), 256, 0, stream>>>(
                          x, static_cast<T*>(xin), n_per_rep, reps)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
@@ -881,37 +844,34 @@ extern "C" int dk_sampler_prepare(dk_ctx* ctx, int dtype, const float* x, void* 
 
 extern "C" int dk_sampler_step(dk_ctx* ctx, int dtype, float* x, const void* xin, const void* out, long long n,
                                float sigma, float sigma_next, float cfg_weight, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_sampler_step: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(sigma != 0.f, "dk_sampler_step: sigma must be non-zero");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (sampler_step_kernel<T><<<grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (sampler_step_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
                          x, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, sigma_next, cfg_weight)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
 
 extern "C" int dk_axpb_f32(dk_ctx* ctx, const float* x, float* y, long long n, float a, float b, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_axpb_f32: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  axpb_kernel<<<grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(x, y, n, a, b);
+  axpb_kernel<<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(x, y, n, a, b);
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
 
 extern "C" int dk_dequant_q4(dk_ctx* ctx, int dtype, const uint32_t* wq, const void* scales, const void* biases,
                              void* out, long long N, int K, int group_size, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_dequant_q4: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(N > 0 && K > 0, "dk_dequant_q4: empty weight");
   DK_REQUIRE(group_size >= 8 && group_size % 8 == 0 && K % group_size == 0,
              "dk_dequant_q4: K (%d) must be a multiple of group_size (%d), itself a multiple of 8", K, group_size);
-  DK_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15u) == 0, "dk_dequant_q4: out must be 16-byte aligned");
+  DK_REQUIRE(dk_aligned16(out), "dk_dequant_q4: out must be 16-byte aligned");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (dequant_q4_kernel<T><<<grid_for(N * (K / 8), 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (dequant_q4_kernel<T><<<dk_grid_for(N * (K / 8), 256, ctx->sm_count), 256, 0, stream>>>(
                          wq, static_cast<const T*>(scales), static_cast<const T*>(biases), static_cast<T*>(out), N, K,
                          group_size)));
   DK_LAUNCH_CHECK(ctx);
@@ -920,13 +880,12 @@ extern "C" int dk_dequant_q4(dk_ctx* ctx, int dtype, const uint32_t* wq, const v
 
 extern "C" int dk_image_pre(dk_ctx* ctx, int dtype, const uint8_t* img, void* out, long long pixels, int src_channels,
                             int cpad, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_image_pre: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(src_channels >= 3, "dk_image_pre: image needs at least 3 channels (got %d)", src_channels);
   DK_REQUIRE(cpad >= 8 && cpad % 8 == 0, "dk_image_pre: cpad (%d) must be a positive multiple of 8", cpad);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (image_pre_kernel<T><<<grid_for(pixels * (cpad / 8), 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (image_pre_kernel<T><<<dk_grid_for(pixels * (cpad / 8), 256, ctx->sm_count), 256, 0, stream>>>(
                          img, static_cast<T*>(out), pixels, src_channels, cpad)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
@@ -934,42 +893,38 @@ extern "C" int dk_image_pre(dk_ctx* ctx, int dtype, const uint8_t* img, void* ou
 
 extern "C" int dk_axpby_f32(dk_ctx* ctx, const float* x, const float* y, float* out, long long n, float a, float b,
                             void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_axpby_f32: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  axpby_kernel<<<grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(x, y, out, n, a, b);
+  axpby_kernel<<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(x, y, out, n, a, b);
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
 
 extern "C" int dk_vae_sample_latent(dk_ctx* ctx, int dtype, const void* hidden, const float* noise, float* out,
                                     long long pixels, int C, float shift, float scale, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_vae_sample_latent: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (vae_sample_latent_kernel<T><<<grid_for(pixels * C, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (vae_sample_latent_kernel<T><<<dk_grid_for(pixels * C, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(hidden), noise, out, pixels, C, shift, scale)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
 
 extern "C" int dk_cast_f32_to_16(dk_ctx* ctx, int dtype, const float* x, void* y, long long n, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_cast_f32_to_16: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (cast_f32_to_16_kernel<T><<<grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (cast_f32_to_16_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
                          x, static_cast<T*>(y), n)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
 extern "C" int dk_cast_16_to_f32(dk_ctx* ctx, int dtype, const void* x, float* y, long long n, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_cast_16_to_f32: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (cast_16_to_f32_kernel<T><<<grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (cast_16_to_f32_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(x), y, n)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
@@ -979,8 +934,7 @@ extern "C" int dk_groupnorm_ws_floats(int B, int G) { return B * GN_MAX_CHUNKS *
 
 extern "C" int dk_groupnorm_stats(dk_ctx* ctx, int dtype, const void* x, float* stats, float* ws, int B, int HW, int C,
                                   int G, float eps, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_groupnorm_stats: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(C % 8 == 0 && C % G == 0 && C <= 2048, "dk_groupnorm_stats: C=%d G=%d unsupported", C, G);
   DK_REQUIRE(ws != nullptr, "dk_groupnorm_stats: workspace of dk_groupnorm_ws_floats(B, G) floats required");
@@ -998,8 +952,7 @@ extern "C" int dk_groupnorm_stats(dk_ctx* ctx, int dtype, const void* x, float* 
 
 extern "C" int dk_groupnorm_finalize(dk_ctx* ctx, const float* partial, float* stats, int B, int G, int slots,
                                      double count, float eps, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_groupnorm_finalize: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_REQUIRE(partial != nullptr && stats != nullptr && B > 0 && G > 0 && slots > 0 && count > 0,
              "dk_groupnorm_finalize: bad arguments");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -1010,8 +963,7 @@ extern "C" int dk_groupnorm_finalize(dk_ctx* ctx, const float* partial, float* s
 
 extern "C" int dk_groupnorm_apply(dk_ctx* ctx, int dtype, const void* x, void* y, const float* stats, const void* gamma,
                                   const void* beta, int B, int HW, int C, int G, int silu, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_groupnorm_apply: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(C % 8 == 0 && C % G == 0 && C <= 2048, "dk_groupnorm_apply: C=%d G=%d unsupported", C, G);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -1030,8 +982,7 @@ extern "C" int dk_groupnorm_apply(dk_ctx* ctx, int dtype, const void* x, void* y
 
 extern "C" int dk_upsample_nearest2x(dk_ctx* ctx, int dtype, const void* x, void* y, int B, int H, int W, int C,
                                      void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_upsample_nearest2x: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(C % 8 == 0, "dk_upsample_nearest2x: C must be a multiple of 8");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -1045,8 +996,7 @@ extern "C" int dk_upsample_nearest2x(dk_ctx* ctx, int dtype, const void* x, void
 
 extern "C" int dk_softmax_rows(dk_ctx* ctx, int dtype, void* x, long long rows, int n, long long ld, float scale,
                                void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_softmax_rows: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(n % 8 == 0 && ld % 8 == 0, "dk_softmax_rows: n and ld must be multiples of 8");
   DK_REQUIRE(rows > 0 && rows < (1LL << 31), "dk_softmax_rows: bad row count");
@@ -1059,11 +1009,10 @@ extern "C" int dk_softmax_rows(dk_ctx* ctx, int dtype, void* x, long long rows, 
 
 extern "C" int dk_image_post(dk_ctx* ctx, int dtype, const void* x, int c_stride, float* img_f32, uint8_t* img_u8,
                              long long pixels, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_image_post: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (image_post_kernel<T><<<grid_for(pixels * 3, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (image_post_kernel<T><<<dk_grid_for(pixels * 3, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(x), c_stride, img_f32, img_u8, pixels)));
   DK_LAUNCH_CHECK(ctx);
   return 0;

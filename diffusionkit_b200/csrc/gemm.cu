@@ -211,8 +211,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // host side
 // ------------------------------------------------------------------------------------------------
 template <typename T, int BN, bool B_MN, int MODE>
-static int launch_gemm_inst(dk_ctx* ctx, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s,
-                            const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
+static int launch_gemm_inst(const char* fn, dk_ctx* ctx, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                            const GemmShape& s, const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
   auto kern = gemm_wgmma_kernel<T, BN, B_MN, MODE>;
   cudaLaunchAttribute cluster;
@@ -228,12 +228,12 @@ static int launch_gemm_inst(dk_ctx* ctx, const CUtensorMap& tmA, const CUtensorM
   cfg.attrs = &cluster;
   cfg.numAttrs = 1;
   // resident clusters: a GPC whose SM count is odd leaves one SM without a partner
-  static int max_clusters = 0;
+  int& max_clusters = ctx->max_clusters[reinterpret_cast<const void*>(kern)];
   if (max_clusters == 0) {
-    DK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    if (int rc = dk_kernel_smem(ctx, reinterpret_cast<const void*>(kern), Cfg::SMEM_BYTES)) return rc;
     int n = 0;
     DK_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
-    DK_REQUIRE(n > 0, "dk_gemm: no 2-CTA cluster of the GEMM kernel fits on the device");
+    DK_REQUIRE(n > 0, "%s: no 2-CTA cluster of the GEMM kernel fits on the device", fn);
     max_clusters = n;
   }
   const int cluster_tiles = dk_ceil_div(s.num_m, CLUSTER) * s.num_n;
@@ -244,11 +244,11 @@ static int launch_gemm_inst(dk_ctx* ctx, const CUtensorMap& tmA, const CUtensorM
 }
 
 template <typename T, bool B_MN, int MODE>
-static int launch_gemm_bn(dk_ctx* ctx, int bn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s,
-                          const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
-  if (bn == 256) return launch_gemm_inst<T, 256, B_MN, MODE>(ctx, tmA, tmB, s, e, g, stream);
-  if (bn == 128) return launch_gemm_inst<T, 128, B_MN, MODE>(ctx, tmA, tmB, s, e, g, stream);
-  return launch_gemm_inst<T, 64, B_MN, MODE>(ctx, tmA, tmB, s, e, g, stream);
+static int launch_gemm_bn(const char* fn, dk_ctx* ctx, int bn, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                          const GemmShape& s, const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
+  if (bn == 256) return launch_gemm_inst<T, 256, B_MN, MODE>(fn, ctx, tmA, tmB, s, e, g, stream);
+  if (bn == 128) return launch_gemm_inst<T, 128, B_MN, MODE>(fn, ctx, tmA, tmB, s, e, g, stream);
+  return launch_gemm_inst<T, 64, B_MN, MODE>(fn, ctx, tmA, tmB, s, e, g, stream);
 }
 
 // Tile-N choice: 256 wide tiles keep the shared-memory operand traffic per MMA lowest; fall back to narrower tiles
@@ -263,24 +263,22 @@ static int pick_bn(const dk_ctx* ctx, int num_m, int N) {
   return (tiles256 * 2 > ctx->sm_count) ? 256 : 128;
 }
 
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 }  // namespace dk
 
 using namespace dk;
 
 extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
-  DK_REQUIRE(ctx != nullptr && a != nullptr, "dk_gemm: null argument");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
+  DK_REQUIRE(a != nullptr, "dk_gemm: null argument");
+  DK_DTYPE_OK(a->dtype);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_REQUIRE(a->dtype == DK_BF16 || a->dtype == DK_FP16, "dk_gemm: bad dtype %d", a->dtype);
   DK_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0, "dk_gemm: empty problem M=%d N=%d K=%d", a->M, a->N, a->K);
   DK_REQUIRE(a->N % 8 == 0 && a->K % 8 == 0, "dk_gemm: N (%d) and K (%d) must be multiples of 8", a->N, a->K);
   DK_REQUIRE(a->lda % 8 == 0 && a->ldw % 8 == 0 && a->ldc % 8 == 0, "dk_gemm: leading dims must be multiples of 8");
-  DK_REQUIRE(aligned16(a->A) && aligned16(a->W) && aligned16(a->out), "dk_gemm: A/W/out must be 16-byte aligned");
-  DK_REQUIRE(a->bias == nullptr || aligned16(a->bias), "dk_gemm: bias must be 16-byte aligned");
-  DK_REQUIRE(a->gate == nullptr || (aligned16(a->gate) && a->gate_ld % 8 == 0), "dk_gemm: gate alignment");
-  DK_REQUIRE(a->res == nullptr || (aligned16(a->res) && a->ldres % 8 == 0), "dk_gemm: residual alignment");
+  DK_REQUIRE(dk_aligned16(a->A) && dk_aligned16(a->W) && dk_aligned16(a->out), "dk_gemm: A/W/out must be 16-byte aligned");
+  DK_REQUIRE(a->bias == nullptr || dk_aligned16(a->bias), "dk_gemm: bias must be 16-byte aligned");
+  DK_REQUIRE(a->gate == nullptr || (dk_aligned16(a->gate) && a->gate_ld % 8 == 0), "dk_gemm: gate alignment");
+  DK_REQUIRE(a->res == nullptr || (dk_aligned16(a->res) && a->ldres % 8 == 0), "dk_gemm: residual alignment");
 
   GemmShape s = {};
   s.M = a->M;
@@ -316,7 +314,7 @@ extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
     DK_REQUIRE(a->N == 3 * e.qk_h && e.qk_h % 128 == 0, "dk_gemm: fused QK epilogue needs N == 3*heads*d, heads*d %% 128 == 0");
     DK_REQUIRE(!a->w_n_major && a->act == DK_ACT_NONE && a->gate == nullptr && a->res == nullptr,
                "dk_gemm: fused QK epilogue excludes act/gate/residual");
-    DK_REQUIRE(a->qk_rope == nullptr || (reinterpret_cast<uintptr_t>(a->qk_rope) & 15u) == 0, "dk_gemm: rope table alignment");
+    DK_REQUIRE(a->qk_rope == nullptr || dk_aligned16(a->qk_rope), "dk_gemm: rope table alignment");
   }
   ConvGeom g = {};
 
@@ -339,27 +337,23 @@ extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
     if (int rc = dk_make_tmap_16b(ctx, &tmB, a->W, 2, dims, strides, box)) return rc;
   }
 
-  if (a->dtype == DK_BF16) {
-    if (a->w_n_major) return launch_gemm_inst<__nv_bfloat16, 128, true, 0>(ctx, tmA, tmB, s, e, g, stream);
-    return launch_gemm_bn<__nv_bfloat16, false, 0>(ctx, bn, tmA, tmB, s, e, g, stream);
-  } else {
-    if (a->w_n_major) return launch_gemm_inst<__half, 128, true, 0>(ctx, tmA, tmB, s, e, g, stream);
-    return launch_gemm_bn<__half, false, 0>(ctx, bn, tmA, tmB, s, e, g, stream);
-  }
+  DK_DISPATCH(a->dtype, {
+    if (a->w_n_major) return launch_gemm_inst<T, 128, true, 0>(__func__, ctx, tmA, tmB, s, e, g, stream);
+    return launch_gemm_bn<T, false, 0>(__func__, ctx, bn, tmA, tmB, s, e, g, stream);
+  });
 }
 
-static int conv3x3_impl(dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias, const void* res,
-                        void* out, int B, int Hin, int Win, int Cin, int Cout, int stride, cudaStream_t stream) {
-  DK_REQUIRE(ctx != nullptr, "dk_conv3x3: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
-  DK_REQUIRE(dtype == DK_BF16 || dtype == DK_FP16, "dk_conv3x3: bad dtype %d", dtype);
-  DK_REQUIRE(B > 0 && Hin > 0 && Win > 0, "dk_conv3x3: empty input");
-  DK_REQUIRE(Cin % 64 == 0, "dk_conv3x3: Cin (%d) must be a multiple of 64 (pad the channels)", Cin);
-  DK_REQUIRE(Cout % 8 == 0, "dk_conv3x3: Cout (%d) must be a multiple of 8 (pad the filters)", Cout);
-  DK_REQUIRE(aligned16(x) && aligned16(w) && aligned16(out), "dk_conv3x3: x/w/out must be 16-byte aligned");
-  DK_REQUIRE(bias == nullptr || aligned16(bias), "dk_conv3x3: bias alignment");
-  DK_REQUIRE(res == nullptr || aligned16(res), "dk_conv3x3: residual alignment");
-  DK_REQUIRE(stride == 1 || (Hin % 2 == 0 && Win % 2 == 0), "dk_conv3x3_s2: input size must be even (got %dx%d)", Hin, Win);
+// The entry point named fn has run DK_ENTRY and DK_DTYPE_OK.
+static int conv3x3_impl(const char* fn, dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias,
+                        const void* res, void* out, int B, int Hin, int Win, int Cin, int Cout, int stride,
+                        cudaStream_t stream) {
+  DK_REQUIRE(B > 0 && Hin > 0 && Win > 0, "%s: empty input", fn);
+  DK_REQUIRE(Cin % 64 == 0, "%s: Cin (%d) must be a multiple of 64 (pad the channels)", fn, Cin);
+  DK_REQUIRE(Cout % 8 == 0, "%s: Cout (%d) must be a multiple of 8 (pad the filters)", fn, Cout);
+  DK_REQUIRE(dk_aligned16(x) && dk_aligned16(w) && dk_aligned16(out), "%s: x/w/out must be 16-byte aligned", fn);
+  DK_REQUIRE(bias == nullptr || dk_aligned16(bias), "%s: bias alignment", fn);
+  DK_REQUIRE(res == nullptr || dk_aligned16(res), "%s: residual alignment", fn);
+  DK_REQUIRE(stride == 1 || (Hin % 2 == 0 && Win % 2 == 0), "%s: input size must be even (got %dx%d)", fn, Hin, Win);
 
   const int H = Hin / stride, W = Win / stride;   // output size
   ConvGeom g;
@@ -407,7 +401,7 @@ static int conv3x3_impl(dk_ctx* ctx, int dtype, const void* x, const void* w, co
     // strided traversal: N elements with stride s need a box entry of N * s
     const uint32_t box[4] = {BK, static_cast<uint32_t>(g.TW * stride), static_cast<uint32_t>(g.TH * stride), 1};
     const uint32_t estr[4] = {1, static_cast<uint32_t>(stride), static_cast<uint32_t>(stride), 1};
-    DK_REQUIRE(box[1] <= 256 && box[2] <= 256, "dk_conv3x3: TMA box too large");
+    DK_REQUIRE(box[1] <= 256 && box[2] <= 256, "%s: TMA box too large", fn);
     if (int rc = dk_make_tmap_16b(ctx, &tmA, x, 4, dims, strides, box, estr)) return rc;
   }
   {
@@ -416,16 +410,21 @@ static int conv3x3_impl(dk_ctx* ctx, int dtype, const void* x, const void* w, co
     const uint32_t box[2] = {BK, static_cast<uint32_t>(bn / CLUSTER)};
     if (int rc = dk_make_tmap_16b(ctx, &tmB, w, 2, dims, strides, box)) return rc;
   }
-  if (dtype == DK_BF16) return launch_gemm_bn<__nv_bfloat16, false, 1>(ctx, bn, tmA, tmB, s, e, g, stream);
-  return launch_gemm_bn<__half, false, 1>(ctx, bn, tmA, tmB, s, e, g, stream);
+  DK_DISPATCH(dtype, return launch_gemm_bn<T, false, 1>(fn, ctx, bn, tmA, tmB, s, e, g, stream));
 }
 
 extern "C" int dk_conv3x3(dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias, const void* res,
                           void* out, int B, int H, int W, int Cin, int Cout, void* stream_) {
-  return conv3x3_impl(ctx, dtype, x, w, bias, res, out, B, H, W, Cin, Cout, 1, static_cast<cudaStream_t>(stream_));
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  return conv3x3_impl(__func__, ctx, dtype, x, w, bias, res, out, B, H, W, Cin, Cout, 1,
+                      static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int dk_conv3x3_s2(dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias, void* out, int B,
                              int H, int W, int Cin, int Cout, void* stream_) {
-  return conv3x3_impl(ctx, dtype, x, w, bias, nullptr, out, B, H, W, Cin, Cout, 2, static_cast<cudaStream_t>(stream_));
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  return conv3x3_impl(__func__, ctx, dtype, x, w, bias, nullptr, out, B, H, W, Cin, Cout, 2,
+                      static_cast<cudaStream_t>(stream_));
 }

@@ -1,33 +1,12 @@
 // Kernels of the text-encoder path (SURVEY.md §8 row f2): CLIP-L/G and the T5-XXL encoder.  The projections and MLPs
-// run on the wgmma GEMM (gemm.cu); this file holds what sits between them: embedding lookup, LayerNorm
-// with affine, T5's RMSNorm over the fp32 residual stream, the gated-GELU product, and attention for short sequences
+// run on the wgmma GEMM (gemm.cu); this file holds what sits between them: embedding lookup, T5's
+// RMSNorm over the fp32 residual stream, the gated-GELU product, and attention for short sequences
 // (S <= 512, head dim 64) with CLIP's causal mask or T5's relative-position bias.  All are small next to the denoise
 // path (T5-XXL at 512 tokens: 4.3 GFLOP of attention per layer against 0.6 TFLOP of GEMM).
 #include "common.cuh"
 #include "host.h"
 
 namespace dk {
-
-template <typename T>
-__device__ __forceinline__ void t_load8(const T* p, float (&v)[8]) {
-  const uint4 u = *reinterpret_cast<const uint4*>(p);
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 f = Half16<T>::unpack(w[i]);
-    v[2 * i] = f.x;
-    v[2 * i + 1] = f.y;
-  }
-}
-template <typename T>
-__device__ __forceinline__ void t_store8(T* p, const float (&v)[8]) {
-  uint4 o;
-  o.x = Half16<T>::pack(v[0], v[1]);
-  o.y = Half16<T>::pack(v[2], v[3]);
-  o.z = Half16<T>::pack(v[4], v[5]);
-  o.w = Half16<T>::pack(v[6], v[7]);
-  *reinterpret_cast<uint4*>(p) = o;
-}
 
 // ------------------------------------------------------------------------------------------------
 // token (+ position) embedding: out[i] = table[ids[i]] (+ pos[i % L])      reference mlx/clip.py:97-98, t5.py:322
@@ -42,68 +21,14 @@ __global__ void embedding_kernel(const T* __restrict__ table, const int* __restr
     const long long r = i / vpr;
     const int c = static_cast<int>(i - r * vpr) * 8;
     float a[8];
-    t_load8(table + static_cast<long long>(ids[r]) * d + c, a);
+    load8(table + static_cast<long long>(ids[r]) * d + c, a);
     if (pos != nullptr) {
       float p[8];
-      t_load8(pos + static_cast<long long>(r % L) * d + c, p);
+      load8(pos + static_cast<long long>(r % L) * d + c, p);
 #pragma unroll
       for (int j = 0; j < 8; ++j) a[j] += p[j];
     }
-    t_store8(out + r * d + c, a);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// LayerNorm with learned affine (mlx nn.LayerNorm -> mx.fast.layer_norm: biased variance, fp32 accumulation),
-// one warp per row, row in registers.     reference mlx/clip.py:32-33,78 (eps 1e-5, the mlx default)
-// ------------------------------------------------------------------------------------------------
-constexpr int TLN_WARPS = 4;
-template <typename T, int NV>
-__global__ void __launch_bounds__(TLN_WARPS * 32)
-layernorm_affine_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ w, const T* __restrict__ b,
-                        int rows, int h, float eps) {
-  const int row = blockIdx.x * TLN_WARPS + (threadIdx.x >> 5);
-  if (row >= rows) return;
-  const int lane = threadIdx.x & 31;
-  const T* xr = x + static_cast<long long>(row) * h;
-  T* yr = y + static_cast<long long>(row) * h;
-  const int nvec = h / 8;
-  float v[NV][8];
-  float s = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int vec = lane + i * 32;
-    if (vec < nvec) {
-      t_load8(xr + vec * 8, v[i]);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s += v[i][j];
-    }
-  }
-  const float mean = warp_sum(s) / h;
-  float q = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int vec = lane + i * 32;
-    if (vec < nvec) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float dlt = v[i][j] - mean;
-        q += dlt * dlt;
-      }
-    }
-  }
-  const float rstd = rsqrtf(warp_sum(q) / h + eps);
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int vec = lane + i * 32;
-    if (vec < nvec) {
-      float a[8], c[8], o[8];
-      t_load8(w + vec * 8, a);
-      t_load8(b + vec * 8, c);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = (v[i][j] - mean) * rstd * a[j] + c[j];
-      t_store8(yr + vec * 8, o);
-    }
+    store8(out + r * d + c, a);
   }
 }
 
@@ -155,7 +80,7 @@ __global__ void add_f32_16_kernel(float* __restrict__ x, const T* __restrict__ y
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float a[8];
-    t_load8(y + i * 8, a);
+    load8(y + i * 8, a);
     float4* xp = reinterpret_cast<float4*>(x + i * 8);
     float4 lo = xp[0], hi = xp[1];
     lo.x += a[0]; lo.y += a[1]; lo.z += a[2]; lo.w += a[3];
@@ -176,11 +101,11 @@ __global__ void glu_gelu_kernel(const T* __restrict__ h, T* __restrict__ out, lo
     const long long r = i / vpr;
     const int c = static_cast<int>(i - r * vpr) * 8;
     float a[8], b[8];
-    t_load8(h + r * 2 * F + c, a);
-    t_load8(h + r * 2 * F + F + c, b);
+    load8(h + r * 2 * F + c, a);
+    load8(h + r * 2 * F + F + c, b);
 #pragma unroll
     for (int j = 0; j < 8; ++j) a[j] = gelu_erf(a[j]) * b[j];
-    t_store8(out + r * F + c, a);
+    store8(out + r * F + c, a);
   }
 }
 
@@ -290,76 +215,34 @@ attention_small_kernel(const T* __restrict__ qkv, const T* __restrict__ rel_bias
   }
 }
 
-static inline int t_grid_for(long long work_items, int threads, int sm_count) {
-  long long blocks = (work_items + threads - 1) / threads;
-  const long long cap = static_cast<long long>(sm_count) * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<int>(blocks);
+// K^T [32][Spad + 1], V [Spad][32] and the query rows of the 8 warps, in 32-bit words
+static inline int as_smem_bytes(int S) {
+  const int Spad = (S + 31) & ~31;
+  return (32 * (Spad + 1) + Spad * 32 + 8 * 32) * 4;
 }
 
 }  // namespace dk
 
 using namespace dk;
 
-#define DK_DTYPE_OK(dt) DK_REQUIRE((dt) == DK_BF16 || (dt) == DK_FP16, "%s: bad dtype %d", __func__, (dt))
-#define DK_DISPATCH(dt, ...)                      \
-  do {                                            \
-    if ((dt) == DK_BF16) {                        \
-      using T = __nv_bfloat16;                    \
-      __VA_ARGS__;                                \
-    } else {                                      \
-      using T = __half;                           \
-      __VA_ARGS__;                                \
-    }                                             \
-  } while (0)
-
 extern "C" int dk_embedding(dk_ctx* ctx, int dtype, const void* table, const int* ids, const void* pos, void* out,
                             long long n, int d, int vocab, int pos_len, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_embedding: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(n > 0 && d > 0 && d % 8 == 0, "dk_embedding: d (%d) must be a positive multiple of 8", d);
   DK_REQUIRE(vocab > 0, "dk_embedding: empty table");
   DK_REQUIRE(pos == nullptr || pos_len > 0, "dk_embedding: position table without a length");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (embedding_kernel<T><<<t_grid_for(n * (d / 8), 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (embedding_kernel<T><<<dk_grid_for(n * (d / 8), 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(table), ids, static_cast<const T*>(pos), static_cast<T*>(out), n, d,
                          pos_len > 0 ? pos_len : 1)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
 
-extern "C" int dk_layernorm(dk_ctx* ctx, int dtype, const void* x, void* y, const void* weight, const void* bias,
-                            int rows, int h, float eps, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_layernorm: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
-  DK_DTYPE_OK(dtype);
-  DK_REQUIRE(rows > 0 && h > 0 && h % 8 == 0 && h <= 4096, "dk_layernorm: h (%d) must be a multiple of 8, <= 4096", h);
-  DK_REQUIRE(weight != nullptr && bias != nullptr, "dk_layernorm: weight and bias are required");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const int blocks = dk_ceil_div(rows, TLN_WARPS);
-  const int nv = dk_ceil_div(h / 8, 32);
-  DK_DISPATCH(dtype, {
-    const T* xp = static_cast<const T*>(x);
-    T* yp = static_cast<T*>(y);
-    const T* wp = static_cast<const T*>(weight);
-    const T* bp = static_cast<const T*>(bias);
-    if (nv <= 4)
-      layernorm_affine_kernel<T, 4><<<blocks, TLN_WARPS * 32, 0, stream>>>(xp, yp, wp, bp, rows, h, eps);
-    else if (nv <= 8)
-      layernorm_affine_kernel<T, 8><<<blocks, TLN_WARPS * 32, 0, stream>>>(xp, yp, wp, bp, rows, h, eps);
-    else
-      layernorm_affine_kernel<T, 16><<<blocks, TLN_WARPS * 32, 0, stream>>>(xp, yp, wp, bp, rows, h, eps);
-  });
-  DK_LAUNCH_CHECK(ctx);
-  return 0;
-}
-
 extern "C" int dk_rmsnorm_f32(dk_ctx* ctx, int dtype, const float* x, const void* weight, void* y, int rows, int d,
                               float eps, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_rmsnorm_f32: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(rows > 0 && d > 0 && d % 4 == 0 && d <= 4096, "dk_rmsnorm_f32: d (%d) must be a multiple of 4, <= 4096", d);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -370,24 +253,22 @@ extern "C" int dk_rmsnorm_f32(dk_ctx* ctx, int dtype, const float* x, const void
 }
 
 extern "C" int dk_add_f32_16(dk_ctx* ctx, int dtype, float* x, const void* y, long long n, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_add_f32_16: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(n % 8 == 0, "dk_add_f32_16: n must be a multiple of 8");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (add_f32_16_kernel<T><<<t_grid_for(n / 8, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (add_f32_16_kernel<T><<<dk_grid_for(n / 8, 256, ctx->sm_count), 256, 0, stream>>>(
                          x, static_cast<const T*>(y), n)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
 
 extern "C" int dk_glu_gelu(dk_ctx* ctx, int dtype, const void* h, void* out, long long rows, int F, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_glu_gelu: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(rows > 0 && F > 0 && F % 8 == 0, "dk_glu_gelu: F (%d) must be a positive multiple of 8", F);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (glu_gelu_kernel<T><<<t_grid_for(rows * (F / 8), 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (glu_gelu_kernel<T><<<dk_grid_for(rows * (F / 8), 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(h), static_cast<T*>(out), rows, F)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
@@ -395,21 +276,18 @@ extern "C" int dk_glu_gelu(dk_ctx* ctx, int dtype, const void* h, void* out, lon
 
 extern "C" int dk_attention_small(dk_ctx* ctx, int dtype, const void* qkv, const void* rel_bias, void* out, int B, int S,
                                   int heads, int head_dim, float scale, int causal, void* stream_) {
-  DK_REQUIRE(ctx != nullptr, "dk_attention_small: null ctx");
-  DkDeviceGuard dk_guard_(ctx);
+  DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(head_dim == 64, "dk_attention_small: head dim %d unsupported (64)", head_dim);
   DK_REQUIRE(B > 0 && heads > 0 && S > 0 && S <= AS_MAX_S, "dk_attention_small: S (%d) must be in [1, %d]", S, AS_MAX_S);
-  DK_REQUIRE((reinterpret_cast<uintptr_t>(qkv) & 15u) == 0, "dk_attention_small: qkv must be 16-byte aligned");
+  DK_REQUIRE(dk_aligned16(qkv), "dk_attention_small: qkv must be 16-byte aligned");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const int Spad = (S + 31) & ~31;
-  const size_t smem = (static_cast<size_t>(32) * (Spad + 1) + static_cast<size_t>(Spad) * 32 + 8 * 32) * 4;
   const dim3 grid(dk_ceil_div(S, AS_QB), heads, B);
   DK_DISPATCH(dtype, {
-    DK_CHECK_CUDA(cudaFuncSetAttribute(attention_small_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(smem)));
-    attention_small_kernel<T><<<grid, 256, smem, stream>>>(static_cast<const T*>(qkv), static_cast<const T*>(rel_bias),
-                                                           static_cast<T*>(out), S, heads, scale, causal);
+    auto kern = attention_small_kernel<T>;
+    if (int rc = dk_kernel_smem(ctx, reinterpret_cast<const void*>(kern), as_smem_bytes(AS_MAX_S))) return rc;
+    kern<<<grid, 256, as_smem_bytes(S), stream>>>(static_cast<const T*>(qkv), static_cast<const T*>(rel_bias),
+                                                  static_cast<T*>(out), S, heads, scale, causal);
   });
   DK_LAUNCH_CHECK(ctx);
   return 0;
