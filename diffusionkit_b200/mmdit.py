@@ -65,6 +65,8 @@ class MMDiT:
         # (timestep-invariant) forward that bakes in their pointers
         self._shapes = ShapeCache()
         self.use_cuda_graphs, self.max_cached_shapes = default_settings()
+        # packed tensors a LoRA merge has touched: (id(owner), attribute, tuple index) -> (owner, base, live)
+        self._lora_live: Dict[Tuple[int, str, Optional[int]], Tuple[object, torch.Tensor, torch.Tensor]] = {}
 
     # ------------------------------------------------------------------------------------------ weight packing
     def _pack(self, P: Dict[str, torch.Tensor]):
@@ -193,6 +195,116 @@ class MMDiT:
     def _mod(self, s_off: int, k: int) -> torch.Tensor:
         """k-th h-wide modulation vector of a block: view (B, h) with row stride mod_total."""
         return self._mod_cur[:, s_off + k * self.h: s_off + (k + 1) * self.h]
+
+    # ------------------------------------------------------------------------------------------ LoRA merge
+    def lora_weight_slots(self) -> Dict[str, Tuple[object, str, Optional[int], slice, slice]]:
+        """reference weight name -> (owner, attribute, tuple index or None, rows, columns): where each weight a LoRA
+        adapter can change lives inside the packed tensors."""
+        h, everything = self.h, slice(None)
+        slots = {}
+
+        def put(name, owner, attr, idx=None, rows=everything, cols=everything):
+            slots[name + ".weight"] = (owner, attr, idx, rows, cols)
+
+        put("x_embedder.proj", self, "w_x")
+        put("context_embedder", self, "w_ctx")
+        for emb in ("y", "t"):
+            put(f"{emb}_embedder.mlp.layers.0", self, emb + "0", 0)
+            put(f"{emb}_embedder.mlp.layers.2", self, emb + "2", 0)
+        put("final_layer.linear", self, "w_final")
+        put("final_layer.adaLN_modulation.layers.1", self, "w_mod",
+            rows=slice(self.final_mod_off, self.final_mod_off + 2 * h))
+        for s in [s for pair in self.double for s in pair] + self.single:
+            p = s.name
+            for j, n in enumerate("qkv"):
+                put(f"{p}.attn.{n}_proj", s, "w_qkv", rows=slice(j * h, (j + 1) * h))
+            put(f"{p}.adaLN_modulation.layers.1", self, "w_mod", rows=slice(s.mod_off, s.mod_off + s.n_mod * h))
+            if s.skip_post:
+                continue
+            put(f"{p}.mlp.fc1", s, "w_fc1")
+            if s.w_out is not None:                                                    # [Wo | W2] column windows
+                put(f"{p}.attn.o_proj", s, "w_out", cols=slice(0, h))
+                put(f"{p}.mlp.fc2", s, "w_out", cols=slice(h, None))
+            else:
+                put(f"{p}.attn.o_proj", s, "w_o")
+                put(f"{p}.mlp.fc2", s, "w_fc2")
+        return slots
+
+    @staticmethod
+    def _bound(owner, attr: str, idx: Optional[int]) -> torch.Tensor:
+        t = getattr(owner, attr)
+        return t if idx is None else t[idx]
+
+    @staticmethod
+    def _rebind(owner, attr: str, idx: Optional[int], t: torch.Tensor):
+        if idx is not None:
+            old = getattr(owner, attr)
+            t = old[:idx] + (t,) + old[idx + 1:]
+        setattr(owner, attr, t)
+
+    def apply_lora(self, stack):
+        """Merge a stack of LoRA adapters, a sequence of (lora.LoRA, scale), into the weights:
+        W = round16(W_base + Σ round16(scale·up) @ round16(down)), one wgmma GEMM per weight with W_base as its
+        residual.  The forward runs exactly the kernels it runs without adapters.
+
+        A packed tensor the stack touches keeps its current tensor as the base, which is never written (it may be the
+        caller's), and gets a live copy the forward reads.  Applying another stack re-merges from the bases in place,
+        so captured CUDA graphs stay valid when only scales change; tensors the stack no longer touches go back to
+        their base and their live copy is freed (an empty stack frees them all).  Binding a live copy or a base drops
+        the captured graphs.  A merge that changes the adaLN or t / y embedder weights clears the modulation cache:
+        call cache_modulation_params again before the next forward."""
+        slots = self.lora_weight_slots()
+        terms: Dict[str, list] = {}
+        for lora, scale in stack:
+            scale = float(scale)
+            if not math.isfinite(scale):
+                raise ValueError(f"LoRA {lora.name}: scale must be finite, got {scale}")
+            for name, (up, down) in lora.targets.items():
+                if name not in slots:
+                    raise KeyError(f"LoRA {lora.name}: the model has no weight {name}")
+                terms.setdefault(name, []).append((scale, up, down))
+        touched = {}
+        for name in terms:
+            owner, attr, idx = slots[name][:3]
+            touched[(id(owner), attr, idx)] = (owner, attr, idx)
+        rebound, mod_changed = False, False
+        for key in [k for k in self._lora_live if k not in touched]:
+            owner, base, _ = self._lora_live.pop(key)
+            self._rebind(owner, key[1], key[2], base)
+            rebound, mod_changed = True, mod_changed or key[1] in ("w_mod", "y0", "y2", "t0", "t2")
+        for key, (owner, attr, idx) in touched.items():
+            if key not in self._lora_live:
+                base = self._bound(owner, attr, idx)
+                self._lora_live[key] = (owner, base, torch.empty_like(base))
+                self._rebind(owner, attr, idx, self._lora_live[key][2])
+                rebound = True
+            _, base, live = self._lora_live[key]
+            live.copy_(base)
+            mod_changed = mod_changed or attr in ("w_mod", "y0", "y2", "t0", "t2")
+        for name, ts in terms.items():
+            owner, attr, idx, rows, cols = slots[name]
+            _, base, live = self._lora_live[(id(owner), attr, idx)]
+            up, down = self._lora_factors(ts)
+            ops.gemm(up, down, out=live[rows, cols], res=base[rows, cols], w_n_major=True)
+        if rebound:
+            self._shapes.drop_graphs()
+        if mod_changed:
+            self.clear_modulation_params_cache()
+            self._cur_t = None
+
+    def _lora_factors(self, terms) -> Tuple[torch.Tensor, torch.Tensor]:
+        """[round16(s1·up1) | round16(s2·up2) | ... | 0] and [round16(down1); round16(down2); ...; 0] on the device:
+        the ranks concatenated and zero-padded to a multiple of 8 (the GEMM's K)"""
+        r = sum(up.shape[1] for _, up, _ in terms)
+        rp = -(-r // 8) * 8
+        up = torch.zeros((terms[0][1].shape[0], rp), dtype=torch.float32)
+        down = torch.zeros((rp, terms[0][2].shape[1]), dtype=torch.float32)
+        o = 0
+        for scale, u, d in terms:
+            up[:, o:o + u.shape[1]] = u * scale
+            down[o:o + u.shape[1]] = d
+            o += u.shape[1]
+        return up.to(self.dtype).to(self.device), down.to(self.dtype).to(self.device)
 
     # ------------------------------------------------------------------------------------------ workspace
     def _workspace(self, st: dict, B: int, N: int, T: int):

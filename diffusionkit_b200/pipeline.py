@@ -176,6 +176,7 @@ class DiffusionPipeline:
         self._weight_seed = weight_seed
         self._params, self._vae_params = params, vae_params
         self._load_decoder = load_decoder
+        self._loras = {}                            # adapter name -> [lora.LoRA, scale], in load order
         self.check_and_load_models()
         self._params = self._vae_params = None      # the models hold packed copies; drop the caller's tensors
         if hasattr(self, "encoder"):
@@ -265,6 +266,57 @@ class DiffusionPipeline:
             ep = {k: v.to(device=self.device, dtype=self.dtype) for k, v in ep.items()}
         self.encoder = VAEEncoder(ep, VAEEncoderConfig(), device=self.device)
         self._vae_encoder_params = None
+
+    # ------------------------------------------------------------------ LoRA adapters (DESIGN.md §8)
+    def load_lora_weights(self, path_or_dict, scale: float = 1.0, adapter_name: Optional[str] = None) -> str:
+        """Load a kohya or PEFT LoRA (.safetensors path or state dict) for the MMDiT and merge it into the weights
+        together with the adapters already loaded.  Returns the adapter's name (default: the file name without its
+        extension, or "adapter")."""
+        from .lora import load_lora
+
+        lora = load_lora(path_or_dict, self.config, name=adapter_name)
+        if lora.name in self._loras:
+            raise ValueError(f"a LoRA adapter named {lora.name!r} is already loaded: pass another adapter_name")
+        self._loras[lora.name] = [lora, float(scale)]
+        try:
+            self._apply_loras()
+        except Exception:
+            del self._loras[lora.name]
+            self._apply_loras()
+            raise
+        return lora.name
+
+    def set_lora_scale(self, adapter_name: str, scale: float):
+        """Change one adapter's scale and re-merge the stack (in place: captured CUDA graphs keep replaying)."""
+        if adapter_name not in self._loras:
+            raise KeyError(f"no LoRA adapter named {adapter_name!r} is loaded")
+        old = self._loras[adapter_name][1]
+        self._loras[adapter_name][1] = float(scale)
+        try:
+            self._apply_loras()
+        except Exception:
+            self._loras[adapter_name][1] = old
+            self._apply_loras()
+            raise
+
+    def unload_lora_weights(self, adapter_name: Optional[str] = None):
+        """Remove one adapter (or all of them with None) and re-merge the rest; with none left the MMDiT runs on its
+        original weights again, bit for bit."""
+        if adapter_name is None:
+            self._loras.clear()
+        elif adapter_name not in self._loras:
+            raise KeyError(f"no LoRA adapter named {adapter_name!r} is loaded")
+        else:
+            del self._loras[adapter_name]
+        self._apply_loras()
+
+    @property
+    def lora_adapters(self) -> Dict[str, float]:
+        """{adapter name: scale} of the loaded adapters, in load order"""
+        return {n: s for n, (_, s) in self._loras.items()}
+
+    def _apply_loras(self):
+        self.mmdit.apply_lora([(lora, s) for lora, s in self._loras.values()])
 
     # ------------------------------------------------------------------ text (SURVEY.md §8 row f2)
     def load_text_encoders(self, clip_l=None, clip_g=None, t5=None, *, tokenizer_l=None, tokenizer_g=None,
