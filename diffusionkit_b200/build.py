@@ -14,6 +14,8 @@ NVCC_FLAGS = [
     "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
 ]
+# ptxas performance advisory: "wgmma.mma_async instructions are serialized due to ..."
+SERIALISED_WGMMA = "C7510"
 
 
 def _stale(obj, src):
@@ -38,16 +40,22 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if force or _stale(obj, src):
             cmd = [nvcc, *NVCC_FLAGS, "-c", src, "-o", obj]
             procs.append((s, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
-    failed = False
+    failed = []
     for s, p in procs:
         out, _ = p.communicate()
         if p.returncode != 0:
-            failed = True
+            failed.append(s)
             sys.stderr.write(f"[build] {s} FAILED\n{out}\n")
+        elif SERIALISED_WGMMA in out:
+            # ptxas serialised a kernel's wgmma instructions (a function call in a wgmma kernel): the code would run,
+            # only much slower, so it is refused here instead of surfacing as a silent slowdown
+            failed.append(s)
+            os.remove(os.path.join(CSRC, s.replace(".cu", ".o")))
+            sys.stderr.write(f"[build] {s} FAILED: ptxas serialised wgmma instructions ({SERIALISED_WGMMA})\n{out}\n")
         elif verbose:
             sys.stderr.write(f"[build] {s}\n{out}\n")
     if failed:
-        raise RuntimeError("nvcc failed")
+        raise RuntimeError(f"nvcc failed: {', '.join(failed)}")
     if procs or not os.path.exists(LIB):
         cmd = [nvcc, "-shared", "-Wno-deprecated-gpu-targets", "-o", LIB, *objs, "-lcudart", "-ldl"]
         subprocess.check_call(cmd)

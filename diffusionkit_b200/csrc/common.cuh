@@ -24,12 +24,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 
 
-// A kernel that dead-locks on an mbarrier hangs the whole GPU box.  Every wait therefore carries a
-// watchdog: ~4 s of SM clock, then trap (the launch fails with an error instead of hanging).
-#ifndef DK_WATCHDOG_CYCLES
-#define DK_WATCHDOG_CYCLES (8000000000LL)
-#endif
-
 // --------------------------------------------------------------------------------------------
 // mbarrier
 // --------------------------------------------------------------------------------------------
@@ -60,26 +54,14 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity
 // Wait until the phase with the given parity has completed.  try_wait suspends the thread in hardware for ~100 clocks
 // per attempt; the retry loop is kept minimal (ncu: with a clock64() watchdog in it the polling loops of the waiting
 // warps were a quarter of all instructions the attention kernel issued).  The watchdog counts attempts instead:
-// 2^26 of them is a few seconds, then the kernel traps (a launch error instead of a hung GPU box).
+// 2^26 of them is a few seconds, then the kernel traps, so a dead-locked pipeline fails its launch with an error
+// instead of hanging the GPU.  The trap is inline and the wait calls nothing: a function call anywhere in a kernel
+// makes ptxas serialise all of its wgmma instructions (warning C7510, which the build refuses), so the watchdog does
+// not report which block or barrier tripped it.
 #ifndef DK_WATCHDOG_SPINS
 #define DK_WATCHDOG_SPINS (1u << 26)
 #endif
-static __device__ __noinline__ void mbar_watchdog_trap(uint64_t* bar, uint32_t parity) {
-  printf("[dkb200] mbarrier watchdog: block (%d,%d,%d) thread %d bar@%u parity %u\n", blockIdx.x, blockIdx.y, blockIdx.z,
-         threadIdx.x, smem_u32(bar), parity);
-  __trap();
-}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++spins == DK_WATCHDOG_SPINS) mbar_watchdog_trap(bar, parity);
-  }
-}
-
-// The same wait with a call-free watchdog (trap without the report), for kernels that wait while wgmma groups are in
-// flight: a function call anywhere in such a kernel makes ptxas serialise all of its wgmma instructions.
-__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (++spins == DK_WATCHDOG_SPINS) asm volatile("trap;");

@@ -121,7 +121,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           x0 = (t % g.tiles_x) * g.TW;
         }
         for (int kb = 0; kb < s.num_k; ++kb) {
-          if (lane == 0) mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
+          if (lane == 0) mbar_wait(&empty_bar[stage], phase ^ 1);
           __syncwarp();
           if (elect_one_sync()) {
             // A (own) + the whole W tile: this CTA's half and the partner's multicast half
@@ -170,7 +170,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       cluster_tile(ct, s, rank, m_blk, n_blk);
       uint32_t prev = 0;
       for (int kb = 0; kb < s.num_k; ++kb) {
-        mbar_wait_nocall(&full_bar[stage], phase);
+        mbar_wait(&full_bar[stage], phase);
         const uint32_t a_base = smem_u32(sA + stage * A_BYTES) + cw * 64 * 128;
         const uint32_t b_base = smem_u32(sB + stage * B_BYTES);
         wgmma_fence();
