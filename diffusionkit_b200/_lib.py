@@ -50,7 +50,10 @@ SIGNATURES = {
     "dk_ctx_destroy": (None, [vp]),
     "dk_ctx_launch_count": (i64, [vp]),
     "dk_gemm": (i32, [vp, C.POINTER(GemmArgs), vp]),
+    "dk_gemm_fp8": (i32, [vp, C.POINTER(GemmArgs), vp, vp, vp]),
+    "dk_quantize_rows_e4m3": (i32, [vp, i32, vp, i64, vp, vp, i32, i32, vp]),
     "dk_ln_modulate": (i32, [vp, i32, vp, vp, vp, vp, i64, i32, i32, i32, f32, vp]),
+    "dk_ln_modulate_fp8": (i32, [vp, i32, vp, vp, vp, vp, vp, i64, i32, i32, i32, f32, vp]),
     "dk_qk_norm_rope": (i32, [vp, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, f32, vp]),
     "dk_attention_fwd": (i32, [vp, i32, vp, i32, i32, i32, i32, f32, i32, vp, i64, vp, i64, vp]),
     "dk_silu_add": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, vp]),

@@ -64,8 +64,8 @@ int dk_kernel_smem(dk_ctx* ctx, const void* func, int bytes) {
   return 0;
 }
 
-int dk_make_tmap_16b(dk_ctx* ctx, CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
-                     const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides) {
+int dk_make_tmap(dk_ctx* ctx, CUtensorMap* map, int elem_bytes, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides) {
   cuuint64_t gdim[5];
   cuuint64_t gstr[4];
   cuuint32_t bdim[5];
@@ -76,8 +76,9 @@ int dk_make_tmap_16b(dk_ctx* ctx, CUtensorMap* map, const void* base, int rank, 
     estr[i] = elem_strides ? elem_strides[i] : 1;
   }
   for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  // the data type only matters for OOB-fill / element size; bf16 and fp16 are both 2-byte tiles
-  CUresult r = ctx->encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, static_cast<cuuint32_t>(rank),
+  // the data type only matters for OOB-fill / element size; bf16 and fp16 are both 2-byte tiles, e4m3 is a byte
+  const CUtensorMapDataType type = elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUresult r = ctx->encode_tiled(map, type, static_cast<cuuint32_t>(rank),
                                  const_cast<void*>(base), gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

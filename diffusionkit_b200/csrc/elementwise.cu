@@ -1,5 +1,7 @@
 // HBM-bound kernels of the denoise + decode path: normalisations, modulation, RoPE, layout shuffles, sampler update.
 // All of them move 128-bit vectors per thread, reduce with warp shuffles, and do their arithmetic in fp32.
+#include <cuda_fp8.h>
+
 #include "common.cuh"
 #include "host.h"
 
@@ -38,12 +40,44 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 constexpr int LN_WARPS = 4;     // rows per block
 constexpr int LN_MAXV = 16;     // h <= 32 lanes * 8 * 16 = 4096
 
+// Row quantisation to e4m3: scale = amax(|row|) / 448 (1 for an all-zero row), q = cvt.rn.satfinite.e4m3(v / scale), all
+// in fp32 with IEEE division, so the result is a function of the row alone.
+__device__ __forceinline__ float e4m3_row_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, 448.0f) : 1.0f; }
+// 8 consecutive values -> 8 e4m3 bytes, one 64-bit store
+__device__ __forceinline__ void store8_e4m3(uint8_t* p, const float (&v)[8], float scale) {
+  uint32_t w[2];
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    uint32_t b[2];
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+      b[j] = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(v[4 * k + 2 * j], scale), __fdiv_rn(v[4 * k + 2 * j + 1], scale)),
+                                      __NV_SATFINITE, __NV_E4M3);
+    w[k] = b[0] | (b[1] << 16);
+  }
+  *reinterpret_cast<uint2*>(p) = make_uint2(w[0], w[1]);
+}
+// A row held by one warp in registers (vector lane + 32 i of nvec) whose lanes know their own maximum -> e4m3 + scale
+template <int NV>
+__device__ __forceinline__ void store_row_e4m3(const float (&v)[NV][8], float lane_amax, int nvec, int lane,
+                                               uint8_t* qr, float* scale_out) {
+  const float sc = e4m3_row_scale(warp_max(lane_amax));
+  if (lane == 0) *scale_out = sc;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int vec = lane + i * 32;
+    if (vec < nvec) store8_e4m3(qr + vec * 8, v[i], sc);
+  }
+}
+
 // One warp per row: the row lives in registers (<= 16 x 128-bit loads in flight per lane), statistics via warp
-// shuffles only — no shared memory, no block barriers.
-template <typename T, int NV, bool MODULATE>
+// shuffles only — no shared memory, no block barriers.  Q8: the fp32 result row is not rounded to 16 bits but
+// quantised to e4m3 (q, qscale[row]) while it is still in registers.
+template <typename T, int NV, bool MODULATE, bool Q8>
 __global__ void __launch_bounds__(LN_WARPS * 32)
 layernorm_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ shift, const T* __restrict__ scale,
-                 long long mod_ld, int rows, int rows_per_batch, int h, float eps) {
+                 long long mod_ld, int rows, int rows_per_batch, int h, float eps, uint8_t* __restrict__ q8,
+                 float* __restrict__ qscale) {
   const int row = blockIdx.x * LN_WARPS + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
@@ -82,6 +116,7 @@ layernorm_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict
     sh += static_cast<long long>(b) * mod_ld;
     sc += static_cast<long long>(b) * mod_ld;
   }
+  float amax = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int vec = lane + i * 32;
@@ -92,22 +127,90 @@ layernorm_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict
 #pragma unroll
       for (int j = 0; j < 8; ++j)
         o[j] = MODULATE ? (v[i][j] - mean) * rstd * (1.0f + a[j]) + c[j] : (v[i][j] - mean) * rstd * a[j] + c[j];
-      store8(yr + vec * 8, o);
+      if (Q8) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          v[i][j] = o[j];
+          amax = fmaxf(amax, fabsf(o[j]));
+        }
+      } else {
+        store8(yr + vec * 8, o);
+      }
+    }
+  }
+  if (Q8) store_row_e4m3<NV>(v, amax, nvec, lane, q8 + static_cast<long long>(row) * h, qscale + row);
+}
+
+// y: 16-bit output, or with Q8 the e4m3 output whose row scales go to qscale
+template <typename T, bool MODULATE, bool Q8 = false>
+static void launch_layernorm(const void* x, void* y, const void* shift, const void* scale, long long mod_ld, int rows,
+                             int rows_per_batch, int h, float eps, cudaStream_t stream, float* qscale = nullptr) {
+  const int blocks = dk_ceil_div(rows, LN_WARPS);
+  const int nv = dk_ceil_div(h / 8, 32);   // vectors per lane
+  auto kern = nv <= 4 ? layernorm_kernel<T, 4, MODULATE, Q8>
+              : nv <= 8 ? layernorm_kernel<T, 8, MODULATE, Q8>
+              : nv <= 12 ? layernorm_kernel<T, 12, MODULATE, Q8>
+              : layernorm_kernel<T, 16, MODULATE, Q8>;
+  kern<<<blocks, LN_WARPS * 32, 0, stream>>>(static_cast<const T*>(x), Q8 ? nullptr : static_cast<T*>(y),
+                                             static_cast<const T*>(shift), static_cast<const T*>(scale), mod_ld, rows,
+                                             rows_per_batch, h, eps, Q8 ? static_cast<uint8_t*>(y) : nullptr, qscale);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Row quantiser to e4m3 (weights by output feature, activations by token).  One warp per row: rows of up to
+// 32 * 8 * LN_MAXV columns are read once and held in registers, wider rows (the [attn | GELU(fc1)] buffer) are read a
+// second time for the conversion.
+// ------------------------------------------------------------------------------------------------
+template <typename T, int NV>
+__global__ void __launch_bounds__(LN_WARPS * 32)
+quantize_rows_e4m3_kernel(const T* __restrict__ x, long long ldx, uint8_t* __restrict__ q, float* __restrict__ scale,
+                          int rows, int cols) {
+  const int row = blockIdx.x * LN_WARPS + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int lane = threadIdx.x & 31;
+  const T* xr = x + static_cast<long long>(row) * ldx;
+  uint8_t* qr = q + static_cast<long long>(row) * cols;
+  const int nvec = cols / 8;
+  float amax = 0.f;
+  if (NV > 0) {
+    float v[NV > 0 ? NV : 1][8];
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const int vec = lane + i * 32;
+      if (vec < nvec) {
+        load8(xr + vec * 8, v[i]);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(v[i][j]));
+      }
+    }
+    store_row_e4m3<(NV > 0 ? NV : 1)>(v, amax, nvec, lane, qr, scale + row);
+  } else {
+    float v[8];
+    for (int vec = lane; vec < nvec; vec += 32) {
+      load8(xr + vec * 8, v);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(v[j]));
+    }
+    const float sc = e4m3_row_scale(warp_max(amax));
+    if (lane == 0) scale[row] = sc;
+    for (int vec = lane; vec < nvec; vec += 32) {
+      load8(xr + vec * 8, v);
+      store8_e4m3(qr + vec * 8, v, sc);
     }
   }
 }
 
-template <typename T, bool MODULATE>
-static void launch_layernorm(const void* x, void* y, const void* shift, const void* scale, long long mod_ld, int rows,
-                             int rows_per_batch, int h, float eps, cudaStream_t stream) {
-  const int blocks = dk_ceil_div(rows, LN_WARPS);
-  const int nv = dk_ceil_div(h / 8, 32);   // vectors per lane
-  auto kern = nv <= 4 ? layernorm_kernel<T, 4, MODULATE>
-              : nv <= 8 ? layernorm_kernel<T, 8, MODULATE>
-              : nv <= 12 ? layernorm_kernel<T, 12, MODULATE>
-              : layernorm_kernel<T, 16, MODULATE>;
-  kern<<<blocks, LN_WARPS * 32, 0, stream>>>(static_cast<const T*>(x), static_cast<T*>(y), static_cast<const T*>(shift),
-                                             static_cast<const T*>(scale), mod_ld, rows, rows_per_batch, h, eps);
+template <typename T>
+static void launch_quantize_rows(const void* x, long long ldx, void* q, float* scale, int rows, int cols,
+                                 cudaStream_t stream) {
+  const int nv = dk_ceil_div(cols / 8, 32);   // vectors per lane
+  auto kern = nv <= 4 ? quantize_rows_e4m3_kernel<T, 4>
+              : nv <= 8 ? quantize_rows_e4m3_kernel<T, 8>
+              : nv <= 12 ? quantize_rows_e4m3_kernel<T, 12>
+              : nv <= LN_MAXV ? quantize_rows_e4m3_kernel<T, 16>
+              : quantize_rows_e4m3_kernel<T, 0>;
+  kern<<<dk_ceil_div(rows, LN_WARPS), LN_WARPS * 32, 0, stream>>>(static_cast<const T*>(x), ldx, static_cast<uint8_t*>(q),
+                                                                  scale, rows, cols);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -710,6 +813,38 @@ extern "C" int dk_ln_modulate(dk_ctx* ctx, int dtype, const void* x, void* y, co
   DK_REQUIRE(mod_ld % 8 == 0, "dk_ln_modulate: mod_ld must be a multiple of 8");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DK_DISPATCH(dtype, (launch_layernorm<T, true>(x, y, shift, scale, mod_ld, rows, rows_per_batch, h, eps, stream)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_ln_modulate_fp8(dk_ctx* ctx, int dtype, const void* x, void* q, float* q_scale, const void* shift,
+                                  const void* scale, long long mod_ld, int rows, int rows_per_batch, int h, float eps,
+                                  void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(rows > 0 && rows_per_batch > 0, "dk_ln_modulate_fp8: empty input");
+  DK_REQUIRE(h % 8 == 0 && h <= 32 * 8 * LN_MAXV, "dk_ln_modulate_fp8: h=%d unsupported (multiple of 8, <= %d)", h,
+             32 * 8 * LN_MAXV);
+  DK_REQUIRE(mod_ld % 8 == 0, "dk_ln_modulate_fp8: mod_ld must be a multiple of 8");
+  DK_REQUIRE(q_scale != nullptr, "dk_ln_modulate_fp8: q_scale is required");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (launch_layernorm<T, true, true>(x, q, shift, scale, mod_ld, rows, rows_per_batch, h, eps, stream,
+                                                      q_scale)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_quantize_rows_e4m3(dk_ctx* ctx, int dtype, const void* x, long long ldx, void* q, float* q_scale,
+                                     int rows, int cols, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(rows > 0 && cols > 0, "dk_quantize_rows_e4m3: empty input");
+  DK_REQUIRE(cols % 8 == 0 && ldx % 8 == 0 && ldx >= cols,
+             "dk_quantize_rows_e4m3: cols (%d) and ldx (%lld) must be multiples of 8, ldx >= cols", cols, ldx);
+  DK_REQUIRE(dk_aligned16(x) && (reinterpret_cast<uintptr_t>(q) & 7u) == 0 && q_scale != nullptr,
+             "dk_quantize_rows_e4m3: x must be 16-byte and q 8-byte aligned, q_scale non-null");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (launch_quantize_rows<T>(x, ldx, q, q_scale, rows, cols, stream)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }

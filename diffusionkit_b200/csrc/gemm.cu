@@ -29,21 +29,39 @@
 namespace dk {
 
 constexpr int BM = 128;
-constexpr int BK = 64;
+constexpr int ROW_BYTES = 128;    // one swizzled shared-memory row of an operand tile
+constexpr int BK = ROW_BYTES / 2;  // K elements per k-block of the 16-bit operands
 constexpr int GEMM_THREADS = 384;
 constexpr int CLUSTER = 2;
+
+// e4m3 operand element: one byte, only ever moved by TMA and read by wgmma
+struct E4m3 {
+  uint8_t bits;
+};
+// K elements per k-block: a tile row is 128 bytes whatever the element, so every byte count below (stage sizes, ring
+// depth, descriptor steps) is the same for 16-bit and 8-bit operands
+template <typename E>
+constexpr int BK_OF = ROW_BYTES / static_cast<int>(sizeof(E));
+static_assert(BK_OF<__nv_bfloat16> == BK && BK_OF<__half> == BK && BK_OF<E4m3> == 2 * BK, "k-block is one 128-byte row");
+
+// Accumulation of the e4m3 MMAs: one fp32 fragment across all of K, like the 16-bit operands.  Hopper's FP8 wgmma is
+// reported to keep fewer than 32 bits inside the tensor core (DeepSeek-V3 technical report, section 3.3.2); measured on
+// an H100 at K = 15360 against an fp32 product of the same e4m3 operands this costs 3.4e-3 .. 3.7e-3 relative L2 after
+// bf16 rounding (1.7e-3 is the rounding alone), inside the 4e-3 bound of the 16-bit kernel, while adding each k-block to
+// a second fragment with CUDA-core adds (1.7e-3) ran at 0.65 of the rate.  DESIGN.md "FP8 linears".
 
 template <int BN>
 struct GemmCfg {
   static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int A_BYTES = BM * ROW_BYTES;
+  static constexpr int B_BYTES = BN * ROW_BYTES;
   static constexpr int PIPE_BYTES = STAGES * (A_BYTES + B_BYTES);
   static constexpr int EPI_BYTES = BM * (BN < 128 ? BN : 128) * 2;   // 16-bit output staging, one column pass
   static constexpr int RSTD_BYTES = BM * 2 * 4;                       // QK-RMSNorm: 1/rms per (row, head of a pass)
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_BYTES = PIPE_BYTES + EPI_BYTES + RSTD_BYTES + BAR_BYTES + 1024;  // +1024: alignment slack
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
+  static_assert(A_BYTES == BM * BK * 2 && B_BYTES == BN * BK * 2, "stage sizes do not depend on the operand element");
 };
 
 // Cluster tile ct -> this CTA's (m-block, n-block).  When num_m is odd the partner of the last m-block gets
@@ -62,8 +80,10 @@ __device__ __forceinline__ void cluster_tile(int ct, const GemmShape& s, uint32_
 
 // MODE 0: plain GEMM.  MODE 1: conv3x3 implicit GEMM (A via 4-D TMA boxes).
 // B_MN: W operand given as [K, N] row-major (MN-major wgmma operand, transposed B).
+// T: 16-bit type of the epilogue's operands and of out.  E: element of A and W, T itself or E4m3 (K-major only,
+// MODE 0 only; the epilogue then applies the row and column scales).
 // Launched in clusters of 2 along x with an even grid of at most (resident clusters) x 2 CTAs.
-template <typename T, int BN, bool B_MN, int MODE>
+template <typename T, int BN, bool B_MN, int MODE, typename E>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape s,
                   const GemmEpi e, const ConvGeom g) {
@@ -71,6 +91,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr int STAGES = Cfg::STAGES;
   constexpr int A_BYTES = Cfg::A_BYTES;
   constexpr int B_BYTES = Cfg::B_BYTES;
+  constexpr bool FP8 = sizeof(E) == 1;
+  constexpr int BKE = BK_OF<E>;
+  static_assert(!FP8 || (!B_MN && MODE == 0), "8-bit operands are K-major and have no convolution form");
 
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need 1024-byte aligned bases.  The multicast writes the partner's shared memory at the same
@@ -129,7 +152,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             uint8_t* a_dst = sA + stage * A_BYTES;
             uint8_t* b_dst = sB + stage * B_BYTES;
             if (MODE == 0) {
-              tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
+              tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BKE, m_blk * BM);
             } else {
               const int tap = kb / g.cblocks;
               const int c0 = (kb - tap * g.cblocks) * BK;
@@ -139,7 +162,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             if (!B_MN) {
               // rows [rank*BN/2, (rank+1)*BN/2) of the W tile
-              tma_load_2d_multicast(b_dst + rank * (B_BYTES / 2), &tmB, &full_bar[stage], kb * BK,
+              tma_load_2d_multicast(b_dst + rank * (B_BYTES / 2), &tmB, &full_bar[stage], kb * BKE,
                                     n_blk * BN + static_cast<int>(rank) * (BN / 2), 0x3);
             } else {
 #pragma unroll
@@ -175,11 +198,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const uint32_t b_base = smem_u32(sB + stage * B_BYTES);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
+        for (int k = 0; k < ROW_BYTES / 32; ++k) {   // one MMA per 32 bytes of K: k16 of 16-bit, k32 of 8-bit elements
           const uint64_t da = make_smem_desc_sw128(a_base + k * 32, 16, 1024);
           const uint64_t db = B_MN ? make_smem_desc_sw128(b_base + k * 16 * 128, BK * 128, 1024)
                                    : make_smem_desc_sw128(b_base + k * 32, 16, 1024);
-          Wgmma<BN, Half16<T>::is_bf16, B_MN ? 1 : 0>::ss(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+          if constexpr (FP8)
+            WgmmaE4m3<BN>::ss(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+          else
+            Wgmma<BN, Half16<T>::is_bf16, B_MN ? 1 : 0>::ss(acc, da, db, (kb | k) != 0 ? 1u : 0u);
         }
         wgmma_commit();
         // the previous k-block's MMAs have retired: its stage can be refilled, in both CTAs of the cluster
@@ -200,7 +226,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         mbar_arrive_cluster(&empty_bar[prev], 0);
         mbar_arrive_cluster(&empty_bar[prev], 1);
       }
-      gemm_epilogue_tile<T, BN, MODE>(acc, s, e, g, m_blk, n_blk, cw, stg + cw * (Cfg::EPI_BYTES / 2), rstd + cw * 128);
+      gemm_epilogue_tile<T, BN, MODE, FP8>(acc, s, e, g, m_blk, n_blk, cw, stg + cw * (Cfg::EPI_BYTES / 2), rstd + cw * 128);
     }
   }
   // no CTA may leave while its partner can still multicast into its shared memory or arrive on its barriers
@@ -210,11 +236,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-template <typename T, int BN, bool B_MN, int MODE>
+template <typename T, int BN, bool B_MN, int MODE, typename E = T>
 static int launch_gemm_inst(const char* fn, dk_ctx* ctx, const CUtensorMap& tmA, const CUtensorMap& tmB,
                             const GemmShape& s, const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_wgmma_kernel<T, BN, B_MN, MODE>;
+  auto kern = gemm_wgmma_kernel<T, BN, B_MN, MODE, E>;
   cudaLaunchAttribute cluster;
   cluster.id = cudaLaunchAttributeClusterDimension;
   cluster.val.clusterDim.x = CLUSTER;
@@ -243,12 +269,12 @@ static int launch_gemm_inst(const char* fn, dk_ctx* ctx, const CUtensorMap& tmA,
   return 0;
 }
 
-template <typename T, bool B_MN, int MODE>
+template <typename T, bool B_MN, int MODE, typename E = T>
 static int launch_gemm_bn(const char* fn, dk_ctx* ctx, int bn, const CUtensorMap& tmA, const CUtensorMap& tmB,
                           const GemmShape& s, const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
-  if (bn == 256) return launch_gemm_inst<T, 256, B_MN, MODE>(fn, ctx, tmA, tmB, s, e, g, stream);
-  if (bn == 128) return launch_gemm_inst<T, 128, B_MN, MODE>(fn, ctx, tmA, tmB, s, e, g, stream);
-  return launch_gemm_inst<T, 64, B_MN, MODE>(fn, ctx, tmA, tmB, s, e, g, stream);
+  if (bn == 256) return launch_gemm_inst<T, 256, B_MN, MODE, E>(fn, ctx, tmA, tmB, s, e, g, stream);
+  if (bn == 128) return launch_gemm_inst<T, 128, B_MN, MODE, E>(fn, ctx, tmA, tmB, s, e, g, stream);
+  return launch_gemm_inst<T, 64, B_MN, MODE, E>(fn, ctx, tmA, tmB, s, e, g, stream);
 }
 
 // Tile-N choice: 256 wide tiles keep the shared-memory operand traffic per MMA lowest; fall back to narrower tiles
@@ -267,25 +293,30 @@ static int pick_bn(const dk_ctx* ctx, int num_m, int N) {
 
 using namespace dk;
 
-extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
-  DK_ENTRY(ctx);
-  DK_REQUIRE(a != nullptr, "dk_gemm: null argument");
-  DK_DTYPE_OK(a->dtype);
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0, "dk_gemm: empty problem M=%d N=%d K=%d", a->M, a->N, a->K);
-  DK_REQUIRE(a->N % 8 == 0 && a->K % 8 == 0, "dk_gemm: N (%d) and K (%d) must be multiples of 8", a->N, a->K);
-  DK_REQUIRE(a->lda % 8 == 0 && a->ldw % 8 == 0 && a->ldc % 8 == 0, "dk_gemm: leading dims must be multiples of 8");
-  DK_REQUIRE(dk_aligned16(a->A) && dk_aligned16(a->W) && dk_aligned16(a->out), "dk_gemm: A/W/out must be 16-byte aligned");
-  DK_REQUIRE(a->bias == nullptr || dk_aligned16(a->bias), "dk_gemm: bias must be 16-byte aligned");
-  DK_REQUIRE(a->gate == nullptr || (dk_aligned16(a->gate) && a->gate_ld % 8 == 0), "dk_gemm: gate alignment");
-  DK_REQUIRE(a->res == nullptr || (dk_aligned16(a->res) && a->ldres % 8 == 0), "dk_gemm: residual alignment");
+// dk_gemm and dk_gemm_fp8.  The entry point named fn has run DK_ENTRY and DK_DTYPE_OK.  E is the element of A and W:
+// the 16-bit type of a->dtype, or E4m3 with the two scale vectors.
+static int gemm_impl(const char* fn, dk_ctx* ctx, const dk_gemm_args* a, const float* a_scale, const float* w_scale,
+                     cudaStream_t stream) {
+  const bool fp8 = a_scale != nullptr;
+  const int esize = fp8 ? 1 : 2;
+  const int kmul = 16 / esize;   // TMA global strides are multiples of 16 bytes
+  DK_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0, "%s: empty problem M=%d N=%d K=%d", fn, a->M, a->N, a->K);
+  DK_REQUIRE(a->N % 8 == 0 && a->K % kmul == 0, "%s: N (%d) must be a multiple of 8 and K (%d) of %d", fn, a->N, a->K,
+             kmul);
+  DK_REQUIRE(a->lda % kmul == 0 && a->ldw % kmul == 0 && a->ldc % 8 == 0,
+             "%s: lda and ldw must be multiples of %d, ldc of 8", fn, kmul);
+  DK_REQUIRE(dk_aligned16(a->A) && dk_aligned16(a->W) && dk_aligned16(a->out), "%s: A/W/out must be 16-byte aligned", fn);
+  DK_REQUIRE(a->bias == nullptr || dk_aligned16(a->bias), "%s: bias must be 16-byte aligned", fn);
+  DK_REQUIRE(a->gate == nullptr || (dk_aligned16(a->gate) && a->gate_ld % 8 == 0), "%s: gate alignment", fn);
+  DK_REQUIRE(a->res == nullptr || (dk_aligned16(a->res) && a->ldres % 8 == 0), "%s: residual alignment", fn);
 
+  const int bk = ROW_BYTES / esize;
   GemmShape s = {};
   s.M = a->M;
   s.N = a->N;
   s.K = a->K;
   s.num_m = dk_ceil_div(a->M, BM);
-  s.num_k = dk_ceil_div(a->K, BK);
+  s.num_k = dk_ceil_div(a->K, bk);
   const int bn = a->w_n_major ? 128 : (a->qk_head_dim != 0 ? 256 : pick_bn(ctx, s.num_m, a->N));
   s.num_n = dk_ceil_div(a->N, bn);
 
@@ -309,27 +340,29 @@ extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
   e.qk_d = a->qk_head_dim;
   e.qk_h = a->qk_heads * a->qk_head_dim;
   e.qk_eps = a->qk_eps;
+  e.a_scale = a_scale;
+  e.w_scale = w_scale;
   if (e.qk_d != 0) {
-    DK_REQUIRE(e.qk_d == 64 || e.qk_d == 128, "dk_gemm: fused QK norm/RoPE supports head dims 64 and 128 (got %d)", e.qk_d);
-    DK_REQUIRE(a->N == 3 * e.qk_h && e.qk_h % 128 == 0, "dk_gemm: fused QK epilogue needs N == 3*heads*d, heads*d %% 128 == 0");
+    DK_REQUIRE(e.qk_d == 64 || e.qk_d == 128, "%s: fused QK norm/RoPE supports head dims 64 and 128 (got %d)", fn, e.qk_d);
+    DK_REQUIRE(a->N == 3 * e.qk_h && e.qk_h % 128 == 0, "%s: fused QK epilogue needs N == 3*heads*d, heads*d %% 128 == 0", fn);
     DK_REQUIRE(!a->w_n_major && a->act == DK_ACT_NONE && a->gate == nullptr && a->res == nullptr,
-               "dk_gemm: fused QK epilogue excludes act/gate/residual");
-    DK_REQUIRE(a->qk_rope == nullptr || dk_aligned16(a->qk_rope), "dk_gemm: rope table alignment");
+               "%s: fused QK epilogue excludes act/gate/residual", fn);
+    DK_REQUIRE(a->qk_rope == nullptr || dk_aligned16(a->qk_rope), "%s: rope table alignment", fn);
   }
   ConvGeom g = {};
 
   CUtensorMap tmA, tmB;
   {
     const uint64_t dims[2] = {static_cast<uint64_t>(a->K), static_cast<uint64_t>(a->M)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(a->lda) * 2};
-    const uint32_t box[2] = {BK, BM};
-    if (int rc = dk_make_tmap_16b(ctx, &tmA, a->A, 2, dims, strides, box)) return rc;
+    const uint64_t strides[1] = {static_cast<uint64_t>(a->lda) * esize};
+    const uint32_t box[2] = {static_cast<uint32_t>(bk), BM};
+    if (int rc = dk_make_tmap(ctx, &tmA, esize, a->A, 2, dims, strides, box)) return rc;
   }
   if (!a->w_n_major) {
     const uint64_t dims[2] = {static_cast<uint64_t>(a->K), static_cast<uint64_t>(a->N)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(a->ldw) * 2};
-    const uint32_t box[2] = {BK, static_cast<uint32_t>(bn / CLUSTER)};   // each CTA of a cluster loads half the tile
-    if (int rc = dk_make_tmap_16b(ctx, &tmB, a->W, 2, dims, strides, box)) return rc;
+    const uint64_t strides[1] = {static_cast<uint64_t>(a->ldw) * esize};
+    const uint32_t box[2] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(bn / CLUSTER)};   // each CTA of a cluster loads half the tile
+    if (int rc = dk_make_tmap(ctx, &tmB, esize, a->W, 2, dims, strides, box)) return rc;
   } else {
     const uint64_t dims[2] = {static_cast<uint64_t>(a->N), static_cast<uint64_t>(a->K)};
     const uint64_t strides[1] = {static_cast<uint64_t>(a->ldw) * 2};
@@ -338,9 +371,28 @@ extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
   }
 
   DK_DISPATCH(a->dtype, {
-    if (a->w_n_major) return launch_gemm_inst<T, 128, true, 0>(__func__, ctx, tmA, tmB, s, e, g, stream);
-    return launch_gemm_bn<T, false, 0>(__func__, ctx, bn, tmA, tmB, s, e, g, stream);
+    if (fp8) return launch_gemm_bn<T, false, 0, E4m3>(fn, ctx, bn, tmA, tmB, s, e, g, stream);
+    if (a->w_n_major) return launch_gemm_inst<T, 128, true, 0>(fn, ctx, tmA, tmB, s, e, g, stream);
+    return launch_gemm_bn<T, false, 0>(fn, ctx, bn, tmA, tmB, s, e, g, stream);
   });
+}
+
+extern "C" int dk_gemm(dk_ctx* ctx, const dk_gemm_args* a, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_REQUIRE(a != nullptr, "dk_gemm: null argument");
+  DK_DTYPE_OK(a->dtype);
+  return gemm_impl(__func__, ctx, a, nullptr, nullptr, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int dk_gemm_fp8(dk_ctx* ctx, const dk_gemm_args* a, const float* a_scale, const float* w_scale,
+                           void* stream_) {
+  DK_ENTRY(ctx);
+  DK_REQUIRE(a != nullptr, "dk_gemm_fp8: null argument");
+  DK_DTYPE_OK(a->dtype);
+  DK_REQUIRE(!a->w_n_major, "dk_gemm_fp8: e4m3 operands are K-major only (w_n_major is not supported)");
+  DK_REQUIRE(a_scale != nullptr && w_scale != nullptr, "dk_gemm_fp8: a_scale and w_scale are required");
+  DK_REQUIRE(dk_aligned16(a_scale) && dk_aligned16(w_scale), "dk_gemm_fp8: a_scale/w_scale must be 16-byte aligned");
+  return gemm_impl(__func__, ctx, a, a_scale, w_scale, static_cast<cudaStream_t>(stream_));
 }
 
 // The entry point named fn has run DK_ENTRY and DK_DTYPE_OK.

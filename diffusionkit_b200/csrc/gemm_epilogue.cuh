@@ -30,6 +30,9 @@ struct GemmEpi {
   const float* qk_rope;  // [S, d/2, 2] (cos, sin) or NULL
   int qk_h, qk_d;
   float qk_eps;
+  // e4m3 operands: the accumulator is multiplied by a_scale[A row] * w_scale[output column] before everything else
+  const float* a_scale;  // [M], indexed by the A row (before any row remap)
+  const float* w_scale;  // [N]
 };
 
 struct ConvGeom {
@@ -86,7 +89,8 @@ __device__ __forceinline__ uint32_t ld_u32(const T* p) {
 // leaves as coalesced 16-byte stores to its destination row.  `rstd` holds 128 floats for this warpgroup.
 // Per element the fp32 order is that of the reference: bias, activation, gate, residual, one rounding; the QK path
 // rounds (acc + bias) to 16 bits for the head's sum of squares, which one thread per (row, head) adds in column order.
-template <typename T, int BN, int MODE>
+// SCALED (e4m3 operands): "acc" above is the accumulator times a_scale[row] * w_scale[column].
+template <typename T, int BN, int MODE, bool SCALED>
 __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], const GemmShape& s, const GemmEpi& e,
                                                    const ConvGeom& g, int m_blk, int n_blk, int cw, uint8_t* stg,
                                                    float* rstd) {
@@ -94,7 +98,8 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
   constexpr int EC = BN < 128 ? BN : 128;  // columns per pass
   constexpr int JP = EC / 8;               // 8-column fragment groups per pass = 16-byte chunks per staged row
   constexpr int ROWB = EC * 2;
-  constexpr int G = 4;                     // fragment groups whose global loads are issued together
+  constexpr int G = SCALED ? 2 : 4;        // fragment groups whose global loads are issued together (the scales
+                                           // take registers: two groups keep the 256-wide tile free of spills)
   constexpr int GQ = 2;                    // the same on the QK path, which holds more per group
   const uint32_t bar = 1 + cw;             // named barrier of this warpgroup
   const int t = threadIdx.x & 127;
@@ -110,6 +115,16 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
   auto slot = [&](int rl, int jj) { return rl * ROWB + ((jj ^ (rl & 7)) << 4) + q * 4; };
   const uint32_t stg_s = smem_u32(stg);
   auto put = [&](int rl, int jj, float lo, float hi) { st_shared_u32(stg_s + slot(rl, jj), H16::pack(lo, hi)); };
+  // scales of this thread's two fragment rows (a row past the end reads row 0 and stores nothing) and of a column pair
+  float as[2] = {1.f, 1.f};
+  if (SCALED) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int m = m_blk * 128 + row0 + rl0 + 8 * i;
+      as[i] = e.a_scale[m < s.M ? m : 0];
+    }
+  }
+  auto wscale = [&](int n) { return *reinterpret_cast<const float2*>(e.w_scale + n); };
 
 #pragma unroll
   for (int p = 0; p < BN / EC; ++p) {
@@ -132,9 +147,14 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
 #pragma unroll
         for (int j0 = 0; j0 < JP; j0 += G) {
           uint32_t bw[G];
+          float2 sw[G];
           if (bias != nullptr) {
 #pragma unroll
             for (int u = 0; u < G; ++u) bw[u] = ld_u32(bias + n_pass + 8 * (j0 + u) + 2 * q);
+          }
+          if (SCALED) {
+#pragma unroll
+            for (int u = 0; u < G; ++u) sw[u] = wscale(n_pass + 8 * (j0 + u) + 2 * q);
           }
 #pragma unroll
           for (int u = 0; u < G; ++u) {
@@ -142,6 +162,10 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
               float v0 = acc[a + 2 * i], v1 = acc[a + 2 * i + 1];
+              if (SCALED) {
+                v0 *= as[i] * sw[u].x;
+                v1 *= as[i] * sw[u].y;
+              }
               if (bias != nullptr) {
                 const float2 b = H16::unpack(bw[u]);
                 v0 += b.x;
@@ -174,13 +198,17 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
 #pragma unroll
       for (int j0 = 0; j0 < JP; j0 += GQ) {
         uint32_t bw[GQ], ww[GQ];
-        float2 cs[2][GQ];
+        float2 cs[2][GQ], sw[GQ];
         if (nw != nullptr) {
 #pragma unroll
           for (int u = 0; u < GQ; ++u) ww[u] = ld_u32(nw + ((8 * (j0 + u) + 2 * q) & (d - 1)));
         } else if (bias != nullptr) {
 #pragma unroll
           for (int u = 0; u < GQ; ++u) bw[u] = ld_u32(bias + n_pass + 8 * (j0 + u) + 2 * q);
+        }
+        if (SCALED && nw == nullptr) {
+#pragma unroll
+          for (int u = 0; u < GQ; ++u) sw[u] = wscale(n_pass + 8 * (j0 + u) + 2 * q);
         }
         if (e.qk_rope != nullptr) {
 #pragma unroll
@@ -212,6 +240,10 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
               const int a = p * (EC / 2) + 4 * (j0 + u) + 2 * i;
               v[u][i][0] = acc[a];
               v[u][i][1] = acc[a + 1];
+              if (SCALED) {
+                v[u][i][0] *= as[i] * sw[u].x;
+                v[u][i][1] *= as[i] * sw[u].y;
+              }
               if (bias != nullptr) {
                 const float2 b = H16::unpack(bw[u]);
                 v[u][i][0] += b.x;
@@ -248,9 +280,14 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
       for (int j0 = 0; j0 < JP; j0 += G) {
         // the loads of a group are issued together (column clamped to N: groups past N are computed, not stored)
         uint32_t bw[G], gw[2][G], rw[2][G];
+        float2 sw[G];
         int n[G];
 #pragma unroll
         for (int u = 0; u < G; ++u) n[u] = min(n_pass + 8 * (j0 + u), s.N - 8) + 2 * q;
+        if (SCALED) {
+#pragma unroll
+          for (int u = 0; u < G; ++u) sw[u] = wscale(n[u]);
+        }
         if (bias != nullptr) {
 #pragma unroll
           for (int u = 0; u < G; ++u) bw[u] = ld_u32(bias + n[u]);
@@ -276,6 +313,10 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
             const int a = p * (EC / 2) + 4 * (j0 + u) + 2 * i;
             v[u][i][0] = acc[a];
             v[u][i][1] = acc[a + 1];
+            if (SCALED) {
+              v[u][i][0] *= as[i] * sw[u].x;
+              v[u][i][1] *= as[i] * sw[u].y;
+            }
           }
         if (bias != nullptr) {
 #pragma unroll

@@ -98,12 +98,18 @@ struct DkDeviceGuard {
 // Raises func's dynamic shared-memory limit to `bytes` the first time it is launched through ctx.
 int dk_kernel_smem(dk_ctx* ctx, const void* func, int bytes);
 
-// Tiled tensor map over a 16-bit tensor, 128B swizzle, zero OOB fill.
-//   rank 2..4; dims[0] is the contiguous dimension; strides_bytes has rank-1 entries (dims 1..).
+// Tiled tensor map over a tensor of 16-bit (elem_bytes 2) or 8-bit (elem_bytes 1) elements, 128B swizzle, zero OOB
+// fill (a zero byte is e4m3 +0).
+//   rank 2..4; dims[0] is the contiguous dimension; strides_bytes has rank-1 entries (dims 1..), multiples of 16.
 //   elem_strides (optional, rank entries): traversal stride per dimension; to load N elements with stride s the box
 //   entry must be N * s (cuTensorMapEncodeTiled semantics).
-int dk_make_tmap_16b(dk_ctx* ctx, CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
-                     const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides = nullptr);
+int dk_make_tmap(dk_ctx* ctx, CUtensorMap* map, int elem_bytes, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides = nullptr);
+static inline int dk_make_tmap_16b(dk_ctx* ctx, CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
+                                   const uint64_t* strides_bytes, const uint32_t* box,
+                                   const uint32_t* elem_strides = nullptr) {
+  return dk_make_tmap(ctx, map, 2, base, rank, dims, strides_bytes, box, elem_strides);
+}
 
 static inline int dk_ceil_div(int a, int b) { return (a + b - 1) / b; }
 

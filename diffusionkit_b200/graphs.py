@@ -41,10 +41,14 @@ class ShapeCache:
             self._states.move_to_end(key)
         return st
 
+    def drop(self, name: str):
+        """Forget entry `name` of every shape's state and keep the rest."""
+        for st in self._states.values():
+            st.pop(name, None)
+
     def drop_graphs(self):
         """Forget every captured graph but keep the buffers (for when an input the graphs read moves)."""
-        for st in self._states.values():
-            st.pop("graph", None)
+        self.drop("graph")
 
     def run(self, st: dict, use_graphs: bool, fn, *inputs: torch.Tensor):
         """fn(*inputs), eagerly or by replaying the graph kept in `st`.  With graphs on, the first call for a shape runs

@@ -16,6 +16,8 @@ H100 layout decisions (vs. the reference's per-module MLX graph):
   * all adaLN modulations for all timesteps and all blocks are ONE batched GEMM (replaces the reference's
     per-timestep, per-block loop, mmdit.py:91-175); a step selects its rows with one small D2D copy, which keeps the
     forward's launch sequence timestep-invariant (CUDA-graph capturable).
+  * opt-in FP8 (`set_fp8`, DESIGN.md "FP8 linears"): the block linears run on row-scaled e4m3 copies of their weights;
+    their inputs are quantised per token by the LayerNorm-modulate kernel or by a row quantiser.
 """
 from __future__ import annotations
 
@@ -28,6 +30,26 @@ from . import ops
 from ._lib import ACT_GELU_ERF, ACT_NONE, ACT_SILU, DkError
 from .config import MMDiTConfig, PositionalEncoding
 from .graphs import ShapeCache, default_settings
+
+
+def fp8_covered_linears(config: MMDiTConfig) -> List[str]:
+    """Reference names of the linears `MMDiT.set_fp8` moves to e4m3: q/k/v, o, fc1 and fc2 of every transformer block
+    stream that has them.  Embedders, adaLN modulation and the final layer stay 16-bit."""
+    c = config
+    names = []
+
+    def block(prefix, skip_post=False):
+        names.extend(f"{prefix}.attn.{n}_proj" for n in "qkv")
+        if not skip_post:
+            names.extend(f"{prefix}.{n}" for n in ("attn.o_proj", "mlp.fc1", "mlp.fc2"))
+
+    for i in range(c.depth_multimodal):
+        block(f"multimodal_transformer_blocks.{i}.image_transformer_block")
+        block(f"multimodal_transformer_blocks.{i}.text_transformer_block",
+              skip_post=(i == c.depth_multimodal - 1) and (c.depth_unified < 1))
+    for i in range(c.depth_unified):
+        block(f"unified_transformer_blocks.{i}.transformer_block")
+    return names
 
 
 class _Stream:
@@ -67,6 +89,9 @@ class MMDiT:
         self.use_cuda_graphs, self.max_cached_shapes = default_settings()
         # packed tensors a LoRA merge has touched: (id(owner), attribute, tuple index) -> (owner, base, live)
         self._lora_live: Dict[Tuple[int, str, Optional[int]], Tuple[object, torch.Tensor, torch.Tensor]] = {}
+        # set_fp8: (id(stream), packed weight attribute) -> (e4m3 copy [N, K], fp32 row scales [N])
+        self._fp8_w: Dict[Tuple[int, str], Tuple[torch.Tensor, torch.Tensor]] = {}
+        self._fp8 = False
 
     # ------------------------------------------------------------------------------------------ weight packing
     def _pack(self, P: Dict[str, torch.Tensor]):
@@ -196,6 +221,36 @@ class MMDiT:
         """k-th h-wide modulation vector of a block: view (B, h) with row stride mod_total."""
         return self._mod_cur[:, s_off + k * self.h: s_off + (k + 1) * self.h]
 
+    # ------------------------------------------------------------------------------------------ FP8 linears
+    @property
+    def fp8(self) -> bool:
+        return self._fp8
+
+    def _fp8_packed(self) -> Dict[Tuple[int, str], _Stream]:
+        """(id(stream), attribute) -> stream of every packed weight that holds a covered linear"""
+        slots = self.lora_weight_slots()
+        out = {}
+        for name in fp8_covered_linears(self.config):
+            owner, attr = slots[name + ".weight"][:2]
+            out[(id(owner), attr)] = owner
+        return out
+
+    def set_fp8(self, enabled: bool):
+        """Run the covered block linears (fp8_covered_linears) on e4m3 tensor cores: an accuracy-for-speed trade the
+        caller makes.  Enabling quantises each covered packed weight once, per output feature, into an e4m3 copy and a
+        scale vector kept beside the 16-bit weight (which LoRA merges still need); disabling frees them and the e4m3
+        activation buffers.  Either way the captured graphs are dropped: the launch sequence changes."""
+        enabled = bool(enabled)
+        if enabled == self._fp8:
+            return
+        self._fp8_w = {}
+        if enabled:
+            for key, s in self._fp8_packed().items():
+                self._fp8_w[key] = ops.quantize_rows_e4m3(getattr(s, key[1]))
+        self._fp8 = enabled
+        self._shapes.drop("graph")
+        self._shapes.drop("ws8")
+
     # ------------------------------------------------------------------------------------------ LoRA merge
     def lora_weight_slots(self) -> Dict[str, Tuple[object, str, Optional[int], slice, slice]]:
         """reference weight name -> (owner, attribute, tuple index or None, rows, columns): where each weight a LoRA
@@ -251,7 +306,8 @@ class MMDiT:
         caller's), and gets a live copy the forward reads.  Applying another stack re-merges from the bases in place,
         so captured CUDA graphs stay valid when only scales change; tensors the stack no longer touches go back to
         their base and their live copy is freed (an empty stack frees them all).  Binding a live copy or a base drops
-        the captured graphs.  A merge that changes the adaLN or t / y embedder weights clears the modulation cache:
+        the captured graphs.  With FP8 on, the e4m3 copy of every weight whose 16-bit tensor changed is re-quantised in
+        place, so it keeps its address too.  A merge that changes the adaLN or t / y embedder weights clears the modulation cache:
         call cache_modulation_params again before the next forward."""
         slots = self.lora_weight_slots()
         terms: Dict[str, list] = {}
@@ -268,6 +324,7 @@ class MMDiT:
             owner, attr, idx = slots[name][:3]
             touched[(id(owner), attr, idx)] = (owner, attr, idx)
         rebound, mod_changed = False, False
+        changed = set(touched) | set(self._lora_live)
         for key in [k for k in self._lora_live if k not in touched]:
             owner, base, _ = self._lora_live.pop(key)
             self._rebind(owner, key[1], key[2], base)
@@ -286,6 +343,11 @@ class MMDiT:
             _, base, live = self._lora_live[(id(owner), attr, idx)]
             up, down = self._lora_factors(ts)
             ops.gemm(up, down, out=live[rows, cols], res=base[rows, cols], w_n_major=True)
+        packed = self._fp8_packed() if self._fp8 else {}
+        for oid, attr, _ in changed:
+            if (oid, attr) in packed:
+                q, sc = self._fp8_w[(oid, attr)]
+                ops.quantize_rows_e4m3(getattr(packed[(oid, attr)], attr), out=q, scale=sc)
         if rebound:
             self._shapes.drop_graphs()
         if mod_changed:
@@ -332,6 +394,26 @@ class MMDiT:
         st["ws"] = ws
         return ws
 
+    def _workspace8(self, st: dict, B: int, N: int, T: int) -> dict:
+        """e4m3 activation buffers and their per-row scales while FP8 is on (nothing otherwise): name -> (q, scale).
+        "m_*" holds a stream's LayerNorm-modulate output and, after attention, its quantised attention output."""
+        if not self._fp8:
+            return {}
+        if "ws8" in st:
+            return st["ws8"]
+        h, dev, r = self.h, self.device, self.config.mlp_ratio
+
+        def buf(rows, cols):
+            return (torch.empty((rows, cols), dtype=torch.float8_e4m3fn, device=dev),
+                    torch.empty((rows,), dtype=torch.float32, device=dev))
+
+        w8 = {"m_img": buf(B * N, h), "m_txt": buf(B * T, h), "hid_img": buf(B * N, r * h), "hid_txt": buf(B * T, r * h)}
+        if self.is_flux:
+            w8["m_u"] = buf(B * (N + T), h)
+            w8["cat"] = buf(B * (N + T), (1 + r) * h)
+        st["ws8"] = w8
+        return w8
+
     def _rope_table(self, st: dict, T: int, hp: int, wp: int) -> torch.Tensor:
         """(S, d/2, 2) fp32 cos/sin; text tokens at position (0,0,0), image token (r, c) at (0, r, c)
         (reference mmdit.py:865-911).  Cached across calls like the reference (:916-932)."""
@@ -359,21 +441,38 @@ class MMDiT:
             return None
         return (self.heads, self.d, s.q_norm, s.k_norm, rope, 1e-6)
 
-    def _attn_stream_pre(self, s: _Stream, x, m, rows_per_batch, S, row_off, qkv, rope):
-        ops.ln_modulate(x, self._mod(s.mod_off, 0), self._mod(s.mod_off, 1), rows_per_batch,
-                        self.config.layer_norm_eps, out=m)
-        ops.gemm(m, s.w_qkv, out=qkv, bias=s.b_qkv, rows_per_batch=rows_per_batch, out_batch_rows=S,
-                 out_row_off=row_off, qk=self._qk_fused(s, rope))
+    # A covered linear's input is a 16-bit tensor or, with FP8 on, the (e4m3, row scales) pair in the buffers `x8`.
+    def _ln_mod(self, x, s: _Stream, k: int, rows_per_batch, m, m8):
+        """LN(x) * (1 + scale_k) + shift_k of stream s as the input of a covered linear"""
+        shift, scale, eps = self._mod(s.mod_off, k), self._mod(s.mod_off, k + 1), self.config.layer_norm_eps
+        if self._fp8:
+            return ops.ln_modulate_fp8(x, shift, scale, rows_per_batch, eps, out=m8[0], out_scale=m8[1])
+        return ops.ln_modulate(x, shift, scale, rows_per_batch, eps, out=m)
 
-    def _stream_post(self, s: _Stream, x, o, m, hid, rows_per_batch):
+    def _lin_in(self, x, x8):
+        """the 16-bit activation x as the input of a covered linear"""
+        return ops.quantize_rows_e4m3(x, out=x8[0], scale=x8[1]) if self._fp8 else x
+
+    def _linear(self, a, s: _Stream, attr: str, **epilogue):
+        """covered linear `attr` of stream s on an input from _ln_mod / _lin_in"""
+        if self._fp8:
+            wq, w_scale = self._fp8_w[(id(s), attr)]
+            return ops.gemm_fp8(a[0], a[1], wq, w_scale, **epilogue)
+        return ops.gemm(a, getattr(s, attr), **epilogue)
+
+    def _attn_stream_pre(self, s: _Stream, x, m, m8, rows_per_batch, S, row_off, qkv, rope):
+        a = self._ln_mod(x, s, 0, rows_per_batch, m, m8)
+        self._linear(a, s, "w_qkv", out=qkv, bias=s.b_qkv, rows_per_batch=rows_per_batch, out_batch_rows=S,
+                     out_row_off=row_off, qk=self._qk_fused(s, rope))
+
+    def _stream_post(self, s: _Stream, x, o, m, m8, hid, hid8, rows_per_batch):
         """x += gate1 * o_proj(o); x += gate2 * fc2(gelu(fc1(LN(x)(1+scale2)+shift2)))  (mmdit.py:521-548)"""
-        ops.gemm(o, s.w_o, out=x, bias=s.b_o, gate=self._mod(s.mod_off, 2), res=x, rows_per_batch=rows_per_batch,
-                 out_batch_rows=rows_per_batch)
-        ops.ln_modulate(x, self._mod(s.mod_off, 3), self._mod(s.mod_off, 4), rows_per_batch,
-                        self.config.layer_norm_eps, out=m)
-        ops.gemm(m, s.w_fc1, out=hid, bias=s.b_fc1, act=ACT_GELU_ERF)
-        ops.gemm(hid, s.w_fc2, out=x, bias=s.b_fc2, gate=self._mod(s.mod_off, 5), res=x,
-                 rows_per_batch=rows_per_batch, out_batch_rows=rows_per_batch)
+        self._linear(self._lin_in(o, m8), s, "w_o", out=x, bias=s.b_o, gate=self._mod(s.mod_off, 2), res=x,
+                     rows_per_batch=rows_per_batch, out_batch_rows=rows_per_batch)
+        a = self._ln_mod(x, s, 3, rows_per_batch, m, m8)
+        self._linear(a, s, "w_fc1", out=hid, bias=s.b_fc1, act=ACT_GELU_ERF)
+        self._linear(self._lin_in(hid, hid8), s, "w_fc2", out=x, bias=s.b_fc2, gate=self._mod(s.mod_off, 5), res=x,
+                     rows_per_batch=rows_per_batch, out_batch_rows=rows_per_batch)
 
     def __call__(self, latent_image_embeddings: torch.Tensor, token_level_text_embeddings: torch.Tensor,
                  timestep=None) -> torch.Tensor:
@@ -413,6 +512,7 @@ class MMDiT:
         S = N + T
         h, heads, d = self.h, self.heads, self.d
         ws = self._workspace(state, B, N, T)
+        w8 = self._workspace8(state, B, N, T).get
         img, txt, qkv = ws["img"], ws["txt"], ws["qkv"]
 
         # ---- input adapters (mmdit.py:195-206)
@@ -435,28 +535,28 @@ class MMDiT:
             off_img, off_txt, split = 0, N, N
 
         for (si, st) in self.double:
-            self._attn_stream_pre(si, img, ws["m_img"], N, S, off_img, qkv, rope)
-            self._attn_stream_pre(st, txt, ws["m_txt"], T, S, off_txt, qkv, rope)
+            self._attn_stream_pre(si, img, ws["m_img"], w8("m_img"), N, S, off_img, qkv, rope)
+            self._attn_stream_pre(st, txt, ws["m_txt"], w8("m_txt"), T, S, off_txt, qkv, rope)
             if self.is_flux:
                 ops.attention(qkv, B, S, heads, d, ws["o_txt"], split=split, out1=ws["o_img"])
             else:
                 ops.attention(qkv, B, S, heads, d, ws["o_img"], split=split, out1=ws["o_txt"])
-            self._stream_post(si, img, ws["o_img"], ws["m_img"], ws["hid_img"], N)
+            self._stream_post(si, img, ws["o_img"], ws["m_img"], w8("m_img"), ws["hid_img"], w8("hid_img"), N)
             if not st.skip_post:
-                self._stream_post(st, txt, ws["o_txt"], ws["m_txt"], ws["hid_txt"], T)
+                self._stream_post(st, txt, ws["o_txt"], ws["m_txt"], w8("m_txt"), ws["hid_txt"], w8("hid_txt"), T)
 
         if self.is_flux:
             u, m_u, cat = ws["u"], ws["m_u"], ws["cat"]
             ops.copy_rows(txt, u, B, T, h, S, 0, T, 0)                                 # u = [text | image] (:234-236)
             ops.copy_rows(img, u, B, N, h, S, T, N, 0)
             for s in self.single:                                                      # mmdit.py:693-751
-                ops.ln_modulate(u, self._mod(s.mod_off, 0), self._mod(s.mod_off, 1), S, c.layer_norm_eps, out=m_u)
-                ops.gemm(m_u, s.w_qkv, out=qkv, bias=s.b_qkv, rows_per_batch=S, out_batch_rows=S,
-                         qk=self._qk_fused(s, rope))
+                a = self._ln_mod(u, s, 0, S, m_u, w8("m_u"))
+                self._linear(a, s, "w_qkv", out=qkv, bias=s.b_qkv, rows_per_batch=S, out_batch_rows=S,
+                             qk=self._qk_fused(s, rope))
                 ops.attention(qkv, B, S, heads, d, cat[:, :h])
-                ops.gemm(m_u, s.w_fc1, out=cat[:, h:], bias=s.b_fc1, act=ACT_GELU_ERF)
-                ops.gemm(cat, s.w_out, out=u, bias=s.b_o, gate=self._mod(s.mod_off, 2), res=u, rows_per_batch=S,
-                         out_batch_rows=S)
+                self._linear(a, s, "w_fc1", out=cat[:, h:], bias=s.b_fc1, act=ACT_GELU_ERF)
+                self._linear(self._lin_in(cat, w8("cat")), s, "w_out", out=u, bias=s.b_o, gate=self._mod(s.mod_off, 2),
+                             res=u, rows_per_batch=S, out_batch_rows=S)
             ops.copy_rows(u, img, B, N, h, N, 0, S, T)                                 # image part (:245-247)
 
         # ---- final layer (mmdit.py:780-796) + unpatchify / unpack

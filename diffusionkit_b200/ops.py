@@ -63,14 +63,25 @@ def gemm(
     w_n_major: bool = False,
     N: Optional[int] = None,
     qk: Optional[tuple] = None,
+    fp8_scales: Optional[tuple] = None,
+    dtype: Optional[torch.dtype] = None,
 ) -> torch.Tensor:
     """out = res + gate * act(A @ W.T + bias)   (see include/dkb200.h, dk_gemm).
 
     A: [M, K] (row stride may exceed K), W: [N, K] (nn.Linear layout) or [K, N] when w_n_major.
     out: 2-D view [rows, >=N] whose row stride is the leading dimension.
+    fp8_scales (gemm_fp8 passes it): A and W hold e4m3 bytes, (a_scale [M], w_scale [N]) are their fp32 row scales and
+    dtype is the 16-bit type of out (dk_gemm_fp8).
     """
-    _chk16(A, "gemm.A")
-    _chk16(W, "gemm.W")
+    if fp8_scales is None:
+        _chk16(A, "gemm.A")
+        _chk16(W, "gemm.W")
+        dtype = A.dtype
+    else:
+        _chk_e4m3(A, "gemm_fp8.A")
+        _chk_e4m3(W, "gemm_fp8.W")
+        a_scale, w_scale = fp8_scales
+        dtype = out.dtype if out is not None else dtype
     assert A.dim() == 2 and W.dim() == 2 and A.stride(1) == 1 and W.stride(1) == 1
     M, K = A.shape
     if w_n_major:
@@ -82,10 +93,10 @@ def gemm(
     if N is not None:
         n = N
     if out is None:
-        out = torch.empty((M, n), dtype=A.dtype, device=A.device)
+        out = torch.empty((M, n), dtype=dtype, device=A.device)
     assert out.dim() == 2 and out.stride(1) == 1
     a = GemmArgs()
-    a.dtype = dtype_code(A.dtype)
+    a.dtype = dtype_code(dtype)
     a.M, a.N, a.K = M, n, K
     a.A, a.lda = ptr(A), A.stride(0)
     a.W, a.ldw = ptr(W), W.stride(0)
@@ -110,8 +121,60 @@ def gemm(
         a.qk_heads, a.qk_head_dim, a.qk_eps = heads, hd, eps
         a.qk_q_weight, a.qk_k_weight, a.qk_rope = ptr(qw), ptr(kw), ptr(rope)
     c = ctx(A.device.index)
-    c.check(c.lib.dk_gemm(c.handle, C.byref(a), c.stream))
+    if fp8_scales is None:
+        c.check(c.lib.dk_gemm(c.handle, C.byref(a), c.stream))
+    else:
+        assert a_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+        assert a_scale.numel() == M and w_scale.numel() >= n and a_scale.is_contiguous() and w_scale.is_contiguous()
+        c.check(c.lib.dk_gemm_fp8(c.handle, C.byref(a), ptr(a_scale), ptr(w_scale), c.stream))
     return out
+
+
+def _chk_e4m3(t: torch.Tensor, name: str):
+    if t.dtype != torch.float8_e4m3fn or not t.is_cuda:
+        raise _lib.DkError(f"{name}: expected a CUDA torch.float8_e4m3fn tensor, got {t.dtype} on {t.device}")
+
+
+def gemm_fp8(A, a_scale, W, w_scale, dtype: Optional[torch.dtype] = None, **epilogue) -> torch.Tensor:
+    """gemm with row-quantised e4m3 operands: A [M, K] with a_scale [M], W [N, K] with w_scale [N] (as
+    quantize_rows_e4m3 / ln_modulate_fp8 produce them); the accumulator is scaled by a_scale[m] * w_scale[n] ahead of
+    gemm's epilogue, whose keyword arguments this takes (not w_n_major).  dtype: 16-bit type of out when out is not
+    given."""
+    return gemm(A, W, fp8_scales=(a_scale, w_scale), dtype=dtype, **epilogue)
+
+
+def quantize_rows_e4m3(x, out=None, scale=None):
+    """x [rows, cols] 16-bit (row stride may exceed cols) -> (q [rows, cols] e4m3, scale [rows] fp32):
+    scale = amax|row| / 448 (1 for a zero row), q = e4m3(x / scale)."""
+    _chk16(x, "quantize_rows_e4m3.x")
+    assert x.dim() == 2 and x.stride(1) == 1
+    rows, cols = x.shape
+    if out is None:
+        out = torch.empty((rows, cols), dtype=torch.float8_e4m3fn, device=x.device)
+    if scale is None:
+        scale = torch.empty((rows,), dtype=torch.float32, device=x.device)
+    _chk_e4m3(out, "quantize_rows_e4m3.out")
+    assert out.is_contiguous() and out.shape == (rows, cols) and scale.dtype == torch.float32 and scale.numel() == rows
+    c = ctx(x.device.index)
+    c.call("dk_quantize_rows_e4m3", dtype_code(x.dtype), ptr(x), x.stride(0), ptr(out), ptr(scale), rows, cols)
+    return out, scale
+
+
+def ln_modulate_fp8(x, shift, scale, rows_per_batch: int, eps: float = 1e-6, out=None, out_scale=None):
+    """ln_modulate whose fp32 result row is quantised like quantize_rows_e4m3 -> (q [rows, h] e4m3, scale [rows])."""
+    _chk16(x, "ln_modulate_fp8.x")
+    rows, h = x.shape
+    assert x.is_contiguous() and shift.stride(0) == scale.stride(0) and shift.stride(1) == 1
+    if out is None:
+        out = torch.empty((rows, h), dtype=torch.float8_e4m3fn, device=x.device)
+    if out_scale is None:
+        out_scale = torch.empty((rows,), dtype=torch.float32, device=x.device)
+    _chk_e4m3(out, "ln_modulate_fp8.out")
+    assert out.is_contiguous() and out_scale.dtype == torch.float32 and out_scale.numel() == rows
+    c = ctx(x.device.index)
+    c.call("dk_ln_modulate_fp8", dtype_code(x.dtype), ptr(x), ptr(out), ptr(out_scale), ptr(shift), ptr(scale),
+           shift.stride(0), rows, rows_per_batch, h, eps)
+    return out, out_scale
 
 
 def ln_modulate(x, shift, scale, rows_per_batch: int, eps: float = 1e-6, out=None):

@@ -318,6 +318,15 @@ class DiffusionPipeline:
     def _apply_loras(self):
         self.mmdit.apply_lora([(lora, s) for lora, s in self._loras.values()])
 
+    # ------------------------------------------------------------------ FP8 linears (DESIGN.md "FP8 linears")
+    def set_fp8(self, enabled: bool):
+        """Run the MMDiT's block linears in e4m3 (MMDiT.set_fp8): faster, less accurate; off by default."""
+        self.mmdit.set_fp8(enabled)
+
+    @property
+    def fp8(self) -> bool:
+        return self.mmdit.fp8
+
     # ------------------------------------------------------------------ text (SURVEY.md §8 row f2)
     def load_text_encoders(self, clip_l=None, clip_g=None, t5=None, *, tokenizer_l=None, tokenizer_g=None,
                            t5_tokenizer=None, clip_l_config=None, clip_g_config=None, t5_config=None):

@@ -102,12 +102,38 @@ typedef struct dk_gemm_args {
 int dk_gemm(dk_ctx* ctx, const dk_gemm_args* args, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * K1 with e4m3 operands — the opt-in FP8 form of the MMDiT block linears (mmdit.py:471-473 q/k/v, :532 o_proj,
+ *     :830-835 FFN; the reference has no 8-bit path, this trades accuracy for tensor-core rate).
+ *     args->A [M, K] and args->W [N, K] hold e4m3 bytes (lda / ldw in elements), quantised per row:
+ *     A[m,k] ~ a_scale[m] * e4m3(A)[m,k], W[n,k] ~ w_scale[n] * e4m3(W)[n,k].  args->dtype is the 16-bit type of
+ *     out / bias / gate / residual / norm weights.  The epilogue is dk_gemm's with the accumulator replaced by
+ *     a_scale[m] * w_scale[n] * sum_k e4m3(A)[m,k] e4m3(W)[n,k]   (a_scale indexed by the A row, before any row map).
+ *     K, lda, ldw multiples of 16; w_n_major is not supported; both scale vectors required, 16-byte aligned.
+ * ------------------------------------------------------------------------------------------- */
+int dk_gemm_fp8(dk_ctx* ctx, const dk_gemm_args* args, const float* a_scale, const float* w_scale, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Row quantiser to e4m3 for dk_gemm_fp8 (weights by output feature — the nn.Linear weights of mmdit.py:471-473,
+ *     :532, :830-835 — and activations by token).  x: [rows, cols] 16-bit, row stride ldx (elements);
+ *     q: [rows, cols] e4m3 bytes, contiguous; q_scale: [rows] fp32.
+ *     q_scale[r] = max_c |x[r,c]| / 448 (1 if the row is all zero); q[r,c] = e4m3_rn_satfinite(x[r,c] / q_scale[r]),
+ *     evaluated in fp32.  cols, ldx multiples of 8.
+ * ------------------------------------------------------------------------------------------- */
+int dk_quantize_rows_e4m3(dk_ctx* ctx, int dtype, const void* x, long long ldx, void* q, float* q_scale, int rows,
+                          int cols, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * K2  LayerNorm (no affine, eps) + adaLN modulate: y = LN(x) * (1 + scale[b]) + shift[b]
  *     replaces affine_transform / mx.fast.layer_norm — mmdit.py:958-972, :838-849.
  *     x, y: [B*rows_per_batch, h]; shift/scale: row b at ptr + b*mod_ld (16-bit).
  * ------------------------------------------------------------------------------------------- */
 int dk_ln_modulate(dk_ctx* ctx, int dtype, const void* x, void* y, const void* shift, const void* scale,
                    long long mod_ld, int rows, int rows_per_batch, int h, float eps, void* stream);
+/* K2 feeding dk_gemm_fp8 (mmdit.py:958-972 ahead of the q/k/v and fc1 linears): the modulated fp32 row is not rounded
+ * to 16 bits but quantised like dk_quantize_rows_e4m3: q [rows, h] e4m3 bytes, q_scale [rows] fp32. */
+int dk_ln_modulate_fp8(dk_ctx* ctx, int dtype, const void* x, void* q, float* q_scale, const void* shift,
+                       const void* scale, long long mod_ld, int rows, int rows_per_batch, int h, float eps,
+                       void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * QK-RMSNorm (mmdit.py:754-764, eps 1e-6, learned weight) + FLUX RoPE (mmdit.py:934-942) applied
