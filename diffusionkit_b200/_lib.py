@@ -77,6 +77,8 @@ SIGNATURES = {
     "dk_vae_sample_latent": (i32, [vp, i32, vp, vp, vp, i64, i32, f32, f32, vp]),
     "dk_cast_f32_to_16": (i32, [vp, i32, vp, vp, i64, vp]),
     "dk_cast_16_to_f32": (i32, [vp, i32, vp, vp, i64, vp]),
+    "dk_residual_delta": (i32, [vp, i32, vp, i64, i32, vp, i64, i32, vp, vp, vp, vp, i32, i32, i32, vp]),
+    "dk_residual_apply": (i32, [vp, i32, vp, vp, vp, i64, vp]),
     "dk_groupnorm_ws_floats": (i32, [i32, i32]),
     "dk_groupnorm_stats": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, i32, f32, vp]),
     "dk_groupnorm_apply": (i32, [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),

@@ -799,6 +799,123 @@ __global__ void image_post_kernel(const T* __restrict__ x, int c_stride, float* 
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// First-block step cache (DESIGN.md §10).  residual_delta: r = fp32(x) - fp32(base) over nseq sequences of `rows`
+// rows; optionally stored to r_out [nseq*rows, h] fp32, and with prev [nseq*rows, h] fp32 the per-sequence sums
+// (Σ|r - prev|, Σ|prev|).  Deterministic: grid (chunks, nseq), each block folds its row slab in a fixed thread order
+// and a fixed shuffle tree into ws[seq][chunk][2]; residual_delta_finalize folds the chunks of a sequence in a fixed
+// order in double.  No atomics, so two launches are bit-identical.
+// ------------------------------------------------------------------------------------------------
+constexpr int RD_THREADS = 256;
+constexpr int RD_MAX_CHUNKS = 256;   // per sequence; ws holds nseq * RD_MAX_CHUNKS * 2 floats
+
+template <typename T>
+__global__ void __launch_bounds__(RD_THREADS)
+residual_delta_kernel(const T* __restrict__ x, long long ldx, int x_seq_rows, const T* __restrict__ base,
+                      long long ldb, int b_seq_rows, float* __restrict__ r_out, const float* __restrict__ prev,
+                      float* __restrict__ ws, int rows, int h) {
+  __shared__ float red[RD_THREADS / 32];
+  const int seq = blockIdx.y, chunk = blockIdx.x, chunks = gridDim.x;
+  const int per = (rows + chunks - 1) / chunks;
+  const int r0 = chunk * per, r1 = min(rows, r0 + per);
+  const int vpr = h / 8;   // vectors per row
+  const long long nvec = r1 > r0 ? static_cast<long long>(r1 - r0) * vpr : 0;
+  float s_diff = 0.f, s_prev = 0.f;
+  for (long long i = threadIdx.x; i < nvec; i += RD_THREADS) {
+    const int r = r0 + static_cast<int>(i / vpr);
+    const int col = static_cast<int>(i % vpr) * 8;
+    float a[8], b[8];
+    load8(x + (static_cast<long long>(seq) * x_seq_rows + r) * ldx + col, a);
+    load8(base + (static_cast<long long>(seq) * b_seq_rows + r) * ldb + col, b);
+    const long long o = (static_cast<long long>(seq) * rows + r) * h + col;
+    float d[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) d[j] = a[j] - b[j];
+    if (r_out != nullptr) {
+      float4* p = reinterpret_cast<float4*>(r_out + o);
+      p[0] = make_float4(d[0], d[1], d[2], d[3]);
+      p[1] = make_float4(d[4], d[5], d[6], d[7]);
+    }
+    if (prev != nullptr) {
+      const float4 p0 = reinterpret_cast<const float4*>(prev + o)[0];
+      const float4 p1 = reinterpret_cast<const float4*>(prev + o)[1];
+      const float pv[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        s_diff += fabsf(d[j] - pv[j]);
+        s_prev += fabsf(pv[j]);
+      }
+    }
+  }
+  if (prev == nullptr) return;   // uniform across the block
+  s_diff = block_sum<RD_THREADS>(s_diff, red);
+  s_prev = block_sum<RD_THREADS>(s_prev, red);
+  if (threadIdx.x == 0) {
+    float* dst = ws + (static_cast<long long>(seq) * chunks + chunk) * 2;
+    dst[0] = s_diff;
+    dst[1] = s_prev;
+  }
+}
+
+// one warp per sequence: lanes stride over the chunk partials, then a fixed shuffle tree, all in double
+__global__ void residual_delta_finalize_kernel(const float* __restrict__ ws, float* __restrict__ sums, int nseq,
+                                               int chunks) {
+  const int seq = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (seq >= nseq) return;
+  const float2* p = reinterpret_cast<const float2*>(ws) + static_cast<long long>(seq) * chunks;
+  double s = 0.0, q = 0.0;
+  for (int c = lane; c < chunks; c += 32) {
+    const float2 v = p[c];
+    s += v.x;
+    q += v.y;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s += __shfl_xor_sync(0xffffffffu, s, o);
+    q += __shfl_xor_sync(0xffffffffu, q, o);
+  }
+  if (lane == 0) {
+    sums[seq * 2] = static_cast<float>(s);
+    sums[seq * 2 + 1] = static_cast<float>(q);
+  }
+}
+
+static inline int rd_chunks(int rows, int h, int sm_count, int nseq) {
+  // about four 8-element vectors per thread, and about four blocks per SM over the whole batch
+  const long long vec = static_cast<long long>(rows) * (h / 8);
+  long long c = (vec + RD_THREADS * 4 - 1) / (RD_THREADS * 4);
+  const long long fill = (4LL * sm_count + nseq - 1) / nseq;
+  if (c > fill) c = fill;
+  if (c > rows) c = rows;
+  if (c > RD_MAX_CHUNKS) c = RD_MAX_CHUNKS;
+  if (c < 1) c = 1;
+  return static_cast<int>(c);
+}
+
+// out = round16(x + r): one fp32 add, one rounding
+template <typename T>
+__global__ void residual_apply_kernel(const T* __restrict__ x, const float* __restrict__ r, T* __restrict__ out,
+                                      long long n) {
+  const long long nvec = n / 8;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float a[8];
+    load8(x + i * 8, a);
+    const float4 r0 = reinterpret_cast<const float4*>(r + i * 8)[0];
+    const float4 r1 = reinterpret_cast<const float4*>(r + i * 8)[1];
+    a[0] += r0.x;
+    a[1] += r0.y;
+    a[2] += r0.z;
+    a[3] += r0.w;
+    a[4] += r1.x;
+    a[5] += r1.y;
+    a[6] += r1.z;
+    a[7] += r1.w;
+    store8(out + i * 8, a);
+  }
+}
+
 }  // namespace dk
 
 using namespace dk;
@@ -1149,6 +1266,51 @@ extern "C" int dk_image_post(dk_ctx* ctx, int dtype, const void* x, int c_stride
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DK_DISPATCH(dtype, (image_post_kernel<T><<<dk_grid_for(pixels * 3, 256, ctx->sm_count), 256, 0, stream>>>(
                          static_cast<const T*>(x), c_stride, img_f32, img_u8, pixels)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_residual_delta(dk_ctx* ctx, int dtype, const void* x, long long ldx, int x_seq_rows, const void* base,
+                                 long long ldb, int b_seq_rows, float* r_out, const float* prev, float* sums, float* ws,
+                                 int nseq, int rows, int h, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(x != nullptr && base != nullptr, "dk_residual_delta: x and base are required");
+  DK_REQUIRE(nseq > 0 && rows > 0 && h > 0, "dk_residual_delta: empty input (nseq %d, rows %d, h %d)", nseq, rows, h);
+  DK_REQUIRE(h % 8 == 0 && ldx % 8 == 0 && ldb % 8 == 0 && ldx >= h && ldb >= h,
+             "dk_residual_delta: h (%d), ldx (%lld) and ldb (%lld) must be multiples of 8, ldx and ldb >= h", h, ldx,
+             ldb);
+  DK_REQUIRE(x_seq_rows >= rows && b_seq_rows >= rows,
+             "dk_residual_delta: x_seq_rows (%d) and b_seq_rows (%d) must be >= rows (%d)", x_seq_rows, b_seq_rows, rows);
+  DK_REQUIRE(r_out != nullptr || prev != nullptr, "dk_residual_delta: nothing to do (r_out and prev are both null)");
+  DK_REQUIRE(prev == nullptr || (sums != nullptr && ws != nullptr), "dk_residual_delta: prev needs sums and ws");
+  DK_REQUIRE(dk_aligned16(x) && dk_aligned16(base) && dk_aligned16(r_out) && dk_aligned16(prev),
+             "dk_residual_delta: x, base, r_out and prev must be 16-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const int chunks = rd_chunks(rows, h, ctx->sm_count, nseq);
+  dim3 grid(chunks, nseq);
+  DK_DISPATCH(dtype, (residual_delta_kernel<T><<<grid, RD_THREADS, 0, stream>>>(
+                         static_cast<const T*>(x), ldx, x_seq_rows, static_cast<const T*>(base), ldb, b_seq_rows, r_out,
+                         prev, ws, rows, h)));
+  DK_LAUNCH_CHECK(ctx);
+  if (prev != nullptr) {
+    residual_delta_finalize_kernel<<<dk_ceil_div(nseq, 4), 128, 0, stream>>>(ws, sums, nseq, chunks);
+    DK_LAUNCH_CHECK(ctx);
+  }
+  return 0;
+}
+
+extern "C" int dk_residual_apply(dk_ctx* ctx, int dtype, const void* x, const float* r, void* out, long long n,
+                                 void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(x != nullptr && r != nullptr && out != nullptr, "dk_residual_apply: x, r and out are required");
+  DK_REQUIRE(n > 0 && n % 8 == 0, "dk_residual_apply: n (%lld) must be a positive multiple of 8", n);
+  DK_REQUIRE(dk_aligned16(x) && dk_aligned16(r) && dk_aligned16(out),
+             "dk_residual_apply: x, r and out must be 16-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (residual_apply_kernel<T><<<dk_grid_for(n / 8, 256, ctx->sm_count), 256, 0, stream>>>(
+                         static_cast<const T*>(x), r, static_cast<T*>(out), n)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }

@@ -42,30 +42,38 @@ class ShapeCache:
         return st
 
     def drop(self, name: str):
-        """Forget entry `name` of every shape's state and keep the rest."""
+        """Forget entry `name` of every shape's state, and the entries "name.<part>" with it, and keep the rest."""
         for st in self._states.values():
-            st.pop(name, None)
+            for key in [k for k in st if k == name or k.startswith(name + ".")]:
+                del st[key]
 
     def drop_graphs(self):
         """Forget every captured graph but keep the buffers (for when an input the graphs read moves)."""
         self.drop("graph")
 
-    def run(self, st: dict, use_graphs: bool, fn, *inputs: torch.Tensor):
-        """fn(*inputs), eagerly or by replaying the graph kept in `st`.  With graphs on, the first call for a shape runs
-        fn eagerly on static copies of the inputs (workspaces, tables, function attributes, allocator), then captures
-        it; every replay copies the inputs into those copies and returns the same output tensor."""
+    def run(self, st: dict, use_graphs: bool, fn, *inputs: torch.Tensor, name: str = "graph",
+            stateful: bool = False, device=None):
+        """fn(*inputs), eagerly or by replaying the graph kept in `st[name]`.  With graphs on, the first call for a shape
+        runs fn eagerly on static copies of the inputs (workspaces, tables, function attributes, allocator), then
+        captures it; every replay copies the inputs into those copies and returns the same output tensor.
+        stateful: fn updates buffers it also reads, so running it twice is not running it once; the first call returns
+        the eager pass's output and the capture is not replayed until the next call.  A graph named "graph.<part>" is
+        one part of a forward and is dropped with "graph".  device: where fn runs when it takes no inputs."""
         if not use_graphs:
             return fn(*inputs)
-        entry = st.get("graph")
+        entry = st.get(name)
         if entry is None:
             static = [t.clone() for t in inputs]
-            fn(*static)
-            torch.cuda.current_stream(static[0].device).synchronize()
+            first = fn(*static)
+            torch.cuda.current_stream(static[0].device if static else device).synchronize()
             n0 = ops.launch_count()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 out = fn(*static)
-            entry = st["graph"] = (graph, static, out, ops.launch_count() - n0)
+            st[name] = (graph, static, out, ops.launch_count() - n0)
+            if stateful:
+                return first
+            entry = st[name]
         graph, static, out, n_launch = entry
         for s, t in zip(static, inputs):
             s.copy_(t)

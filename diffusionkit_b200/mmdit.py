@@ -18,6 +18,8 @@ H100 layout decisions (vs. the reference's per-module MLX graph):
     forward's launch sequence timestep-invariant (CUDA-graph capturable).
   * opt-in FP8 (`set_fp8`, DESIGN.md "FP8 linears"): the block linears run on row-scaled e4m3 copies of their weights;
     their inputs are quantised per token by the LayerNorm-modulate kernel or by a row quantiser.
+  * opt-in first-block step cache (`set_step_cache`, DESIGN.md §10): a forward whose first-block residual
+    barely changed since the last full one skips the other blocks and reuses their residual.
 """
 from __future__ import annotations
 
@@ -30,6 +32,7 @@ from . import ops
 from ._lib import ACT_GELU_ERF, ACT_NONE, ACT_SILU, DkError
 from .config import MMDiTConfig, PositionalEncoding
 from .graphs import ShapeCache, default_settings
+from .step_cache import StepCachePolicy
 
 
 def fp8_covered_linears(config: MMDiTConfig) -> List[str]:
@@ -92,6 +95,9 @@ class MMDiT:
         # set_fp8: (id(stream), packed weight attribute) -> (e4m3 copy [N, K], fp32 row scales [N])
         self._fp8_w: Dict[Tuple[int, str], Tuple[torch.Tensor, torch.Tensor]] = {}
         self._fp8 = False
+        # set_step_cache: the skip policy (None: off) and the input shape its residuals belong to
+        self._step_cache: Optional[StepCachePolicy] = None
+        self._step_cache_key = None
 
     # ------------------------------------------------------------------------------------------ weight packing
     def _pack(self, P: Dict[str, torch.Tensor]):
@@ -200,6 +206,7 @@ class MMDiT:
             self._shapes.drop_graphs()
         self._mod_batch = B
         self._mod_index = {}
+        self._reset_step_cache()
         for i, t in enumerate(ts):
             self._mod_index.setdefault(t, i)
         self._cur_t = None
@@ -241,6 +248,7 @@ class MMDiT:
         scale vector kept beside the 16-bit weight (which LoRA merges still need); disabling frees them and the e4m3
         activation buffers.  Either way the captured graphs are dropped: the launch sequence changes."""
         enabled = bool(enabled)
+        self._reset_step_cache()
         if enabled == self._fp8:
             return
         self._fp8_w = {}
@@ -250,6 +258,38 @@ class MMDiT:
         self._fp8 = enabled
         self._shapes.drop("graph")
         self._shapes.drop("ws8")
+
+    # ------------------------------------------------------------------------------------------ step cache
+    def set_step_cache(self, threshold: Optional[float], max_consecutive_skips: Optional[int] = None):
+        """First-block step cache (DESIGN.md §10), an accuracy-for-speed trade the caller makes; off by default.
+        Each forward runs the input adapters and the first block, compares that block's residual with the one of the
+        last fully computed forward (step_cache.StepCachePolicy) and, when the relative change of every sequence is
+        below `threshold` and fewer than `max_consecutive_skips` forwards in a row were skipped (None: no cap), skips
+        the other blocks and reuses their residual from that forward.  threshold None turns the cache off and frees its
+        buffers; 0 never skips.  The cache restarts (the next forward runs in full) on every call of this method,
+        cache_modulation_params, apply_lora, set_fp8 and a change of input shape or batch."""
+        if threshold is not None and not self.double:
+            raise DkError("MMDiT: the step cache needs at least one double-stream block")
+        self._step_cache = None if threshold is None else StepCachePolicy(threshold, max_consecutive_skips)
+        self._step_cache_key = None
+        self._shapes.drop("graph")
+        self._shapes.drop("sc")
+
+    @property
+    def step_cache(self) -> Optional[Tuple[float, Optional[int]]]:
+        """(threshold, max_consecutive_skips) while the step cache is on, else None"""
+        p = self._step_cache
+        return None if p is None else (p.threshold, p.max_consecutive_skips)
+
+    @property
+    def step_cache_log(self) -> List[Tuple[Optional[float], bool]]:
+        """(max rel, skipped) of every forward since the last reset (rel is None on the first, which never skips);
+        empty while the cache is off"""
+        return [] if self._step_cache is None else list(self._step_cache.log)
+
+    def _reset_step_cache(self):
+        if self._step_cache is not None:
+            self._step_cache.reset()
 
     # ------------------------------------------------------------------------------------------ LoRA merge
     def lora_weight_slots(self) -> Dict[str, Tuple[object, str, Optional[int], slice, slice]]:
@@ -350,6 +390,7 @@ class MMDiT:
                 ops.quantize_rows_e4m3(getattr(packed[(oid, attr)], attr), out=q, scale=sc)
         if rebound:
             self._shapes.drop_graphs()
+        self._reset_step_cache()
         if mod_changed:
             self.clear_modulation_params_cache()
             self._cur_t = None
@@ -501,67 +542,145 @@ class MMDiT:
                 self.select_timestep(tval)
         if self._mod_cur is None or self._mod_batch != B:
             raise DkError(f"modulation cache holds batch {self._mod_batch}, forward got batch {B}")
-        state = self._shapes.state((B, H, W, Cl, T), self.max_cached_shapes)
+        key = (B, H, W, Cl, T)
+        state = self._shapes.state(key, self.max_cached_shapes)
+        if self._step_cache is not None:
+            return self._cached_forward(state, key, x, text, B, H, W, Cl, T)
         return self._shapes.run(state, self.use_cuda_graphs,
                                 lambda xx, tt: self._forward_impl(state, xx, tt, B, H, W, Cl, T), x, text)
 
-    def _forward_impl(self, state, x, text, B, H, W, Cl, T):
+    def _geometry(self, state, B, H, W, T) -> dict:
+        """buffers and sizes of one input shape that the forward pieces below share"""
         c = self.config
         hp, wp = H // c.patch_size, W // c.patch_size
         N = hp * wp
-        S = N + T
-        h, heads, d = self.h, self.heads, self.d
-        ws = self._workspace(state, B, N, T)
-        w8 = self._workspace8(state, B, N, T).get
-        img, txt, qkv = ws["img"], ws["txt"], ws["qkv"]
+        g = {"B": B, "T": T, "N": N, "S": N + T, "hp": hp, "wp": wp, "ws": self._workspace(state, B, N, T),
+             "w8": self._workspace8(state, B, N, T).get, "state": state}
+        g["rope"] = self._rope_table(state, T, hp, wp) if c.pos_embed_type == PositionalEncoding.PreSDPARope else None
+        # joint sequence order: FLUX [text, image] (mmdit.py:594-606), SD3 [image, text] (:608-625)
+        g["off_img"], g["off_txt"], g["split"] = (T, 0, T) if self.is_flux else (0, N, N)
+        return g
 
-        # ---- input adapters (mmdit.py:195-206)
-        ops.gemm(text, self.w_ctx, out=txt, bias=self.b_ctx)
+    def _embed(self, g, x, text):
+        """input adapters (mmdit.py:195-206): text -> txt, latent -> img"""
+        c, ws, state, N = self.config, g["ws"], g["state"], g["N"]
+        ops.gemm(text, self.w_ctx, out=ws["txt"], bias=self.b_ctx)
         if c.patchify_via_reshape:
             ops.patchify(x, 0, out=ws["rows_in"])
-            ops.gemm(ws["rows_in"], self.w_x, out=img, bias=self.b_x)
+            ops.gemm(ws["rows_in"], self.w_x, out=ws["img"], bias=self.b_x)
         else:
             ops.patchify(x, 1, out=ws["rows_in"])
             if "pos" not in state:
-                state["pos"] = ops.pos_embed_crop(self.pos_table, c.max_latent_resolution, hp, wp)
-            ops.gemm(ws["rows_in"], self.w_x, out=img, bias=self.b_x, res=state["pos"], rows_per_batch=N,
+                state["pos"] = ops.pos_embed_crop(self.pos_table, c.max_latent_resolution, g["hp"], g["wp"])
+            ops.gemm(ws["rows_in"], self.w_x, out=ws["img"], bias=self.b_x, res=state["pos"], rows_per_batch=N,
                      out_batch_rows=N, res_batch_rows=0)
 
-        rope = self._rope_table(state, T, hp, wp) if c.pos_embed_type == PositionalEncoding.PreSDPARope else None
-        # joint sequence order: FLUX [text, image] (mmdit.py:594-606), SD3 [image, text] (:608-625)
+    def _double_block(self, g, i: int):
+        ws, w8, B, N, T, S, rope = g["ws"], g["w8"], g["B"], g["N"], g["T"], g["S"], g["rope"]
+        img, txt, qkv = ws["img"], ws["txt"], ws["qkv"]
+        si, st = self.double[i]
+        self._attn_stream_pre(si, img, ws["m_img"], w8("m_img"), N, S, g["off_img"], qkv, rope)
+        self._attn_stream_pre(st, txt, ws["m_txt"], w8("m_txt"), T, S, g["off_txt"], qkv, rope)
         if self.is_flux:
-            off_img, off_txt, split = T, 0, T
+            ops.attention(qkv, B, S, self.heads, self.d, ws["o_txt"], split=g["split"], out1=ws["o_img"])
         else:
-            off_img, off_txt, split = 0, N, N
+            ops.attention(qkv, B, S, self.heads, self.d, ws["o_img"], split=g["split"], out1=ws["o_txt"])
+        self._stream_post(si, img, ws["o_img"], ws["m_img"], w8("m_img"), ws["hid_img"], w8("hid_img"), N)
+        if not st.skip_post:
+            self._stream_post(st, txt, ws["o_txt"], ws["m_txt"], w8("m_txt"), ws["hid_txt"], w8("hid_txt"), T)
 
-        for (si, st) in self.double:
-            self._attn_stream_pre(si, img, ws["m_img"], w8("m_img"), N, S, off_img, qkv, rope)
-            self._attn_stream_pre(st, txt, ws["m_txt"], w8("m_txt"), T, S, off_txt, qkv, rope)
-            if self.is_flux:
-                ops.attention(qkv, B, S, heads, d, ws["o_txt"], split=split, out1=ws["o_img"])
-            else:
-                ops.attention(qkv, B, S, heads, d, ws["o_img"], split=split, out1=ws["o_txt"])
-            self._stream_post(si, img, ws["o_img"], ws["m_img"], w8("m_img"), ws["hid_img"], w8("hid_img"), N)
-            if not st.skip_post:
-                self._stream_post(st, txt, ws["o_txt"], ws["m_txt"], w8("m_txt"), ws["hid_txt"], w8("hid_txt"), T)
+    def _single_blocks(self, g):
+        """FLUX: u = [text | image], every single-stream block, image rows of u back to img (nothing for SD3)"""
+        if not self.is_flux:
+            return
+        ws, w8, B, N, T, S, rope, h = g["ws"], g["w8"], g["B"], g["N"], g["T"], g["S"], g["rope"], self.h
+        img, txt, qkv = ws["img"], ws["txt"], ws["qkv"]
+        u, m_u, cat = ws["u"], ws["m_u"], ws["cat"]
+        ops.copy_rows(txt, u, B, T, h, S, 0, T, 0)                                     # u = [text | image] (:234-236)
+        ops.copy_rows(img, u, B, N, h, S, T, N, 0)
+        for s in self.single:                                                          # mmdit.py:693-751
+            a = self._ln_mod(u, s, 0, S, m_u, w8("m_u"))
+            self._linear(a, s, "w_qkv", out=qkv, bias=s.b_qkv, rows_per_batch=S, out_batch_rows=S,
+                         qk=self._qk_fused(s, rope))
+            ops.attention(qkv, B, S, self.heads, self.d, cat[:, :h])
+            self._linear(a, s, "w_fc1", out=cat[:, h:], bias=s.b_fc1, act=ACT_GELU_ERF)
+            self._linear(self._lin_in(cat, w8("cat")), s, "w_out", out=u, bias=s.b_o, gate=self._mod(s.mod_off, 2),
+                         res=u, rows_per_batch=S, out_batch_rows=S)
+        ops.copy_rows(u, img, B, N, h, N, 0, S, T)                                     # image part (:245-247)
 
-        if self.is_flux:
-            u, m_u, cat = ws["u"], ws["m_u"], ws["cat"]
-            ops.copy_rows(txt, u, B, T, h, S, 0, T, 0)                                 # u = [text | image] (:234-236)
-            ops.copy_rows(img, u, B, N, h, S, T, N, 0)
-            for s in self.single:                                                      # mmdit.py:693-751
-                a = self._ln_mod(u, s, 0, S, m_u, w8("m_u"))
-                self._linear(a, s, "w_qkv", out=qkv, bias=s.b_qkv, rows_per_batch=S, out_batch_rows=S,
-                             qk=self._qk_fused(s, rope))
-                ops.attention(qkv, B, S, heads, d, cat[:, :h])
-                self._linear(a, s, "w_fc1", out=cat[:, h:], bias=s.b_fc1, act=ACT_GELU_ERF)
-                self._linear(self._lin_in(cat, w8("cat")), s, "w_out", out=u, bias=s.b_o, gate=self._mod(s.mod_off, 2),
-                             res=u, rows_per_batch=S, out_batch_rows=S)
-            ops.copy_rows(u, img, B, N, h, N, 0, S, T)                                 # image part (:245-247)
-
-        # ---- final layer (mmdit.py:780-796) + unpatchify / unpack
-        ops.ln_modulate(img, self._mod(self.final_mod_off, 0), self._mod(self.final_mod_off, 1), N, c.layer_norm_eps,
-                        out=ws["m_img"])
+    def _final_layer(self, g, H, W, Cl):
+        """final layer (mmdit.py:780-796) on img + unpatchify / unpack"""
+        c, ws = self.config, g["ws"]
+        ops.ln_modulate(ws["img"], self._mod(self.final_mod_off, 0), self._mod(self.final_mod_off, 1), g["N"],
+                        c.layer_norm_eps, out=ws["m_img"])
         ops.gemm(ws["m_img"], self.w_final, out=ws["rows_out"], bias=self.b_final)
-        out = ops.unpatchify(ws["rows_out"], B, H, W, Cl, 0 if c.patchify_via_reshape else 1)
-        return out
+        return ops.unpatchify(ws["rows_out"], g["B"], H, W, Cl, 0 if c.patchify_via_reshape else 1)
+
+    def _forward_impl(self, state, x, text, B, H, W, Cl, T):
+        g = self._geometry(state, B, H, W, T)
+        self._embed(g, x, text)
+        for i in range(len(self.double)):
+            self._double_block(g, i)
+        self._single_blocks(g)
+        return self._final_layer(g, H, W, Cl)
+
+    # ------------------------------------------------------------------------------------------ step cache
+    # The cached forward is three pieces per shape, each its own captured graph when graphs are on:
+    #   head  embedders, e -> snap, block 0 (img = a), r0 = a - e and its per-sequence sums against r0prev;
+    #   tail  a -> snap, the other blocks (img = f), R = f - a, r0prev = r0, final layer;
+    #   skip  img = round16(a + R), final layer.
+    # Between head and the rest the host reads the sums (one stream synchronise per step) and decides.
+    def _step_cache_buffers(self, state: dict, B: int, N: int) -> dict:
+        if "sc" in state:
+            return state["sc"]
+        h, dev = self.h, self.device
+
+        def f32(*shape):
+            return torch.empty(shape, dtype=torch.float32, device=dev)
+
+        state["sc"] = {"snap": torch.empty((B * N, h), dtype=self.dtype, device=dev), "r0": f32(B * N, h),
+                       "r0prev": torch.zeros((B * N, h), dtype=torch.float32, device=dev), "R": f32(B * N, h),
+                       "sums": f32(B, 2), "ws": f32(B * 512),
+                       "host": torch.empty((B, 2), dtype=torch.float32, pin_memory=True)}
+        return state["sc"]
+
+    def _head_impl(self, state, x, text, B, H, W, Cl, T):
+        g = self._geometry(state, B, H, W, T)
+        sc, img, BN = state["sc"], g["ws"]["img"], B * g["N"]
+        self._embed(g, x, text)
+        ops.copy_rows(img, sc["snap"], 1, BN, self.h, BN, 0, BN, 0)                 # e
+        self._double_block(g, 0)
+        return ops.residual_delta(img, sc["snap"], B, g["N"], r_out=sc["r0"], prev=sc["r0prev"], sums=sc["sums"],
+                                  ws=sc["ws"])
+
+    def _tail_impl(self, state, B, H, W, Cl, T):
+        g = self._geometry(state, B, H, W, T)
+        sc, img, BN = state["sc"], g["ws"]["img"], B * g["N"]
+        ops.copy_rows(img, sc["snap"], 1, BN, self.h, BN, 0, BN, 0)                 # a
+        for i in range(1, len(self.double)):
+            self._double_block(g, i)
+        self._single_blocks(g)
+        ops.residual_delta(img, sc["snap"], B, g["N"], r_out=sc["R"])                 # R = f - a
+        # r0prev = r0: a bit copy of the fp32 rows, viewed as twice as many 16-bit columns
+        ops.copy_rows(sc["r0"].view(self.dtype), sc["r0prev"].view(self.dtype), 1, BN, 2 * self.h, BN, 0, BN, 0)
+        return self._final_layer(g, H, W, Cl)
+
+    def _skip_impl(self, state, B, H, W, Cl, T):
+        g = self._geometry(state, B, H, W, T)
+        ops.residual_apply(g["ws"]["img"], state["sc"]["R"], out=g["ws"]["img"])    # f = round16(a + R)
+        return self._final_layer(g, H, W, Cl)
+
+    def _cached_forward(self, state, key, x, text, B, H, W, Cl, T):
+        policy = self._step_cache
+        if key != self._step_cache_key:
+            policy.reset()
+            self._step_cache_key = key
+        sc = self._step_cache_buffers(state, B, (H // self.config.patch_size) * (W // self.config.patch_size))
+        graphs = self.use_cuda_graphs
+        self._shapes.run(state, graphs, lambda xx, tt: self._head_impl(state, xx, tt, B, H, W, Cl, T), x, text,
+                         name="graph.head")
+        sc["host"].copy_(sc["sums"], non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        part = self._skip_impl if policy.step(sc["host"].tolist()) else self._tail_impl
+        return self._shapes.run(state, graphs, lambda: part(state, B, H, W, Cl, T), stateful=True, device=self.device,
+                                name="graph.skip" if part == self._skip_impl else "graph.tail")

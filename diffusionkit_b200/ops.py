@@ -433,6 +433,42 @@ def cast_to_f32(x, out=None):
     return out
 
 
+def residual_delta(x, base, nseq: int, rows: int, x_seq_rows: Optional[int] = None,
+                   b_seq_rows: Optional[int] = None, r_out=None, prev=None, sums=None, ws=None):
+    """r = fp32(x) - fp32(base) over nseq sequences of `rows` rows (x, base: 2-D 16-bit views whose row stride is the
+    leading dimension; sequence s starts at row s * x_seq_rows, default rows).  r_out [nseq * rows, h] fp32 receives r;
+    with prev (same shape), returns sums [nseq, 2] = (Σ|r - prev|, Σ|prev|) per sequence, reduced deterministically."""
+    _chk16(x, "residual_delta.x")
+    _chk16(base, "residual_delta.base")
+    assert x.dim() == 2 and base.dim() == 2 and x.stride(1) == 1 and base.stride(1) == 1 and x.dtype == base.dtype
+    h = x.shape[1]
+    for t in (r_out, prev):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.numel() == nseq * rows * h)
+    if prev is not None:
+        if sums is None:
+            sums = torch.empty((nseq, 2), dtype=torch.float32, device=x.device)
+        if ws is None:
+            ws = torch.empty((nseq * 512,), dtype=torch.float32, device=x.device)
+        assert sums.dtype == torch.float32 and sums.numel() >= 2 * nseq and ws.numel() >= 512 * nseq
+    c = ctx(x.device.index)
+    c.call("dk_residual_delta", dtype_code(x.dtype), ptr(x), x.stride(0), rows if x_seq_rows is None else x_seq_rows,
+           ptr(base), base.stride(0), rows if b_seq_rows is None else b_seq_rows, ptr(r_out), ptr(prev), ptr(sums),
+           ptr(ws), nseq, rows, h)
+    return sums
+
+
+def residual_apply(x, r, out=None):
+    """out = round16(x + r): x 16-bit, r fp32, both contiguous with the same number of elements; out may be x."""
+    _chk16(x, "residual_apply.x")
+    assert x.is_contiguous() and r.dtype == torch.float32 and r.is_contiguous() and r.numel() == x.numel()
+    if out is None:
+        out = torch.empty_like(x)
+    assert out.dtype == x.dtype and out.is_contiguous() and out.numel() == x.numel()
+    c = ctx(x.device.index)
+    c.call("dk_residual_apply", dtype_code(x.dtype), ptr(x), ptr(r), ptr(out), x.numel())
+    return out
+
+
 def groupnorm_stats(x, G: int, eps: float = 1e-5, ws=None):
     """x NHWC [B, H, W, C] -> stats [B, G, 2] (mean, rstd)."""
     _chk16(x, "groupnorm_stats.x")

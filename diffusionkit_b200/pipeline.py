@@ -327,6 +327,18 @@ class DiffusionPipeline:
     def fp8(self) -> bool:
         return self.mmdit.fp8
 
+    # ------------------------------------------------------------------ step cache (DESIGN.md §10)
+    def set_step_cache(self, threshold: Optional[float], max_consecutive_skips: Optional[int] = None):
+        """Skip the MMDiT blocks after the first on denoise steps whose first-block residual changed by less than
+        `threshold` (relative L1) since the last full step (MMDiT.set_step_cache): faster, less accurate; off by
+        default, None turns it off.  generate_image then logs each step's change and decision."""
+        self.mmdit.set_step_cache(threshold, max_consecutive_skips)
+
+    @property
+    def step_cache(self) -> Optional[Tuple[float, Optional[int]]]:
+        """(threshold, max_consecutive_skips) while the step cache is on, else None"""
+        return self.mmdit.step_cache
+
     # ------------------------------------------------------------------ text (SURVEY.md §8 row f2)
     def load_text_encoders(self, clip_l=None, clip_g=None, t5=None, *, tokenizer_l=None, tokenizer_g=None,
                            t5_tokenizer=None, clip_l_config=None, clip_g_config=None, t5_config=None):
@@ -540,6 +552,9 @@ class DiffusionPipeline:
         log["denoising"]["post"] = mem()
         log["denoising"]["time"] = round(time.time() - t0, 3)
         log["denoising"]["iter_time"] = iter_time
+        if self.mmdit.step_cache is not None:
+            log["denoising"]["step_cache"] = [{"rel": rel, "skipped": skipped}
+                                              for rel, skipped in self.mmdit.step_cache_log]
         log["peak_memory"] = max(log["peak_memory"], log["denoising"]["post"]["peak_memory"])
 
         torch.cuda.reset_peak_memory_stats(self.device)

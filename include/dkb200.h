@@ -230,6 +230,16 @@ int dk_vae_sample_latent(dk_ctx* ctx, int dtype, const void* hidden, const float
 /* fp32 <-> 16-bit casts */
 int dk_cast_f32_to_16(dk_ctx* ctx, int dtype, const float* x, void* y, long long n, void* stream);
 int dk_cast_16_to_f32(dk_ctx* ctx, int dtype, const void* x, float* y, long long n, void* stream);
+/* First-block step cache (opt-in, MMDiT.set_step_cache).  Over nseq sequences of `rows` rows of width h:
+ *     r = fp32(x) - fp32(base), row r of sequence s at x + (s * x_seq_rows + r) * ldx (base likewise);
+ * r_out [nseq * rows, h] fp32 or NULL receives r; with prev [nseq * rows, h] fp32, sums [nseq, 2] fp32 receives
+ * (sum |r - prev|, sum |prev|) per sequence, reduced in a fixed order without atomics (two launches are bit-identical);
+ * ws is scratch of nseq * 512 floats.  prev NULL: no sums (store only).  16-byte aligned x, base, r_out, prev. */
+int dk_residual_delta(dk_ctx* ctx, int dtype, const void* x, long long ldx, int x_seq_rows, const void* base,
+                      long long ldb, int b_seq_rows, float* r_out, const float* prev, float* sums, float* ws, int nseq,
+                      int rows, int h, void* stream);
+/* out = round16(x + r), x and out 16-bit, r fp32, n elements (one fp32 add, one rounding); out may alias x */
+int dk_residual_apply(dk_ctx* ctx, int dtype, const void* x, const float* r, void* out, long long n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * VAE decoder kernels (vae.py:20-149, 336-401)
