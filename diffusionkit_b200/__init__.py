@@ -12,8 +12,8 @@ from .config import FLUX_DEV, FLUX_SCHNELL, SD3_2b, SD3_8b, MMDiTConfig, VAEDeco
 from .lora import LoRA, load_lora  # noqa: F401
 from .mmdit import MMDiT  # noqa: F401
 from .pipeline import (CFGDenoiser, DiffusionPipeline, FluxLatentFormat, FluxPipeline, LatentFormat,  # noqa: F401
-                       SD3LatentFormat, sample_euler)
-from .sampler import FluxSampler, ModelSamplingDiscreteFlow  # noqa: F401
+                       SD3LatentFormat, sample_dpmpp_2m, sample_euler, sample_heun)
+from .sampler import FluxSampler, ModelSamplingDiscreteFlow, dpmpp_2m_coefficients  # noqa: F401
 from .vae import VAEDecoder, VAEEncoder  # noqa: F401
 
 __version__ = "0.1.0"

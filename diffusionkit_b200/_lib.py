@@ -64,6 +64,9 @@ SIGNATURES = {
     "dk_copy_rows": (i32, [vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
     "dk_sampler_prepare": (i32, [vp, i32, vp, vp, i64, i32, vp]),
     "dk_sampler_step": (i32, [vp, i32, vp, vp, vp, i64, f32, f32, f32, vp]),
+    "dk_sampler_heun_predict": (i32, [vp, i32, vp, vp, vp, vp, vp, i64, f32, f32, f32, vp]),
+    "dk_sampler_heun_correct": (i32, [vp, i32, vp, vp, vp, vp, vp, i64, f32, f32, f32, vp]),
+    "dk_sampler_dpmpp_2m": (i32, [vp, i32, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, vp]),
     "dk_axpb_f32": (i32, [vp, vp, vp, i64, f32, f32, vp]),
     "dk_embedding": (i32, [vp, i32, vp, vp, vp, vp, i64, i32, i32, i32, vp]),
     "dk_layernorm": (i32, [vp, i32, vp, vp, vp, vp, i32, i32, f32, vp]),

@@ -402,20 +402,69 @@ __global__ void sampler_prepare_kernel(const float* __restrict__ x, T* __restric
     for (int k = 0; k < reps; ++k) xin[k * n + i] = v;
   }
 }
+// The CFG-mixed denoised estimate D of element i, shared by every sampler update.  The negative rows sit n elements
+// after the positive ones ([positive x B | negative x B], reference :718).
+template <typename T>
+__device__ __forceinline__ float cfg_denoised(const T* __restrict__ xin, const T* __restrict__ out, long long n,
+                                              long long i, float sigma, float cfg) {
+  // calculate_denoised: model_input - model_output * sigma (fp32 sigma promotes to fp32)
+  float den = Half16<T>::to_f(xin[i]) - Half16<T>::to_f(out[i]) * sigma;
+  if (cfg > 0.f) {
+    const float den_neg = Half16<T>::to_f(xin[n + i]) - Half16<T>::to_f(out[n + i]) * sigma;
+    den = den_neg + cfg * (den - den_neg);
+  }
+  return den;
+}
 template <typename T>
 __global__ void sampler_step_kernel(float* __restrict__ x, const T* __restrict__ xin, const T* __restrict__ out,
                                     long long n, float sigma, float sigma_next, float cfg) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    // calculate_denoised: model_input - model_output * sigma (fp32 sigma promotes to fp32)
-    float den = Half16<T>::to_f(xin[i]) - Half16<T>::to_f(out[i]) * sigma;
-    if (cfg > 0.f) {
-      const float den_neg = Half16<T>::to_f(xin[n + i]) - Half16<T>::to_f(out[n + i]) * sigma;
-      den = den_neg + cfg * (den - den_neg);
-    }
+    const float den = cfg_denoised(xin, out, n, i, sigma, cfg);
     const float xv = x[i];
     const float d = (xv - den) / sigma;          // to_d
     x[i] = xv + d * (sigma_next - sigma);        // Euler
+  }
+}
+// Heun predictor (Karras et al. 2022, Alg. 2): the Euler step to x2, keeping its slope d for the corrector; x is
+// left as it is.
+template <typename T>
+__global__ void sampler_heun_predict_kernel(const float* __restrict__ x, const T* __restrict__ xin,
+                                            const T* __restrict__ out, float* __restrict__ d, float* __restrict__ x2,
+                                            long long n, float sigma, float sigma_next, float cfg) {
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float xv = x[i];
+    const float dv = (xv - cfg_denoised(xin, out, n, i, sigma, cfg)) / sigma;
+    d[i] = dv;
+    x2[i] = xv + dv * (sigma_next - sigma);
+  }
+}
+// Heun corrector: xin / out are the forward at (x2, sigma_next); x moves by the mean of the two slopes.
+template <typename T>
+__global__ void sampler_heun_correct_kernel(float* __restrict__ x, const float* __restrict__ d,
+                                            const float* __restrict__ x2, const T* __restrict__ xin,
+                                            const T* __restrict__ out, long long n, float sigma, float sigma_next,
+                                            float cfg) {
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float d2 = (x2[i] - cfg_denoised(xin, out, n, i, sigma_next, cfg)) / sigma_next;
+    x[i] += (d[i] + d2) * 0.5f * (sigma_next - sigma);
+  }
+}
+// DPM-Solver++(2M): x <- a x + b D + c D_prev, then D_prev <- D.  d_prev is not read when c == 0: on the first step
+// it holds whatever the allocation held, and 0 * NaN is NaN.
+template <typename T>
+__global__ void sampler_dpmpp_2m_kernel(float* __restrict__ x, float* __restrict__ d_prev, const T* __restrict__ xin,
+                                        const T* __restrict__ out, long long n, float sigma, float a, float b, float c,
+                                        float cfg) {
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float den = cfg_denoised(xin, out, n, i, sigma, cfg);
+    float v = a * x[i] + b * den;
+    if (c != 0.f) v += c * d_prev[i];
+    x[i] = v;
+    d_prev[i] = den;
   }
 }
 __global__ void axpb_kernel(const float* __restrict__ x, float* __restrict__ y, long long n, float a, float b) {
@@ -1102,6 +1151,47 @@ extern "C" int dk_sampler_step(dk_ctx* ctx, int dtype, float* x, const void* xin
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DK_DISPATCH(dtype, (sampler_step_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
                          x, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, sigma_next, cfg_weight)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_sampler_heun_predict(dk_ctx* ctx, int dtype, const float* x, const void* xin, const void* out,
+                                       float* d, float* x2, long long n, float sigma, float sigma_next,
+                                       float cfg_weight, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(sigma != 0.f, "dk_sampler_heun_predict: sigma must be non-zero");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (sampler_heun_predict_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+                         x, static_cast<const T*>(xin), static_cast<const T*>(out), d, x2, n, sigma, sigma_next,
+                         cfg_weight)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_sampler_heun_correct(dk_ctx* ctx, int dtype, float* x, const float* d, const float* x2,
+                                       const void* xin, const void* out, long long n, float sigma, float sigma_next,
+                                       float cfg_weight, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(sigma_next != 0.f, "dk_sampler_heun_correct: sigma_next must be non-zero (the last step is an Euler step)");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (sampler_heun_correct_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+                         x, d, x2, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, sigma_next,
+                         cfg_weight)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_sampler_dpmpp_2m(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin, const void* out,
+                                   long long n, float sigma, float a, float b, float c, float cfg_weight,
+                                   void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (sampler_dpmpp_2m_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+                         x, d_prev, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, a, b, c,
+                         cfg_weight)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }

@@ -27,7 +27,7 @@ from . import ops
 from ._lib import DkError
 from .config import MODEL_CONFIGS, T5_MAX_LENGTH, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig
 from .mmdit import MMDiT
-from .sampler import FluxSampler, ModelSamplingDiscreteFlow
+from .sampler import FluxSampler, ModelSamplingDiscreteFlow, dpmpp_2m_coefficients
 from .vae import VAEDecoder, VAEEncoder
 from .weights import init_params, mmdit_param_specs, vae_decoder_param_specs, vae_encoder_param_specs
 
@@ -98,9 +98,9 @@ class CFGDenoiser:
         return xin, out
 
 
-def sample_euler(model: CFGDenoiser, x, sigmas, extra_args=None):
-    """Implements Algorithm 2 (Euler steps) from Karras et al. (2022) — reference mlx/__init__.py:761-788.
-    x: (B, H, W, 16) fp32 device tensor (updated in place); sigmas: 1-D float32 numpy/torch array."""
+def _start_sampling(model: CFGDenoiser, sigmas, extra_args):
+    """What every sampler does first: the timesteps of the schedule into the modulation cache.
+    -> (sigmas fp32, timesteps, conditioning, cfg_weight, events (one per sigma, the first recorded))"""
     extra_args = {} if extra_args is None else dict(extra_args)
     pipe = model.model
     sig = np.asarray(sigmas, dtype=np.float32)
@@ -113,15 +113,70 @@ def sample_euler(model: CFGDenoiser, x, sigmas, extra_args=None):
     conditioning = extra_args["conditioning"]
     events = [torch.cuda.Event(enable_timing=True) for _ in range(len(sig))]
     events[0].record()
+    return sig, timesteps, conditioning, cfg_weight, events
+
+
+def _finish_sampling(model: CFGDenoiser, events):
+    """-> iter_time: seconds per step, from the events recorded after each step"""
+    model.clear_cache()
+    torch.cuda.current_stream().synchronize()  # the reference syncs every step (mx.eval, :782); once is enough here
+    return [round(events[i].elapsed_time(events[i + 1]) / 1e3, 3) for i in range(len(events) - 1)]
+
+
+def sample_euler(model: CFGDenoiser, x, sigmas, extra_args=None):
+    """Implements Algorithm 2 (Euler steps) from Karras et al. (2022) — reference mlx/__init__.py:761-788.
+    x: (B, H, W, 16) fp32 device tensor (updated in place); sigmas: 1-D float32 numpy/torch array."""
+    sig, timesteps, conditioning, cfg_weight, events = _start_sampling(model, sigmas, extra_args)
     for i in range(len(sig) - 1):
         xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight)
         # denoised = xin - out * sigma; CFG mix; d = (x - denoised) / sigma; x += d * (sigma_next - sigma)
         ops.sampler_step(x, xin, out, float(sig[i]), float(sig[i + 1]), cfg_weight)
         events[i + 1].record()
-    model.clear_cache()
-    torch.cuda.current_stream().synchronize()  # the reference syncs every step (mx.eval, :782); once is enough here
-    iter_time = [round(events[i].elapsed_time(events[i + 1]) / 1e3, 3) for i in range(len(sig) - 1)]
-    return x, iter_time
+    return x, _finish_sampling(model, events)
+
+
+def sample_heun(model: CFGDenoiser, x, sigmas, extra_args=None):
+    """Heun's method, Algorithm 2 of Karras et al. (2022) without churn, on the ODE sample_euler integrates: an Euler
+    predictor to x2, then a corrector with the slope at (x2, sigma_next) — two forwards per step; a step to sigma = 0
+    is the plain Euler step.  Same arguments and return value as sample_euler; iter_time has one entry per step."""
+    sig, timesteps, conditioning, cfg_weight, events = _start_sampling(model, sigmas, extra_args)
+    d = x2 = None
+    for i in range(len(sig) - 1):
+        s, s_next = float(sig[i]), float(sig[i + 1])
+        xin, out = model(x, timesteps[i], s, conditioning, cfg_weight)
+        if s_next == 0.0:
+            ops.sampler_step(x, xin, out, s, s_next, cfg_weight)
+        else:
+            if d is None:
+                d, x2 = torch.empty_like(x), torch.empty_like(x)
+            ops.sampler_heun_predict(x, xin, out, s, s_next, cfg_weight, d, x2)
+            xin, out = model(x2, timesteps[i + 1], s_next, conditioning, cfg_weight)
+            ops.sampler_heun_correct(x, d, x2, xin, out, s, s_next, cfg_weight)
+        events[i + 1].record()
+    return x, _finish_sampling(model, events)
+
+
+def sample_dpmpp_2m(model: CFGDenoiser, x, sigmas, extra_args=None):
+    """DPM-Solver++(2M) (Lu et al. 2022) on the same ODE: one forward per step, the previous step's denoised estimate
+    kept on the device; coefficients from sampler.dpmpp_2m_coefficients.  Same arguments and return value as
+    sample_euler."""
+    sig, timesteps, conditioning, cfg_weight, events = _start_sampling(model, sigmas, extra_args)
+    coef = dpmpp_2m_coefficients(sig)
+    d_prev = torch.empty_like(x)
+    for i in range(len(sig) - 1):
+        xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight)
+        a, b, c = (float(v) for v in coef[i])
+        ops.sampler_dpmpp_2m(x, d_prev, xin, out, float(sig[i]), a, b, c, cfg_weight)
+        events[i + 1].record()
+    return x, _finish_sampling(model, events)
+
+
+SOLVERS = {"euler": sample_euler, "heun": sample_heun, "dpmpp_2m": sample_dpmpp_2m}
+
+
+def _check_solver(solver: str):
+    if solver not in SOLVERS:
+        raise ValueError(f"unknown solver {solver!r}: expected one of {', '.join(repr(k) for k in SOLVERS)}")
 
 
 class DiffusionPipeline:
@@ -438,11 +493,14 @@ class DiffusionPipeline:
         denoise: float = 1.0,
         *,
         noise: Optional[torch.Tensor] = None,
+        solver: str = "euler",
     ):
         """-> (latent NHWC (B, H, W, 16) fp32 on the device, iter_time list).  `noise` (optional, device fp32
         (B, H, W, 16)) replaces the host-side numpy draw of get_noise for callers whose inputs already live in HBM.
         `image_path` (img2img): a file path, a PIL image or a uint8 HWC array; the latent size then follows the image
-        (the reference ignores latent_size in that case too, :273)."""
+        (the reference ignores latent_size in that case too, :273).  `solver`: "euler" (the reference's sampler),
+        "heun" (two model evaluations per step but the last) or "dpmpp_2m" (one per step), DESIGN.md §11."""
+        _check_solver(solver)
         if image_path is None:
             denoise = 1.0                                                   # :270-271
         elif not (0.0 <= denoise <= 1.0):
@@ -498,7 +556,7 @@ class DiffusionPipeline:
             x = ops.axpby(noise, x_T, s0, 1.0 - s0)
         extra_args = {"conditioning": conditioning, "cfg_weight": cfg_weight,
                       "pooled_conditioning": pooled_conditioning}
-        latent, iter_time = sample_euler(CFGDenoiser(self), x, sigmas, extra_args=extra_args)
+        latent, iter_time = SOLVERS[solver](CFGDenoiser(self), x, sigmas, extra_args=extra_args)
         latent = ops.axpb(latent, 1.0 / self.latent_format.scale_factor, self.latent_format.shift_factor)  # process_out
         return latent, iter_time
 
@@ -517,7 +575,9 @@ class DiffusionPipeline:
         *,
         conditioning=None,
         pooled_conditioning=None,
+        solver: str = "euler",
     ):
+        _check_solver(solver)
         assert latent_size[0] % 2 == 0, f"Height must be divisible by 16 ({latent_size[0]*8}/16={latent_size[0]/2})"
         assert latent_size[1] % 2 == 0, f"Width must be divisible by 16 ({latent_size[1]*8}/16={latent_size[1]/2})"
         self.check_and_load_models()
@@ -547,11 +607,16 @@ class DiffusionPipeline:
         log["denoising"]["pre"] = mem()
         latents, iter_time = self.denoise_latents(conditioning, pooled_conditioning, num_steps=num_steps,
                                                   cfg_weight=cfg_weight, latent_size=latent_size, seed=seed,
-                                                  image_path=image_path, denoise=denoise)
+                                                  image_path=image_path, denoise=denoise, solver=solver)
         torch.cuda.synchronize(self.device)
         log["denoising"]["post"] = mem()
         log["denoising"]["time"] = round(time.time() - t0, 3)
         log["denoising"]["iter_time"] = iter_time
+        if solver != "euler":
+            # every schedule ends at sigma = 0, and only there: a Heun step costs two forwards except the last
+            n = len(iter_time)
+            log["denoising"]["solver"] = solver
+            log["denoising"]["nfe"] = max(2 * n - 1, 0) if solver == "heun" else n
         if self.mmdit.step_cache is not None:
             log["denoising"]["step_cache"] = [{"rel": rel, "skipped": skipped}
                                               for rel, skipped in self.mmdit.step_cache_log]

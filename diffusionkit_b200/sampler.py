@@ -1,7 +1,8 @@
 """Sampler schedules — same classes and methods as the reference (python/src/diffusionkit/mlx/sampler.py:10-77).
 
 Host-side scalar arithmetic (numpy fp32, like the reference's fp32 mx arrays); the per-step tensor math runs in the
-fused CUDA sampler kernels (csrc/elementwise.cu: dk_sampler_prepare / dk_sampler_step).
+fused CUDA sampler kernels (csrc/elementwise.cu: dk_sampler_prepare / dk_sampler_step, and the Heun and
+DPM-Solver++(2M) updates, whose fp64 coefficients dpmpp_2m_coefficients computes).
 """
 import numpy as np
 
@@ -46,3 +47,32 @@ class FluxSampler(ModelSamplingDiscreteFlow):
     """Helper for sampler scheduling for Flux models (sampler.py:45-77): table over t = 0..1000."""
 
     _t_first = 0
+
+
+def dpmpp_2m_coefficients(sigmas) -> np.ndarray:
+    """DPM-Solver++(2M) (Lu et al. 2022) for x = (1 - sigma) x0 + sigma eps, as per-step coefficients of
+    x_{i+1} = a x_i + b D_i + c D_{i-1} (dk_sampler_dpmpp_2m), in fp64 -> (n, 3) for n + 1 sigmas.
+
+    alpha = 1 - sigma, lambda = log(alpha / sigma), h_i = lambda_{i+1} - lambda_i.  First order, a = sigma_{i+1} /
+    sigma_i and b = -alpha_{i+1} expm1(-h_i), is the Euler step; sigma_i = 1 gives h_i = inf and b = alpha_{i+1}.
+    Second order extrapolates D' = (1 + 1/(2r)) D_i - 1/(2r) D_{i-1}, r = h_{i-1} / h_i.  It is used except on the
+    first step, after an interval with h = inf, and on the last two steps: on the SD3 schedules the step from about
+    1/n down to sigma_min has r << 1, and extrapolating across it is less accurate than Euler.  A step to sigma = 0
+    returns D_i: (0, 1, 0)."""
+    s = np.asarray(sigmas, dtype=np.float64)
+    n = len(s) - 1
+    with np.errstate(divide="ignore"):
+        lam = np.log1p(-s) - np.log(s)                  # -inf at sigma = 1, +inf at sigma = 0
+    h = lam[1:] - lam[:-1]
+    coef = np.zeros((n, 3), dtype=np.float64)
+    for i in range(n):
+        if s[i + 1] == 0.0:
+            coef[i] = (0.0, 1.0, 0.0)
+            continue
+        b1 = -(1.0 - s[i + 1]) * np.expm1(-h[i])
+        if 1 <= i < n - 2 and np.isfinite(h[i - 1]):
+            half_r = 0.5 * h[i] / h[i - 1]              # 1 / (2r)
+            coef[i] = (s[i + 1] / s[i], b1 * (1.0 + half_r), -b1 * half_r)
+        else:
+            coef[i] = (s[i + 1] / s[i], b1, 0.0)
+    return coef

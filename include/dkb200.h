@@ -186,10 +186,22 @@ int dk_copy_rows(dk_ctx* ctx, int dtype, const void* src, void* dst, int B, int 
  *   dk_sampler_prepare: xin[(k*B + b)] = cast16(x[b]) for k in 0..reps-1  (reps = 2 when cfg > 0, :700-706)
  *   dk_sampler_step:    den = float(xin) - float(out) * sigma; if cfg: den = den_neg + w (den_text - den_neg)
  *                       x += ((x - den) / sigma) * (sigma_next - sigma)
+ *   Higher-order solvers of the same ODE dx/dsigma = (x - D(x, sigma)) / sigma, D = den above (DESIGN.md §11):
+ *   dk_sampler_heun_predict: d = (x - D(x, sigma)) / sigma; x2 = x + d * (sigma_next - sigma)   (x unchanged)
+ *   dk_sampler_heun_correct: xin / out = forward at (x2, sigma_next), sigma_next != 0:
+ *                            d2 = (x2 - D(x2, sigma_next)) / sigma_next; x += (d + d2) / 2 * (sigma_next - sigma)
+ *   dk_sampler_dpmpp_2m:     x = a x + b D + c d_prev; d_prev = D   (d_prev not read when c == 0; a, b, c from
+ *                            sampler.dpmpp_2m_coefficients)
  * ------------------------------------------------------------------------------------------- */
 int dk_sampler_prepare(dk_ctx* ctx, int dtype, const float* x, void* xin, long long n_per_rep, int reps, void* stream);
 int dk_sampler_step(dk_ctx* ctx, int dtype, float* x, const void* xin, const void* out, long long n, float sigma,
                     float sigma_next, float cfg_weight, void* stream);
+int dk_sampler_heun_predict(dk_ctx* ctx, int dtype, const float* x, const void* xin, const void* out, float* d,
+                            float* x2, long long n, float sigma, float sigma_next, float cfg_weight, void* stream);
+int dk_sampler_heun_correct(dk_ctx* ctx, int dtype, float* x, const float* d, const float* x2, const void* xin,
+                            const void* out, long long n, float sigma, float sigma_next, float cfg_weight, void* stream);
+int dk_sampler_dpmpp_2m(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin, const void* out, long long n,
+                        float sigma, float a, float b, float c, float cfg_weight, void* stream);
 /* y = x * a + b (fp32): latent_format.process_out (__init__.py:732-733) and noise scaling (sampler.py:41-42) */
 int dk_axpb_f32(dk_ctx* ctx, const float* x, float* y, long long n, float a, float b, void* stream);
 /* ---- text encoders (SURVEY.md §8 row f2): CLIP-L/G (mlx/clip.py) and the T5-XXL encoder (mlx/t5.py) ------------- */
