@@ -13,7 +13,7 @@ from .lora import LoRA, load_lora  # noqa: F401
 from .mmdit import MMDiT  # noqa: F401
 from .pipeline import (CFGDenoiser, DiffusionPipeline, FluxLatentFormat, FluxPipeline, LatentFormat,  # noqa: F401
                        SD3LatentFormat, sample_dpmpp_2m, sample_euler, sample_heun)
-from .sampler import FluxSampler, ModelSamplingDiscreteFlow, dpmpp_2m_coefficients  # noqa: F401
+from .sampler import FluxSampler, ModelSamplingDiscreteFlow, dpmpp_2m_coefficients, flux_resolution_shift  # noqa: F401
 from .vae import VAEDecoder, VAEEncoder  # noqa: F401
 
 __version__ = "0.1.0"

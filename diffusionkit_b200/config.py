@@ -71,6 +71,7 @@ FLUX_SCHNELL = MMDiTConfig(
 )
 
 # Defined by the reference but never used: FLUX.1-dev is loaded with FLUX_SCHNELL (mlx/model_io.py:109,756; quirk Q1).
+# Here mmdit_config=FLUX_DEV opts in to the guidance embedder (DESIGN.md §12); MODEL_CONFIGS keeps the quirk.
 FLUX_DEV = replace(FLUX_SCHNELL, guidance_embed=True)
 
 

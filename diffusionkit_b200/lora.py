@@ -79,6 +79,9 @@ def module_table(config: MMDiTConfig) -> Dict[str, Tuple[int, List[str]]]:
                  "vector_in.in_layer": "y_embedder.mlp.layers.0", "vector_in.out_layer": "y_embedder.mlp.layers.2",
                  "final_layer.linear": "final_layer.linear",
                  "final_layer.adaLN_modulation.1": "final_layer.adaLN_modulation.layers.1"}
+        if c.guidance_embed:                                         # FLUX.1-dev's guidance embedder
+            embed.update({"guidance_in.in_layer": "guidance_in.mlp.layers.0",
+                          "guidance_in.out_layer": "guidance_in.mlp.layers.2"})
     else:                                                            # Stability SD3 / SD3.5 layout
         for i in range(c.depth_multimodal):
             skip_text = i == c.depth_multimodal - 1                  # the last context block has no post-attention
@@ -101,7 +104,8 @@ def module_table(config: MMDiTConfig) -> Dict[str, Tuple[int, List[str]]]:
 
 
 def _is_skipped(module: str) -> bool:
-    return module.startswith(("guidance_in.", "guidance_in_"))      # FLUX.1-dev's guidance embedder (quirk Q1)
+    # FLUX.1-dev's guidance embedder on a model without one (quirk Q1); with one, module_table lists it
+    return module.startswith(("guidance_in.", "guidance_in_"))
 
 
 def _split_key(key: str, kohya: Dict[str, str], table) -> Tuple[str, str]:
@@ -149,8 +153,8 @@ def load_lora(path_or_state_dict: Union[str, os.PathLike, Dict[str, Tensor]], co
     """Parse a kohya or PEFT LoRA (.safetensors path or state dict) for the model `config` describes.
 
     Raises ValueError for LyCORIS / DoRA keys, incomplete modules and shapes that do not match the model, and KeyError
-    naming the first key that matches no module of the model.  Text-encoder and guidance-embedder keys are skipped and
-    listed in `LoRA.skipped`."""
+    naming the first key that matches no module of the model.  Text-encoder keys, and guidance-embedder keys when the
+    config has no guidance embedder (`guidance_embed`), are skipped and listed in `LoRA.skipped`."""
     if isinstance(path_or_state_dict, (str, os.PathLike)):
         path = os.fspath(path_or_state_dict)
         sd = model_io.load_safetensors(path)

@@ -20,6 +20,8 @@ H100 layout decisions (vs. the reference's per-module MLX graph):
     their inputs are quantised per token by the LayerNorm-modulate kernel or by a row quantiser.
   * opt-in first-block step cache (`set_step_cache`, DESIGN.md §10): a forward whose first-block residual
     barely changed since the last full one skips the other blocks and reuses their residual.
+  * FLUX.1-dev's guidance embedder (`config.guidance_embed`, DESIGN.md §12) joins the conditioning vector inside
+    cache_modulation_params; the per-step forward does not change.
 """
 from __future__ import annotations
 
@@ -66,6 +68,9 @@ class MMDiT:
     def __init__(self, config: MMDiTConfig, params: Dict[str, torch.Tensor], device=None):
         self.config = config
         c = config
+        if c.guidance_embed and c.depth_unified == 0:
+            raise ValueError("MMDiT: guidance_embed (FLUX.1-dev's guidance embedder) needs a FLUX-shaped config "
+                             "(depth_unified > 0)")
         any_p = next(iter(params.values()))
         self.device = torch.device(device) if device is not None else any_p.device
         if self.device.type != "cuda":
@@ -117,6 +122,10 @@ class MMDiT:
         self.y2 = (get("y_embedder.mlp.layers.2.weight"), get("y_embedder.mlp.layers.2.bias"))
         self.t0 = (get("t_embedder.mlp.layers.0.weight"), get("t_embedder.mlp.layers.0.bias"))
         self.t2 = (get("t_embedder.mlp.layers.2.weight"), get("t_embedder.mlp.layers.2.bias"))
+        self.g0 = self.g2 = None
+        if c.guidance_embed:
+            self.g0 = (get("guidance_in.mlp.layers.0.weight"), get("guidance_in.mlp.layers.0.bias"))
+            self.g2 = (get("guidance_in.mlp.layers.2.weight"), get("guidance_in.mlp.layers.2.bias"))
         self.w_ctx, self.b_ctx = get("context_embedder.weight"), get("context_embedder.bias")
         self.w_final, self.b_final = get("final_layer.linear.weight"), get("final_layer.linear.bias")
 
@@ -185,16 +194,55 @@ class MMDiT:
         args = (t.reshape(-1, 1).float().to(cd).float() * freqs.float()[None]).to(cd)
         return torch.cat([torch.cos(args.float()).to(cd), torch.sin(args.float()).to(cd)], dim=-1)
 
-    def cache_modulation_params(self, pooled_text_embeddings: torch.Tensor, timesteps):
+    def guidance_embedding(self, guidance) -> torch.Tensor:
+        """FLUX.1-dev's guidance sinusoid, as BFL's timestep_embedding computes it for the checkpoint: v = round(1000 ·
+        round(g)) in the activation dtype, fp32 angles v · f_k with f_k = exp(-ln(max_period) · k / half), cos first,
+        the result rounded to the activation dtype.  Unlike the timestep's (quirk Q5), the angles are not rounded:
+        the reference has no working guidance path to follow.  (B,) floats -> (B, frequency_embed_dim).  Tiny host
+        math."""
+        c, ad = self.config, self.dtype
+        half = c.frequency_embed_dim // 2
+        v = (torch.tensor(guidance, dtype=torch.float32).reshape(-1).to(ad).float() * 1000.0).to(ad).float()
+        freqs = torch.exp(-math.log(c.max_period) * torch.arange(0, half, dtype=torch.float32) / half)
+        args = v[:, None] * freqs[None]
+        return torch.cat([torch.cos(args), torch.sin(args)], dim=-1).to(ad)
+
+    def _check_guidance(self, guidance, B: int) -> Optional[List[float]]:
+        """guidance as cache_modulation_params takes it -> one float per conditioning row (None without the embedder)"""
+        if not self.config.guidance_embed:
+            if guidance is not None:
+                raise ValueError("guidance is FLUX.1-dev's distilled guidance: this model has no guidance embedder "
+                                 "(MMDiTConfig.guidance_embed is False)")
+            return None
+        if guidance is None:
+            raise ValueError("this model has a guidance embedder (FLUX.1-dev): pass one guidance value per "
+                             "conditioning row")
+        vals = [float(g) for g in (guidance.tolist() if hasattr(guidance, "tolist") else guidance)]
+        if len(vals) != B:
+            raise ValueError(f"guidance has {len(vals)} values for {B} conditioning rows")
+        if not all(math.isfinite(g) for g in vals):
+            raise ValueError(f"guidance must be finite, got {vals}")
+        return vals
+
+    def cache_modulation_params(self, pooled_text_embeddings: torch.Tensor, timesteps, guidance=None):
         """All adaLN modulation vectors for every timestep and every block in one batched GEMM
         (reference mmdit.py:77-180).  pooled: (B, P); timesteps: iterable of floats already rounded to the activation
-        dtype by the caller (mlx/__init__.py:769-771)."""
-        pooled = pooled_text_embeddings.reshape(pooled_text_embeddings.shape[0], -1)
+        dtype by the caller (mlx/__init__.py:769-771).  guidance: one float per row of pooled, required with a guidance
+        embedder (FLUX.1-dev) and refused without one; its embedding joins the pooled-text one, once per row, ahead of
+        the SiLU that feeds the modulation GEMM."""
+        B = pooled_text_embeddings.shape[0]
+        gvals = self._check_guidance(guidance, B)
+        pooled = pooled_text_embeddings.reshape(B, -1)
         pooled = pooled.to(device=self.device, dtype=self.dtype).contiguous()
-        B = pooled.shape[0]
         ts = [float(t) for t in (timesteps.tolist() if hasattr(timesteps, "tolist") else timesteps)]
         n_t = len(ts)
-        y = ops.gemm(ops.gemm(pooled, self.y0[0], bias=self.y0[1], act=ACT_SILU), self.y2[0], bias=self.y2[1])
+        gvec = None
+        if gvals is not None:
+            gemb = self.guidance_embedding(gvals).to(device=self.device)
+            gvec = ops.gemm(ops.gemm(gemb, self.g0[0], bias=self.g0[1], act=ACT_SILU), self.g2[0], bias=self.g2[1])
+        # y = y_embedder(pooled) (+ guidance_in(g) through the epilogue's residual: one rounding of the sum)
+        y = ops.gemm(ops.gemm(pooled, self.y0[0], bias=self.y0[1], act=ACT_SILU), self.y2[0], bias=self.y2[1],
+                     res=gvec)
         temb = self.timestep_embedding(torch.tensor(ts, dtype=torch.float32)).to(device=self.device, dtype=self.dtype)
         tvec = ops.gemm(ops.gemm(temb.contiguous(), self.t0[0], bias=self.t0[1], act=ACT_SILU), self.t2[0],
                         bias=self.t2[1])
@@ -306,6 +354,9 @@ class MMDiT:
         for emb in ("y", "t"):
             put(f"{emb}_embedder.mlp.layers.0", self, emb + "0", 0)
             put(f"{emb}_embedder.mlp.layers.2", self, emb + "2", 0)
+        if self.g0 is not None:
+            put("guidance_in.mlp.layers.0", self, "g0", 0)
+            put("guidance_in.mlp.layers.2", self, "g2", 0)
         put("final_layer.linear", self, "w_final")
         put("final_layer.adaLN_modulation.layers.1", self, "w_mod",
             rows=slice(self.final_mod_off, self.final_mod_off + 2 * h))
@@ -347,8 +398,8 @@ class MMDiT:
         so captured CUDA graphs stay valid when only scales change; tensors the stack no longer touches go back to
         their base and their live copy is freed (an empty stack frees them all).  Binding a live copy or a base drops
         the captured graphs.  With FP8 on, the e4m3 copy of every weight whose 16-bit tensor changed is re-quantised in
-        place, so it keeps its address too.  A merge that changes the adaLN or t / y embedder weights clears the modulation cache:
-        call cache_modulation_params again before the next forward."""
+        place, so it keeps its address too.  A merge that changes the adaLN or t / y / guidance embedder weights clears
+        the modulation cache: call cache_modulation_params again before the next forward."""
         slots = self.lora_weight_slots()
         terms: Dict[str, list] = {}
         for lora, scale in stack:
@@ -364,11 +415,12 @@ class MMDiT:
             owner, attr, idx = slots[name][:3]
             touched[(id(owner), attr, idx)] = (owner, attr, idx)
         rebound, mod_changed = False, False
+        mod_attrs = ("w_mod", "y0", "y2", "t0", "t2", "g0", "g2")        # what the modulation cache was built from
         changed = set(touched) | set(self._lora_live)
         for key in [k for k in self._lora_live if k not in touched]:
             owner, base, _ = self._lora_live.pop(key)
             self._rebind(owner, key[1], key[2], base)
-            rebound, mod_changed = True, mod_changed or key[1] in ("w_mod", "y0", "y2", "t0", "t2")
+            rebound, mod_changed = True, mod_changed or key[1] in mod_attrs
         for key, (owner, attr, idx) in touched.items():
             if key not in self._lora_live:
                 base = self._bound(owner, attr, idx)
@@ -377,7 +429,7 @@ class MMDiT:
                 rebound = True
             _, base, live = self._lora_live[key]
             live.copy_(base)
-            mod_changed = mod_changed or attr in ("w_mod", "y0", "y2", "t0", "t2")
+            mod_changed = mod_changed or attr in mod_attrs
         for name, ts in terms.items():
             owner, attr, idx, rows, cols = slots[name]
             _, base, live = self._lora_live[(id(owner), attr, idx)]

@@ -33,7 +33,12 @@ def _conv_oihw_to_ohwi(w: Tensor) -> Tensor:
 _FLUX_STREAM = {"img": "image_transformer_block", "txt": "text_transformer_block"}
 
 
-def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, mlp_ratio: int = 4) -> Dict[str, Tensor]:
+_FLUX_GUIDANCE_KEYS = {f"guidance_in.{layer}.{leaf}": f"guidance_in.mlp.layers.{idx}.{leaf}"
+                       for layer, idx in (("in_layer", 0), ("out_layer", 2)) for leaf in ("weight", "bias")}
+
+
+def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, mlp_ratio: int = 4, *,
+                              guidance_embed: bool = False) -> Dict[str, Tensor]:
     """BFL `flux1-*.safetensors` -> MMDiT parameter tree (reference model_io.py:130-311).
 
     double_blocks.i.{img,txt}_attn.qkv        -> split 3 (rows)  -> ...{image,text}_transformer_block.attn.{q,k,v}_proj
@@ -45,7 +50,9 @@ def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, ml
     single_blocks.i.linear2.weight            -> split cols [h, r*h]       -> attn.o_proj.weight, mlp.fc2.weight
     single_blocks.i.linear2.bias              -> attn.o_proj.bias (and mlp.fc2.bias, which the forward zeroes, mmdit.py:742)
     img_in / txt_in / time_in / vector_in / final_layer.adaLN_modulation.1 -> embedders / final layer
-    The K-projection bias is dropped (quirk Q3) and guidance_in.* is ignored (quirk Q1).
+    guidance_in.{in,out}_layer                -> guidance_in.mlp.layers.{0,2}  (guidance_embed only)
+    The K-projection bias is dropped (quirk Q3).  Without `guidance_embed` guidance_in.* is ignored, as the reference
+    does (quirk Q1); with it, FLUX.1-dev's guidance embedder is loaded and must be present.
     """
     h = hidden_size
     out: Dict[str, Tensor] = {}
@@ -117,9 +124,17 @@ def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, ml
         elif key.startswith("final_layer.linear."):
             out[key] = v
         elif key.startswith("guidance_in."):
-            continue  # quirk Q1: the reference ignores the guidance embedder (model_io.py:756,783)
+            if not guidance_embed:
+                continue  # quirk Q1: the reference ignores the guidance embedder (model_io.py:756,783)
+            if key not in _FLUX_GUIDANCE_KEYS:
+                raise KeyError(f"unrecognised FLUX key {key}")
+            out[_FLUX_GUIDANCE_KEYS[key]] = v
         else:
             raise KeyError(f"unrecognised FLUX key {key}")
+    if guidance_embed:
+        missing = sorted(k for k in _FLUX_GUIDANCE_KEYS if k not in sd)
+        if missing:
+            raise ValueError(f"the config has a guidance embedder (FLUX.1-dev) but the checkpoint lacks {missing}")
     return out
 
 

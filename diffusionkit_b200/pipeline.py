@@ -13,6 +13,8 @@ Differences that are deliberate (documented in DESIGN.md):
   * img2img (`image_path`, `denoise`): the VAE encoder is built on first use.
   * batch-N extension: `seed` may be a list of ints — one independent image per seed (the reference is batch 1);
     a scalar seed behaves exactly like the reference.
+  * FLUX.1-dev's distilled guidance (`guidance=` of FluxPipeline.generate_image / denoise_latents) when the pipeline is
+    built with mmdit_config=FLUX_DEV; the reference loads dev without its guidance embedder (quirk Q1).
 """
 from __future__ import annotations
 
@@ -39,6 +41,9 @@ MMDIT_CKPT = {  # reference mlx/__init__.py:37-44
     "argmaxinc/mlx-FLUX.1-schnell-4bit-quantized": "argmaxinc/mlx-FLUX.1-schnell-4bit-quantized",
     "argmaxinc/mlx-FLUX.1-dev": "argmaxinc/mlx-FLUX.1-dev",
 }
+
+# FLUX.1-dev's guidance when the caller passes none (BFL's default for the dev checkpoint)
+DEFAULT_GUIDANCE = 3.5
 
 
 class LatentFormat:
@@ -81,8 +86,9 @@ class CFGDenoiser:
     def __init__(self, model: "DiffusionPipeline"):
         self.model = model
 
-    def cache_modulation_params(self, pooled_text_embeddings, sigmas):
-        self.model.mmdit.cache_modulation_params(pooled_text_embeddings, sigmas)
+    def cache_modulation_params(self, pooled_text_embeddings, sigmas, guidance=None):
+        """guidance: one FLUX.1-dev guidance value per row of pooled (None without a guidance embedder)"""
+        self.model.mmdit.cache_modulation_params(pooled_text_embeddings, sigmas, guidance)
 
     def clear_cache(self):
         # the reference re-reads the adaLN weights it dropped (:686-689); nothing was dropped here
@@ -99,7 +105,8 @@ class CFGDenoiser:
 
 
 def _start_sampling(model: CFGDenoiser, sigmas, extra_args):
-    """What every sampler does first: the timesteps of the schedule into the modulation cache.
+    """What every sampler does first: the timesteps of the schedule (and, for FLUX.1-dev, the per-row guidance values
+    extra_args["guidance"]) into the modulation cache.
     -> (sigmas fp32, timesteps, conditioning, cfg_weight, events (one per sigma, the first recorded))"""
     extra_args = {} if extra_args is None else dict(extra_args)
     pipe = model.model
@@ -108,7 +115,7 @@ def _start_sampling(model: CFGDenoiser, sigmas, extra_args):
     timesteps = torch.from_numpy(np.asarray(pipe.sampler.timestep(sig), dtype=np.float32)).to(
         pipe.activation_dtype).to(torch.float32).tolist()
     pooled = extra_args.pop("pooled_conditioning")
-    model.cache_modulation_params(pooled, timesteps)
+    model.cache_modulation_params(pooled, timesteps, extra_args.pop("guidance", None))
     cfg_weight = float(extra_args.get("cfg_weight", 0.0))
     conditioning = extra_args["conditioning"]
     events = [torch.cuda.Event(enable_timing=True) for _ in range(len(sig))]
@@ -262,7 +269,8 @@ class DiffusionPipeline:
                         if sub:
                             out[part] = sub
             elif isinstance(self, FluxPipeline):
-                params = model_io.flux_checkpoint_to_params(sd, self.config.hidden_size, self.config.mlp_ratio)
+                params = model_io.flux_checkpoint_to_params(sd, self.config.hidden_size, self.config.mlp_ratio,
+                                                            guidance_embed=self.config.guidance_embed)
             else:
                 params = model_io.sd3_checkpoint_to_params(sd)
                 if "vae" not in paths and any("decoder." in k for k in sd):
@@ -500,6 +508,32 @@ class DiffusionPipeline:
         `image_path` (img2img): a file path, a PIL image or a uint8 HWC array; the latent size then follows the image
         (the reference ignores latent_size in that case too, :273).  `solver`: "euler" (the reference's sampler),
         "heun" (two model evaluations per step but the last) or "dpmpp_2m" (one per step), DESIGN.md §11."""
+        return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
+                                     image_path, denoise, noise=noise, solver=solver, guidance=None)
+
+    def _guidance_values(self, guidance, n_images: int) -> Optional[List[float]]:
+        """FluxPipeline's `guidance` -> one FLUX.1-dev guidance value per image, or None for a model without a
+        guidance embedder.  Raises ValueError, before any GPU work, for a value the model cannot take."""
+        if not self.config.guidance_embed:
+            if guidance is not None:
+                raise ValueError("guidance is FLUX.1-dev's distilled guidance, and this model has no guidance embedder:"
+                                 " build the pipeline with mmdit_config=FLUX_DEV (or guidance_embed=True)")
+            return None
+        if guidance is None:
+            guidance = DEFAULT_GUIDANCE
+        if np.ndim(guidance) == 0:
+            vals = [float(guidance)] * n_images
+        else:
+            vals = [float(g) for g in guidance]
+            if len(vals) != n_images:
+                raise ValueError(f"guidance has {len(vals)} values for {n_images} image(s): pass one float, or one "
+                                 "per seed")
+        if not all(math.isfinite(g) for g in vals):
+            raise ValueError(f"guidance must be finite, got {vals}")
+        return vals
+
+    def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
+                         denoise, *, noise, solver, guidance):
         _check_solver(solver)
         if image_path is None:
             denoise = 1.0                                                   # :270-271
@@ -513,6 +547,7 @@ class DiffusionPipeline:
         else:
             seeds = [int(seed)]
         B = len(seeds)
+        guidance = self._guidance_values(guidance, B)
         H, W = latent_size
         conditioning = torch.as_tensor(conditioning).to(device=self.device, dtype=self.activation_dtype)
         pooled_conditioning = torch.as_tensor(pooled_conditioning).to(device=self.device, dtype=self.activation_dtype)
@@ -556,6 +591,9 @@ class DiffusionPipeline:
             x = ops.axpby(noise, x_T, s0, 1.0 - s0)
         extra_args = {"conditioning": conditioning, "cfg_weight": cfg_weight,
                       "pooled_conditioning": pooled_conditioning}
+        if guidance is not None:
+            # rows [positive x B | negative x B]: both rows of an image get its value
+            extra_args["guidance"] = guidance * reps
         latent, iter_time = SOLVERS[solver](CFGDenoiser(self), x, sigmas, extra_args=extra_args)
         latent = ops.axpb(latent, 1.0 / self.latent_format.scale_factor, self.latent_format.shift_factor)  # process_out
         return latent, iter_time
@@ -577,7 +615,14 @@ class DiffusionPipeline:
         pooled_conditioning=None,
         solver: str = "euler",
     ):
+        return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
+                                    denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
+                                    solver=solver, guidance=None)
+
+    def _generate_image(self, text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
+                        denoise, *, conditioning, pooled_conditioning, solver, guidance):
         _check_solver(solver)
+        guidance = self._guidance_values(guidance, len(seed) if isinstance(seed, (list, tuple)) else 1)
         assert latent_size[0] % 2 == 0, f"Height must be divisible by 16 ({latent_size[0]*8}/16={latent_size[0]/2})"
         assert latent_size[1] % 2 == 0, f"Width must be divisible by 16 ({latent_size[1]*8}/16={latent_size[1]/2})"
         self.check_and_load_models()
@@ -605,9 +650,9 @@ class DiffusionPipeline:
         torch.cuda.reset_peak_memory_stats(self.device)
         t0 = time.time()
         log["denoising"]["pre"] = mem()
-        latents, iter_time = self.denoise_latents(conditioning, pooled_conditioning, num_steps=num_steps,
-                                                  cfg_weight=cfg_weight, latent_size=latent_size, seed=seed,
-                                                  image_path=image_path, denoise=denoise, solver=solver)
+        latents, iter_time = self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight,
+                                                   latent_size, seed, image_path, denoise, noise=None, solver=solver,
+                                                   guidance=guidance)
         torch.cuda.synchronize(self.device)
         log["denoising"]["post"] = mem()
         log["denoising"]["time"] = round(time.time() - t0, 3)
@@ -617,6 +662,8 @@ class DiffusionPipeline:
             n = len(iter_time)
             log["denoising"]["solver"] = solver
             log["denoising"]["nfe"] = max(2 * n - 1, 0) if solver == "heun" else n
+        if guidance is not None:
+            log["denoising"]["guidance"] = guidance
         if self.mmdit.step_cache is not None:
             log["denoising"]["step_cache"] = [{"rel": rel, "skipped": skipped}
                                               for rel, skipped in self.mmdit.step_cache_log]
@@ -768,6 +815,26 @@ class FluxPipeline(DiffusionPipeline):
         self.use_t5 = True
         self.use_clip_g = False
         self.quantize_mmdit = quantize_mmdit
+
+    def denoise_latents(self, conditioning, pooled_conditioning, num_steps: int = 2, cfg_weight: float = 0.0,
+                        latent_size: Tuple[int, int] = (64, 64), seed=None, image_path: Optional[str] = None,
+                        denoise: float = 1.0, *, noise: Optional[torch.Tensor] = None, solver: str = "euler",
+                        guidance=None):
+        """DiffusionPipeline.denoise_latents, plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
+        float for every image or one per seed, and None means DEFAULT_GUIDANCE (3.5) when the model has a guidance
+        embedder (mmdit_config=FLUX_DEV).  A model without one refuses any value but None."""
+        return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
+                                     image_path, denoise, noise=noise, solver=solver, guidance=guidance)
+
+    def generate_image(self, text: str, num_steps: int = 2, cfg_weight: float = 0.0, negative_text: str = "",
+                       latent_size: Tuple[int, int] = (64, 64), seed=None, verbose: bool = True,
+                       image_path: Optional[str] = None, denoise: float = 1.0, *, conditioning=None,
+                       pooled_conditioning=None, solver: str = "euler", guidance=None):
+        """DiffusionPipeline.generate_image with `guidance` as in denoise_latents; with a guidance embedder the log
+        holds the value of each image under log["denoising"]["guidance"]."""
+        return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
+                                    denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
+                                    solver=solver, guidance=guidance)
 
     def encode_text(self, text: str, cfg_weight: float = 7.5, negative_text: str = ""):
         """reference :642-671: CLIP-L pooled output + T5 sequence of the POSITIVE prompt only, T5 padded with zeros to

@@ -4,6 +4,8 @@ Host-side scalar arithmetic (numpy fp32, like the reference's fp32 mx arrays); t
 fused CUDA sampler kernels (csrc/elementwise.cu: dk_sampler_prepare / dk_sampler_step, and the Heun and
 DPM-Solver++(2M) updates, whose fp64 coefficients dpmpp_2m_coefficients computes).
 """
+import math
+
 import numpy as np
 
 
@@ -47,6 +49,19 @@ class FluxSampler(ModelSamplingDiscreteFlow):
     """Helper for sampler scheduling for Flux models (sampler.py:45-77): table over t = 0..1000."""
 
     _t_first = 0
+
+
+def flux_resolution_shift(latent_size, base_shift: float = 0.5, max_shift: float = 1.15) -> float:
+    """exp(mu) of BFL's resolution-dependent FLUX.1-dev schedule, for FluxSampler(shift=...) / FluxPipeline(shift=...).
+    mu is linear in the image token count n = (H/2)·(W/2) of the latent (H, W): base_shift at 256 tokens, max_shift at
+    4096.  BFL applies time_shift(mu, 1, t) = e^mu / (e^mu + 1/t - 1) to t on linspace(1, 0, steps + 1); FluxSampler
+    with shift = e^mu gives the same sigmas.  1024^2 (latent 128^2): 3.1582."""
+    H, W = (int(s) for s in latent_size)
+    if H < 2 or W < 2:
+        raise ValueError(f"latent_size must be at least (2, 2), got {tuple(latent_size)}")
+    n = (H // 2) * (W // 2)
+    mu = base_shift + (max_shift - base_shift) * (n - 256) / (4096 - 256)
+    return math.exp(mu)
 
 
 def dpmpp_2m_coefficients(sigmas) -> np.ndarray:

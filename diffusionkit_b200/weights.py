@@ -63,6 +63,11 @@ def mmdit_param_specs(cfg: MMDiTConfig) -> List[Spec]:
         block(f"unified_transformer_blocks.{i}.transformer_block", 3 if cfg.parallel_mlp_for_unified_blocks else 6)
     lin("final_layer.linear", p * p * cfg.vae_latent_dim, h)
     lin("final_layer.adaLN_modulation.layers.1", 2 * h, h)
+    if cfg.guidance_embed:
+        # FLUX.1-dev's guidance MLPEmbedder (reference mlx/mmdit.py:31-34, 945-955).  Last, so that init_params (seeded
+        # by spec index) gives every other tensor the values it has without the embedder.
+        lin("guidance_in.mlp.layers.0", h, cfg.frequency_embed_dim)
+        lin("guidance_in.mlp.layers.2", h, h)
     return specs
 
 
