@@ -8,12 +8,14 @@ DiffusionPipeline / FluxPipeline API (reference: argmaxinc/DiffusionKit, python/
                                      conditioning=cond, pooled_conditioning=pooled)
 """
 from ._lib import DkError  # noqa: F401
-from .config import FLUX_DEV, FLUX_SCHNELL, SD3_2b, SD3_8b, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig  # noqa: F401
+from .config import (FLUX_DEV, FLUX_SCHNELL, SD3_2b, SD3_8b, SD35_MEDIUM, MMDiTConfig, VAEDecoderConfig,  # noqa: F401
+                     VAEEncoderConfig)
 from .lora import LoRA, load_lora  # noqa: F401
 from .mmdit import MMDiT  # noqa: F401
 from .pipeline import (CFGDenoiser, DiffusionPipeline, FluxLatentFormat, FluxPipeline, LatentFormat,  # noqa: F401
                        SD3LatentFormat, sample_dpmpp_2m, sample_euler, sample_heun)
-from .sampler import FluxSampler, ModelSamplingDiscreteFlow, dpmpp_2m_coefficients, flux_resolution_shift  # noqa: F401
+from .sampler import (FluxSampler, ModelSamplingDiscreteFlow, SkipLayerGuidance, dpmpp_2m_coefficients,  # noqa: F401
+                      flux_resolution_shift)
 from .vae import VAEDecoder, VAEEncoder  # noqa: F401
 
 __version__ = "0.1.0"

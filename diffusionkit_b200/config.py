@@ -45,6 +45,12 @@ class MMDiTConfig:
     float16_dtype: torch.dtype = torch.bfloat16
     low_memory_mode: bool = True
     guidance_embed: bool = False
+    # MMDiT-X (SD3.5 Medium): the joint blocks whose image stream has a second self-attention, attn2, over the image
+    # tokens only, with its own adaLN shift, scale and gate (Stability's field name)
+    x_block_self_attn_layers: Tuple[int, ...] = ()
+    # keep the k bias of the q/k/v projections; False drops it (quirk Q3), which SD3.5 Medium cannot: with QK-RMSNorm
+    # the bias enters before the norm and changes the output
+    attn_k_bias: bool = False
 
     @property
     def head_dim(self) -> int:
@@ -69,6 +75,11 @@ FLUX_SCHNELL = MMDiTConfig(
     float16_dtype=torch.bfloat16,
     dtype=torch.bfloat16,
 )
+
+# Stability's SD3.5 Medium: SD3-medium's width and depth with QK-RMSNorm, a 384^2 position table, attn2 in joint
+# blocks 0-12 (MMDiT-X) and the k bias kept (DESIGN.md §13)
+SD35_MEDIUM = replace(SD3_2b, use_qk_norm=True, max_latent_resolution=384, x_block_self_attn_layers=tuple(range(13)),
+                      attn_k_bias=True)
 
 # Defined by the reference but never used: FLUX.1-dev is loaded with FLUX_SCHNELL (mlx/model_io.py:109,756; quirk Q1).
 # Here mmdit_config=FLUX_DEV opts in to the guidance embedder (DESIGN.md §12); MODEL_CONFIGS keeps the quirk.
@@ -105,6 +116,7 @@ MODEL_CONFIGS = {
     "argmaxinc/mlx-FLUX.1-dev": FLUX_SCHNELL,  # quirk Q1
     "argmaxinc/mlx-stable-diffusion-3.5-large": SD3_8b,
     "argmaxinc/mlx-stable-diffusion-3.5-large-4bit-quantized": SD3_8b,
+    "stabilityai/stable-diffusion-3.5-medium": SD35_MEDIUM,
 }
 
 # T5 sequence lengths (mlx/__init__.py:46-53)
@@ -115,6 +127,7 @@ T5_MAX_LENGTH = {
     "argmaxinc/mlx-FLUX.1-schnell": 256,
     "argmaxinc/mlx-FLUX.1-schnell-4bit-quantized": 256,
     "argmaxinc/mlx-FLUX.1-dev": 512,
+    "stabilityai/stable-diffusion-3.5-medium": 512,
 }
 
 
@@ -124,6 +137,11 @@ def tiny_sd35_config(hidden: int = 128, heads: int = 2, depth: int = 2) -> MMDiT
     return MMDiTConfig(num_heads=heads, depth_multimodal=depth, hidden_size_override=hidden, use_qk_norm=True,
                        upcast_multimodal_blocks=[depth - 1], max_latent_resolution=24, pooled_text_embed_dim=64,
                        token_level_text_embed_dim=128)
+
+
+def tiny_sd35_medium_config() -> MMDiTConfig:
+    """Small SD3.5-Medium-shaped config for tests: MMDiT-X blocks 0 and 1 of 3, QK-RMSNorm, k bias, fp16."""
+    return replace(tiny_sd3_config(), use_qk_norm=True, x_block_self_attn_layers=(0, 1), attn_k_bias=True)
 
 
 def tiny_flux_config(hidden: int = 256, heads: int = 2, depth_mm: int = 2, depth_uni: int = 2) -> MMDiTConfig:

@@ -403,24 +403,31 @@ __global__ void sampler_prepare_kernel(const float* __restrict__ x, T* __restric
   }
 }
 // The CFG-mixed denoised estimate D of element i, shared by every sampler update.  The negative rows sit n elements
-// after the positive ones ([positive x B | negative x B], reference :718).
-template <typename T>
+// after the positive ones ([positive x B | negative x B], reference :718).  SLG (skip-layer guidance, DESIGN.md §13):
+// a third block of rows at 2n holds the positive rows' forward with joint blocks skipped, and
+// D = D_neg + w (D_pos - D_neg) + slg (D_pos - D_skip).  The entry points refuse SLG without CFG.
+template <bool SLG, typename T>
 __device__ __forceinline__ float cfg_denoised(const T* __restrict__ xin, const T* __restrict__ out, long long n,
-                                              long long i, float sigma, float cfg) {
+                                              long long i, float sigma, float cfg, float slg) {
   // calculate_denoised: model_input - model_output * sigma (fp32 sigma promotes to fp32)
   float den = Half16<T>::to_f(xin[i]) - Half16<T>::to_f(out[i]) * sigma;
   if (cfg > 0.f) {
+    const float den_pos = den;
     const float den_neg = Half16<T>::to_f(xin[n + i]) - Half16<T>::to_f(out[n + i]) * sigma;
-    den = den_neg + cfg * (den - den_neg);
+    den = den_neg + cfg * (den_pos - den_neg);
+    if constexpr (SLG) {
+      const float den_skip = Half16<T>::to_f(xin[2 * n + i]) - Half16<T>::to_f(out[2 * n + i]) * sigma;
+      den += slg * (den_pos - den_skip);
+    }
   }
   return den;
 }
-template <typename T>
+template <typename T, bool SLG>
 __global__ void sampler_step_kernel(float* __restrict__ x, const T* __restrict__ xin, const T* __restrict__ out,
-                                    long long n, float sigma, float sigma_next, float cfg) {
+                                    long long n, float sigma, float sigma_next, float cfg, float slg) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float den = cfg_denoised(xin, out, n, i, sigma, cfg);
+    const float den = cfg_denoised<SLG>(xin, out, n, i, sigma, cfg, slg);
     const float xv = x[i];
     const float d = (xv - den) / sigma;          // to_d
     x[i] = xv + d * (sigma_next - sigma);        // Euler
@@ -428,39 +435,39 @@ __global__ void sampler_step_kernel(float* __restrict__ x, const T* __restrict__
 }
 // Heun predictor (Karras et al. 2022, Alg. 2): the Euler step to x2, keeping its slope d for the corrector; x is
 // left as it is.
-template <typename T>
+template <typename T, bool SLG>
 __global__ void sampler_heun_predict_kernel(const float* __restrict__ x, const T* __restrict__ xin,
                                             const T* __restrict__ out, float* __restrict__ d, float* __restrict__ x2,
-                                            long long n, float sigma, float sigma_next, float cfg) {
+                                            long long n, float sigma, float sigma_next, float cfg, float slg) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float xv = x[i];
-    const float dv = (xv - cfg_denoised(xin, out, n, i, sigma, cfg)) / sigma;
+    const float dv = (xv - cfg_denoised<SLG>(xin, out, n, i, sigma, cfg, slg)) / sigma;
     d[i] = dv;
     x2[i] = xv + dv * (sigma_next - sigma);
   }
 }
 // Heun corrector: xin / out are the forward at (x2, sigma_next); x moves by the mean of the two slopes.
-template <typename T>
+template <typename T, bool SLG>
 __global__ void sampler_heun_correct_kernel(float* __restrict__ x, const float* __restrict__ d,
                                             const float* __restrict__ x2, const T* __restrict__ xin,
                                             const T* __restrict__ out, long long n, float sigma, float sigma_next,
-                                            float cfg) {
+                                            float cfg, float slg) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float d2 = (x2[i] - cfg_denoised(xin, out, n, i, sigma_next, cfg)) / sigma_next;
+    const float d2 = (x2[i] - cfg_denoised<SLG>(xin, out, n, i, sigma_next, cfg, slg)) / sigma_next;
     x[i] += (d[i] + d2) * 0.5f * (sigma_next - sigma);
   }
 }
 // DPM-Solver++(2M): x <- a x + b D + c D_prev, then D_prev <- D.  d_prev is not read when c == 0: on the first step
 // it holds whatever the allocation held, and 0 * NaN is NaN.
-template <typename T>
+template <typename T, bool SLG>
 __global__ void sampler_dpmpp_2m_kernel(float* __restrict__ x, float* __restrict__ d_prev, const T* __restrict__ xin,
                                         const T* __restrict__ out, long long n, float sigma, float a, float b, float c,
-                                        float cfg) {
+                                        float cfg, float slg) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float den = cfg_denoised(xin, out, n, i, sigma, cfg);
+    const float den = cfg_denoised<SLG>(xin, out, n, i, sigma, cfg, slg);
     float v = a * x[i] + b * den;
     if (c != 0.f) v += c * d_prev[i];
     x[i] = v;
@@ -1149,8 +1156,9 @@ extern "C" int dk_sampler_step(dk_ctx* ctx, int dtype, float* x, const void* xin
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(sigma != 0.f, "dk_sampler_step: sigma must be non-zero");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (sampler_step_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
-                         x, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, sigma_next, cfg_weight)));
+  DK_DISPATCH(dtype, (sampler_step_kernel<T, false><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+                         x, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, sigma_next, cfg_weight,
+                         0.f)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
@@ -1162,9 +1170,9 @@ extern "C" int dk_sampler_heun_predict(dk_ctx* ctx, int dtype, const float* x, c
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(sigma != 0.f, "dk_sampler_heun_predict: sigma must be non-zero");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (sampler_heun_predict_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (sampler_heun_predict_kernel<T, false><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
                          x, static_cast<const T*>(xin), static_cast<const T*>(out), d, x2, n, sigma, sigma_next,
-                         cfg_weight)));
+                         cfg_weight, 0.f)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
@@ -1176,9 +1184,9 @@ extern "C" int dk_sampler_heun_correct(dk_ctx* ctx, int dtype, float* x, const f
   DK_DTYPE_OK(dtype);
   DK_REQUIRE(sigma_next != 0.f, "dk_sampler_heun_correct: sigma_next must be non-zero (the last step is an Euler step)");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (sampler_heun_correct_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (sampler_heun_correct_kernel<T, false><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
                          x, d, x2, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, sigma_next,
-                         cfg_weight)));
+                         cfg_weight, 0.f)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
@@ -1189,12 +1197,78 @@ extern "C" int dk_sampler_dpmpp_2m(dk_ctx* ctx, int dtype, float* x, float* d_pr
   DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DK_DISPATCH(dtype, (sampler_dpmpp_2m_kernel<T><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+  DK_DISPATCH(dtype, (sampler_dpmpp_2m_kernel<T, false><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
                          x, d_prev, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, a, b, c,
-                         cfg_weight)));
+                         cfg_weight, 0.f)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }
+
+// The same four updates with skip-layer guidance (DESIGN.md §13): xin / out hold three blocks of n elements,
+// [positive | negative | positive with joint blocks skipped], so they need CFG.
+#define DK_SLG_REQUIRE(cfg_weight, slg)                                                                     \
+  DK_REQUIRE((cfg_weight) > 0.f, "%s: skip-layer guidance needs CFG (cfg_weight > 0)", __func__);          \
+  DK_REQUIRE(isfinite(slg), "%s: the skip-layer guidance scale must be finite", __func__)
+
+extern "C" int dk_sampler_step_slg(dk_ctx* ctx, int dtype, float* x, const void* xin, const void* out, long long n,
+                                   float sigma, float sigma_next, float cfg_weight, float slg, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(sigma != 0.f, "dk_sampler_step_slg: sigma must be non-zero");
+  DK_SLG_REQUIRE(cfg_weight, slg);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (sampler_step_kernel<T, true><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+                         x, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, sigma_next, cfg_weight,
+                         slg)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_sampler_heun_predict_slg(dk_ctx* ctx, int dtype, const float* x, const void* xin, const void* out,
+                                           float* d, float* x2, long long n, float sigma, float sigma_next,
+                                           float cfg_weight, float slg, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(sigma != 0.f, "dk_sampler_heun_predict_slg: sigma must be non-zero");
+  DK_SLG_REQUIRE(cfg_weight, slg);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (sampler_heun_predict_kernel<T, true><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+                         x, static_cast<const T*>(xin), static_cast<const T*>(out), d, x2, n, sigma, sigma_next,
+                         cfg_weight, slg)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_sampler_heun_correct_slg(dk_ctx* ctx, int dtype, float* x, const float* d, const float* x2,
+                                           const void* xin, const void* out, long long n, float sigma,
+                                           float sigma_next, float cfg_weight, float slg, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(sigma_next != 0.f,
+             "dk_sampler_heun_correct_slg: sigma_next must be non-zero (the last step is an Euler step)");
+  DK_SLG_REQUIRE(cfg_weight, slg);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (sampler_heun_correct_kernel<T, true><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+                         x, d, x2, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, sigma_next,
+                         cfg_weight, slg)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_sampler_dpmpp_2m_slg(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin,
+                                       const void* out, long long n, float sigma, float a, float b, float c,
+                                       float cfg_weight, float slg, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_SLG_REQUIRE(cfg_weight, slg);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DK_DISPATCH(dtype, (sampler_dpmpp_2m_kernel<T, true><<<dk_grid_for(n, 256, ctx->sm_count), 256, 0, stream>>>(
+                         x, d_prev, static_cast<const T*>(xin), static_cast<const T*>(out), n, sigma, a, b, c,
+                         cfg_weight, slg)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+#undef DK_SLG_REQUIRE
 
 extern "C" int dk_axpb_f32(dk_ctx* ctx, const float* x, float* y, long long n, float a, float b, void* stream_) {
   DK_ENTRY(ctx);

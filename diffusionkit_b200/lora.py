@@ -93,6 +93,10 @@ def module_table(config: MMDiTConfig) -> Dict[str, Tuple[int, List[str]]]:
                     lin(f"{u}.mlp.fc1", b + ".mlp.fc1")
                     lin(f"{u}.mlp.fc2", b + ".mlp.fc2")
                 lin(f"{u}.adaLN_modulation.1", b + ".adaLN_modulation.layers.1")
+            if i in c.x_block_self_attn_layers:                      # SD3.5 Medium's MMDiT-X second attention
+                b, u = f"multimodal_transformer_blocks.{i}.image_transformer_block", f"joint_blocks.{i}.x_block"
+                lin(f"{u}.attn2.qkv", [f"{b}.attn2.{n}_proj" for n in "qkv"])
+                lin(f"{u}.attn2.proj", b + ".attn2.o_proj")
         embed = {"x_embedder.proj": "x_embedder.proj", "context_embedder": "context_embedder",
                  "t_embedder.mlp.0": "t_embedder.mlp.layers.0", "t_embedder.mlp.2": "t_embedder.mlp.layers.2",
                  "y_embedder.mlp.0": "y_embedder.mlp.layers.0", "y_embedder.mlp.2": "y_embedder.mlp.layers.2",

@@ -22,6 +22,9 @@ H100 layout decisions (vs. the reference's per-module MLX graph):
     barely changed since the last full one skips the other blocks and reuses their residual.
   * FLUX.1-dev's guidance embedder (`config.guidance_embed`, DESIGN.md §12) joins the conditioning vector inside
     cache_modulation_params; the per-step forward does not change.
+  * SD3.5 Medium's MMDiT-X blocks (`config.x_block_self_attn_layers`, DESIGN.md §13): the image stream's second
+    self-attention is one more packed stream (attn2) run by the same kernels, and a forward can skip listed blocks
+    for its trailing sequences (skip-layer guidance).
 """
 from __future__ import annotations
 
@@ -52,9 +55,26 @@ def fp8_covered_linears(config: MMDiTConfig) -> List[str]:
         block(f"multimodal_transformer_blocks.{i}.image_transformer_block")
         block(f"multimodal_transformer_blocks.{i}.text_transformer_block",
               skip_post=(i == c.depth_multimodal - 1) and (c.depth_unified < 1))
+    for i in sorted(c.x_block_self_attn_layers):
+        names.extend(f"multimodal_transformer_blocks.{i}.image_transformer_block.attn2.{n}_proj" for n in "qkvo")
     for i in range(c.depth_unified):
         block(f"unified_transformer_blocks.{i}.transformer_block")
     return names
+
+
+def check_x_layers(config: MMDiTConfig):
+    """Raise ValueError for MMDiT-X layers (x_block_self_attn_layers) the engine does not run: on a FLUX-shaped config,
+    out of range or listed twice, or without QK-RMSNorm (no published model has that form)."""
+    c, xl = config, tuple(config.x_block_self_attn_layers)
+    if not xl:
+        return
+    if c.depth_unified > 0:
+        raise ValueError("MMDiT: x_block_self_attn_layers (MMDiT-X) needs an SD3-shaped config (depth_unified == 0)")
+    if len(set(xl)) != len(xl) or not all(isinstance(i, int) and 0 <= i < c.depth_multimodal for i in xl):
+        raise ValueError(f"MMDiT: x_block_self_attn_layers {xl} must be distinct block indices in "
+                         f"[0, {c.depth_multimodal})")
+    if not c.use_qk_norm:
+        raise ValueError("MMDiT: x_block_self_attn_layers (MMDiT-X) needs use_qk_norm=True")
 
 
 class _Stream:
@@ -71,6 +91,7 @@ class MMDiT:
         if c.guidance_embed and c.depth_unified == 0:
             raise ValueError("MMDiT: guidance_embed (FLUX.1-dev's guidance embedder) needs a FLUX-shaped config "
                              "(depth_unified > 0)")
+        check_x_layers(c)
         any_p = next(iter(params.values()))
         self.device = torch.device(device) if device is not None else any_p.device
         if self.device.type != "cuda":
@@ -91,6 +112,7 @@ class MMDiT:
         self._mod_all: Optional[torch.Tensor] = None
         self._mod_cur: Optional[torch.Tensor] = None
         self._mod_batch = 0
+        self._mod_skip_batch = 0
         # workspace, RoPE table and cropped positional embedding live per input shape, next to the CUDA graph of the
         # (timestep-invariant) forward that bakes in their pointers
         self._shapes = ShapeCache()
@@ -140,6 +162,11 @@ class MMDiT:
             self.mod_total += w.shape[0]
             return off
 
+        def qkv_bias(attn):
+            bq, bv = get(attn + ".q_proj.bias"), get(attn + ".v_proj.bias")
+            bk = get(attn + ".k_proj.bias") if c.attn_k_bias else torch.zeros_like(bq)  # no k bias: quirk Q3
+            return torch.cat([bq, bk, bv]).contiguous()
+
         def stream(prefix, n_mod, skip_post=False, parallel=False) -> _Stream:
             s = _Stream()
             s.name, s.n_mod, s.skip_post = prefix, n_mod, skip_post
@@ -147,8 +174,7 @@ class MMDiT:
             wq, wk, wv = get(prefix + ".attn.q_proj.weight"), get(prefix + ".attn.k_proj.weight"), get(
                 prefix + ".attn.v_proj.weight")
             s.w_qkv = torch.cat([wq, wk, wv], dim=0).contiguous()
-            bq, bv = get(prefix + ".attn.q_proj.bias"), get(prefix + ".attn.v_proj.bias")
-            s.b_qkv = torch.cat([bq, torch.zeros_like(bq), bv]).contiguous()          # no k bias (quirk Q3)
+            s.b_qkv = qkv_bias(prefix + ".attn")
             s.w_o = s.b_o = s.w_fc1 = s.b_fc1 = s.w_fc2 = s.b_fc2 = s.w_out = None
             if not skip_post:
                 s.b_o = get(prefix + ".attn.o_proj.bias")
@@ -166,13 +192,30 @@ class MMDiT:
                 s.k_norm = get(prefix + ".qk_norm.k_norm.weight")
             return s
 
+        def attn2(img: _Stream) -> _Stream:
+            """MMDiT-X: the image stream's second self-attention; its shift, scale and gate are modulation chunks 6-8
+            of the image stream"""
+            p, s = img.name + ".attn2", _Stream()
+            s.name, s.n_mod, s.skip_post, s.mod_off = p, 3, False, img.mod_off + 6 * h
+            s.w_qkv = torch.cat([get(f"{p}.{n}_proj.weight") for n in "qkv"], dim=0).contiguous()
+            s.b_qkv = qkv_bias(p)
+            s.w_o, s.b_o = get(p + ".o_proj.weight"), get(p + ".o_proj.bias")
+            s.w_fc1 = s.b_fc1 = s.w_fc2 = s.b_fc2 = s.w_out = None
+            s.q_norm = get(img.name + ".qk_norm2.q_norm.weight")
+            s.k_norm = get(img.name + ".qk_norm2.k_norm.weight")
+            return s
+
         self.double: List[Tuple[_Stream, _Stream]] = []
+        self.attn2: Dict[int, _Stream] = {}                                           # block index -> attn2
         for i in range(c.depth_multimodal):
             skip_text = (i == c.depth_multimodal - 1) and (c.depth_unified < 1)       # mmdit.py:62-66
-            img = stream(f"multimodal_transformer_blocks.{i}.image_transformer_block", 6)
+            x_block = i in c.x_block_self_attn_layers
+            img = stream(f"multimodal_transformer_blocks.{i}.image_transformer_block", 9 if x_block else 6)
             txt = stream(f"multimodal_transformer_blocks.{i}.text_transformer_block", 2 if skip_text else 6,
                          skip_post=skip_text)
             self.double.append((img, txt))
+            if x_block:
+                self.attn2[i] = attn2(img)
         self.single: List[_Stream] = []
         par = c.parallel_mlp_for_unified_blocks
         if c.depth_unified > 0 and not par:
@@ -224,13 +267,17 @@ class MMDiT:
             raise ValueError(f"guidance must be finite, got {vals}")
         return vals
 
-    def cache_modulation_params(self, pooled_text_embeddings: torch.Tensor, timesteps, guidance=None):
+    def cache_modulation_params(self, pooled_text_embeddings: torch.Tensor, timesteps, guidance=None, *,
+                                skip_batch: int = 0):
         """All adaLN modulation vectors for every timestep and every block in one batched GEMM
         (reference mmdit.py:77-180).  pooled: (B, P); timesteps: iterable of floats already rounded to the activation
         dtype by the caller (mlx/__init__.py:769-771).  guidance: one float per row of pooled, required with a guidance
         embedder (FLUX.1-dev) and refused without one; its embedding joins the pooled-text one, once per row, ahead of
-        the SiLU that feeds the modulation GEMM."""
+        the SiLU that feeds the modulation GEMM.  skip_batch: the last skip_batch rows condition only the skip-layer
+        forwards of skip-layer guidance; a forward of the leading B - skip_batch rows alone is accepted too."""
         B = pooled_text_embeddings.shape[0]
+        if not 0 <= int(skip_batch) < B:
+            raise ValueError(f"skip_batch must be in [0, {B}), got {skip_batch}")
         gvals = self._check_guidance(guidance, B)
         pooled = pooled_text_embeddings.reshape(B, -1)
         pooled = pooled.to(device=self.device, dtype=self.dtype).contiguous()
@@ -253,6 +300,7 @@ class MMDiT:
             self._mod_cur = torch.empty((B, self.mod_total), dtype=self.dtype, device=self.device)
             self._shapes.drop_graphs()
         self._mod_batch = B
+        self._mod_skip_batch = int(skip_batch)
         self._mod_index = {}
         self._reset_step_cache()
         for i, t in enumerate(ts):
@@ -360,6 +408,10 @@ class MMDiT:
         put("final_layer.linear", self, "w_final")
         put("final_layer.adaLN_modulation.layers.1", self, "w_mod",
             rows=slice(self.final_mod_off, self.final_mod_off + 2 * h))
+        for s in self.attn2.values():
+            for j, n in enumerate("qkv"):
+                put(f"{s.name}.{n}_proj", s, "w_qkv", rows=slice(j * h, (j + 1) * h))
+            put(f"{s.name}.o_proj", s, "w_o")
         for s in [s for pair in self.double for s in pair] + self.single:
             p = s.name
             for j, n in enumerate("qkv"):
@@ -480,6 +532,9 @@ class MMDiT:
             "hid_img": buf(B * N, r * h), "hid_txt": buf(B * T, r * h),
             "rows_in": buf(B * N, self.w_x.shape[1]), "rows_out": buf(B * N, self.w_final.shape[0]),
         }
+        if self.attn2:                                 # MMDiT-X: attn2's packed q/k/v and its attention output
+            ws["qkv2"] = buf(B * N, 3 * h)
+            ws["o2"] = buf(B * N, h)
         if self.is_flux:
             ws["u"] = buf(B * S, h)
             ws["m_u"] = buf(B * S, h)
@@ -558,20 +613,31 @@ class MMDiT:
         self._linear(a, s, "w_qkv", out=qkv, bias=s.b_qkv, rows_per_batch=rows_per_batch, out_batch_rows=S,
                      out_row_off=row_off, qk=self._qk_fused(s, rope))
 
-    def _stream_post(self, s: _Stream, x, o, m, m8, hid, hid8, rows_per_batch):
-        """x += gate1 * o_proj(o); x += gate2 * fc2(gelu(fc1(LN(x)(1+scale2)+shift2)))  (mmdit.py:521-548)"""
-        self._linear(self._lin_in(o, m8), s, "w_o", out=x, bias=s.b_o, gate=self._mod(s.mod_off, 2), res=x,
-                     rows_per_batch=rows_per_batch, out_batch_rows=rows_per_batch)
+    def _stream_post(self, s: _Stream, x, o, m, m8, hid, hid8, rows_per_batch, x_attn=None):
+        """x += gate1 * o_proj(o); x += gate2 * fc2(gelu(fc1(LN(x)(1+scale2)+shift2)))  (mmdit.py:521-548).
+        x_attn = (attn2 stream, its attention output): MMDiT-X's x += gate_msa2 * attn2.o_proj(o2) between the two."""
+        for st, ot in [(s, o)] + ([x_attn] if x_attn is not None else []):
+            self._linear(self._lin_in(ot, m8), st, "w_o", out=x, bias=st.b_o, gate=self._mod(st.mod_off, 2), res=x,
+                         rows_per_batch=rows_per_batch, out_batch_rows=rows_per_batch)
         a = self._ln_mod(x, s, 3, rows_per_batch, m, m8)
         self._linear(a, s, "w_fc1", out=hid, bias=s.b_fc1, act=ACT_GELU_ERF)
         self._linear(self._lin_in(hid, hid8), s, "w_fc2", out=x, bias=s.b_fc2, gate=self._mod(s.mod_off, 5), res=x,
                      rows_per_batch=rows_per_batch, out_batch_rows=rows_per_batch)
 
     def __call__(self, latent_image_embeddings: torch.Tensor, token_level_text_embeddings: torch.Tensor,
-                 timestep=None) -> torch.Tensor:
+                 timestep=None, *, skip_layers=(), skip_batch: int = 0) -> torch.Tensor:
         """latent (B, H, W, 16) NHWC, text (B, T, 1, 4096) or (B, T, 4096), timestep (B,) tensor / float
-        (all entries equal, as in the reference which reads timestep[0], mmdit.py:445-447) -> (B, H, W, 16)."""
+        (all entries equal, as in the reference which reads timestep[0], mmdit.py:445-447) -> (B, H, W, 16).
+        skip_layers / skip_batch (skip-layer guidance): the last skip_batch sequences skip the listed joint blocks,
+        both of their streams passing through them unchanged."""
         c = self.config
+        skip_layers = tuple(sorted(set(int(i) for i in skip_layers)))
+        if skip_layers:
+            if self.is_flux:
+                raise ValueError("skip_layers: skip-layer guidance runs on SD3-family models only")
+            if not all(0 <= i < c.depth_multimodal for i in skip_layers):
+                raise ValueError(f"skip_layers {skip_layers} must be joint block indices in [0, {c.depth_multimodal})")
+        skip_batch = int(skip_batch) if skip_layers else 0
         x = latent_image_embeddings
         if x.dim() != 4:
             raise ValueError(f"Input tensor must have rank 4, got {x.dim()}")
@@ -592,10 +658,14 @@ class MMDiT:
             tval = float(timestep.reshape(-1)[0]) if torch.is_tensor(timestep) else float(timestep)
             if tval != getattr(self, "_cur_t", None):
                 self.select_timestep(tval)
-        if self._mod_cur is None or self._mod_batch != B:
+        if skip_layers and not 0 < skip_batch < B:
+            raise ValueError(f"skip_batch must be in (0, {B}) with skip_layers, got {skip_batch}")
+        lead = self._mod_batch - self._mod_skip_batch        # a forward without the skip rows reads the leading rows
+        if self._mod_cur is None or B not in (self._mod_batch, lead):
             raise DkError(f"modulation cache holds batch {self._mod_batch}, forward got batch {B}")
-        key = (B, H, W, Cl, T)
+        key = (B, H, W, Cl, T, skip_layers, skip_batch)
         state = self._shapes.state(key, self.max_cached_shapes)
+        state["skip"] = (frozenset(skip_layers), skip_batch)
         if self._step_cache is not None:
             return self._cached_forward(state, key, x, text, B, H, W, Cl, T)
         return self._shapes.run(state, self.use_cuda_graphs,
@@ -607,7 +677,8 @@ class MMDiT:
         hp, wp = H // c.patch_size, W // c.patch_size
         N = hp * wp
         g = {"B": B, "T": T, "N": N, "S": N + T, "hp": hp, "wp": wp, "ws": self._workspace(state, B, N, T),
-             "w8": self._workspace8(state, B, N, T).get, "state": state}
+             "w8": self._workspace8(state, B, N, T).get, "state": state,
+             "skip_layers": state["skip"][0], "skip_batch": state["skip"][1]}
         g["rope"] = self._rope_table(state, T, hp, wp) if c.pos_embed_type == PositionalEncoding.PreSDPARope else None
         # joint sequence order: FLUX [text, image] (mmdit.py:594-606), SD3 [image, text] (:608-625)
         g["off_img"], g["off_txt"], g["split"] = (T, 0, T) if self.is_flux else (0, N, N)
@@ -628,6 +699,8 @@ class MMDiT:
                      out_batch_rows=N, res_batch_rows=0)
 
     def _double_block(self, g, i: int):
+        if i in g["skip_layers"]:
+            g = self._leading(g, g["B"] - g["skip_batch"])
         ws, w8, B, N, T, S, rope = g["ws"], g["w8"], g["B"], g["N"], g["T"], g["S"], g["rope"]
         img, txt, qkv = ws["img"], ws["txt"], ws["qkv"]
         si, st = self.double[i]
@@ -637,9 +710,29 @@ class MMDiT:
             ops.attention(qkv, B, S, self.heads, self.d, ws["o_txt"], split=g["split"], out1=ws["o_img"])
         else:
             ops.attention(qkv, B, S, self.heads, self.d, ws["o_img"], split=g["split"], out1=ws["o_txt"])
-        self._stream_post(si, img, ws["o_img"], ws["m_img"], w8("m_img"), ws["hid_img"], w8("hid_img"), N)
+        x_attn = None
+        if i in self.attn2:                            # MMDiT-X: self-attention over the image tokens alone
+            s2 = self.attn2[i]
+            self._attn_stream_pre(s2, img, ws["m_img"], w8("m_img"), N, N, 0, ws["qkv2"], rope)
+            ops.attention(ws["qkv2"], B, N, self.heads, self.d, ws["o2"])
+            x_attn = (s2, ws["o2"])
+        self._stream_post(si, img, ws["o_img"], ws["m_img"], w8("m_img"), ws["hid_img"], w8("hid_img"), N, x_attn)
         if not st.skip_post:
             self._stream_post(st, txt, ws["o_txt"], ws["m_txt"], w8("m_txt"), ws["hid_txt"], w8("hid_txt"), T)
+
+    @staticmethod
+    def _leading(g, nb: int) -> dict:
+        """the geometry of the leading nb sequences alone: every batch-major buffer cut to its first nb sequences, so
+        the trailing ones pass through untouched"""
+        B = g["B"]
+
+        def cut(t):
+            return t[: nb * (t.shape[0] // B)]
+
+        w8 = g["w8"]
+        sub = dict(g, B=nb, ws={k: cut(t) for k, t in g["ws"].items()})
+        sub["w8"] = lambda name: None if w8(name) is None else tuple(cut(t) for t in w8(name))
+        return sub
 
     def _single_blocks(self, g):
         """FLUX: u = [text | image], every single-stream block, image rows of u back to img (nothing for SD3)"""

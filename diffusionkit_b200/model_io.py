@@ -139,9 +139,13 @@ def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, ml
 
 
 # ------------------------------------------------------------------------------------------------ SD3 (SAI layout)
-def sd3_checkpoint_to_params(sd: Dict[str, Tensor], prefix: str = "model.diffusion_model.") -> Dict[str, Tensor]:
-    """Stability `sd3_medium.safetensors` -> MMDiT parameter tree (reference model_io.py:314-408).
-    VAE (`first_stage_model.` / `decoder.` / `encoder.`) and `teacher_model.` tensors are skipped here."""
+def sd3_checkpoint_to_params(sd: Dict[str, Tensor], prefix: str = "model.diffusion_model.", *,
+                             k_bias: bool = False) -> Dict[str, Tensor]:
+    """Stability `sd3_medium.safetensors` / `sd3.5_*.safetensors` -> MMDiT parameter tree (reference
+    model_io.py:314-408).  VAE (`first_stage_model.` / `decoder.` / `encoder.`) and `teacher_model.` tensors are
+    skipped here.  SD3.5 Medium's x-block second attention (MMDiT-X) maps as the first one does:
+    attn2.qkv -> attn2.{q,k,v}_proj, attn2.proj -> attn2.o_proj, attn2.ln_{q,k} -> qk_norm2.{q,k}_norm.
+    The k bias of every qkv is dropped (quirk Q3) unless `k_bias` (MMDiTConfig.attn_k_bias) keeps it."""
     out: Dict[str, Tensor] = {}
     for key, v in sd.items():
         if "decoder." in key or "encoder." in key or "teacher_model." in key:
@@ -153,18 +157,19 @@ def sd3_checkpoint_to_params(sd: Dict[str, Tensor], prefix: str = "model.diffusi
             i, blk, rest = m.groups()
             stream = "text_transformer_block" if blk == "context_block" else "image_transformer_block"
             base = f"multimodal_transformer_blocks.{i}.{stream}"
-            if rest.startswith("attn.qkv."):
-                leaf = rest[9:]
-                for name, chunk in zip("qkv", v.chunk(3, dim=0)):
-                    if name == "k" and leaf == "bias":
-                        continue                     # model_io.py:389-390
-                    out[f"{base}.attn.{name}_proj.{leaf}"] = chunk.contiguous()
-            elif rest.startswith("attn.proj."):
-                out[f"{base}.attn.o_proj.{rest[10:]}"] = v
-            elif rest.startswith("attn.ln_q."):
-                out[f"{base}.qk_norm.q_norm.{rest[10:]}"] = v
-            elif rest.startswith("attn.ln_k."):
-                out[f"{base}.qk_norm.k_norm.{rest[10:]}"] = v
+            a = re.fullmatch(r"(attn2?)\.(qkv|proj|ln_q|ln_k)\.(.+)", rest)
+            if a:
+                attn, part, leaf = a.groups()
+                norm = "qk_norm" if attn == "attn" else "qk_norm2"
+                if part == "qkv":
+                    for name, chunk in zip("qkv", v.chunk(3, dim=0)):
+                        if name == "k" and leaf == "bias" and not k_bias:
+                            continue                 # model_io.py:389-390
+                        out[f"{base}.{attn}.{name}_proj.{leaf}"] = chunk.contiguous()
+                elif part == "proj":
+                    out[f"{base}.{attn}.o_proj.{leaf}"] = v
+                else:
+                    out[f"{base}.{norm}.{part[-1]}_norm.{leaf}"] = v
             elif rest.startswith("adaLN_modulation."):
                 out[f"{base}.adaLN_modulation.layers.{rest[17:]}"] = v
             else:                                    # mlp.fc1 / mlp.fc2 keep their names

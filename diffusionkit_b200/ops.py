@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Optional
+from typing import Optional, Tuple
 
 import torch
 
@@ -280,15 +280,22 @@ def sampler_prepare(x, xin, reps: int):
     return xin
 
 
-def sampler_step(x, xin, out, sigma: float, sigma_next: float, cfg_weight: float):
+def _slg_entry(name: str, slg: float) -> Tuple[str, tuple]:
+    """the plain solver-update entry point for slg == 0, its skip-layer-guidance twin (DESIGN.md §13) otherwise:
+    then xin / out hold [positive | negative | positive skipping joint blocks] and D gains slg (D_pos - D_skip)"""
+    return (name, ()) if slg == 0.0 else (name + "_slg", (float(slg),))
+
+
+def sampler_step(x, xin, out, sigma: float, sigma_next: float, cfg_weight: float, slg: float = 0.0):
     assert x.dtype == torch.float32 and x.is_contiguous()
     c = ctx(x.device.index)
-    c.call("dk_sampler_step", dtype_code(xin.dtype), ptr(x), ptr(xin), ptr(out), x.numel(), sigma, sigma_next,
-           cfg_weight)
+    name, extra = _slg_entry("dk_sampler_step", slg)
+    c.call(name, dtype_code(xin.dtype), ptr(x), ptr(xin), ptr(out), x.numel(), sigma, sigma_next, cfg_weight, *extra)
     return x
 
 
-def sampler_heun_predict(x, xin, out, sigma: float, sigma_next: float, cfg_weight: float, d=None, x2=None):
+def sampler_heun_predict(x, xin, out, sigma: float, sigma_next: float, cfg_weight: float, d=None, x2=None,
+                         slg: float = 0.0):
     """-> (d, x2): the slope at (x, sigma) and the Euler step to sigma_next (fp32, like x); x is not modified"""
     assert x.dtype == torch.float32 and x.is_contiguous()
     d = torch.empty_like(x) if d is None else d
@@ -296,28 +303,32 @@ def sampler_heun_predict(x, xin, out, sigma: float, sigma_next: float, cfg_weigh
     assert d.shape == x2.shape == x.shape and d.dtype == x2.dtype == torch.float32
     assert d.is_contiguous() and x2.is_contiguous()
     c = ctx(x.device.index)
-    c.call("dk_sampler_heun_predict", dtype_code(xin.dtype), ptr(x), ptr(xin), ptr(out), ptr(d), ptr(x2), x.numel(),
-           sigma, sigma_next, cfg_weight)
+    name, extra = _slg_entry("dk_sampler_heun_predict", slg)
+    c.call(name, dtype_code(xin.dtype), ptr(x), ptr(xin), ptr(out), ptr(d), ptr(x2), x.numel(), sigma, sigma_next,
+           cfg_weight, *extra)
     return d, x2
 
 
-def sampler_heun_correct(x, d, x2, xin, out, sigma: float, sigma_next: float, cfg_weight: float):
+def sampler_heun_correct(x, d, x2, xin, out, sigma: float, sigma_next: float, cfg_weight: float, slg: float = 0.0):
     """x += (d + d2) / 2 * (sigma_next - sigma), d2 the slope of the forward (xin, out) at (x2, sigma_next)"""
     assert x.dtype == d.dtype == x2.dtype == torch.float32
     assert x.is_contiguous() and d.is_contiguous() and x2.is_contiguous() and d.shape == x2.shape == x.shape
     c = ctx(x.device.index)
-    c.call("dk_sampler_heun_correct", dtype_code(xin.dtype), ptr(x), ptr(d), ptr(x2), ptr(xin), ptr(out), x.numel(),
-           sigma, sigma_next, cfg_weight)
+    name, extra = _slg_entry("dk_sampler_heun_correct", slg)
+    c.call(name, dtype_code(xin.dtype), ptr(x), ptr(d), ptr(x2), ptr(xin), ptr(out), x.numel(), sigma, sigma_next,
+           cfg_weight, *extra)
     return x
 
 
-def sampler_dpmpp_2m(x, d_prev, xin, out, sigma: float, a: float, b: float, c: float, cfg_weight: float):
+def sampler_dpmpp_2m(x, d_prev, xin, out, sigma: float, a: float, b: float, c: float, cfg_weight: float,
+                     slg: float = 0.0):
     """x = a x + b D + c d_prev, then d_prev = D (both in place); d_prev is not read when c == 0"""
     assert x.dtype == d_prev.dtype == torch.float32 and x.is_contiguous() and d_prev.is_contiguous()
     assert d_prev.shape == x.shape
     cx = ctx(x.device.index)
-    cx.call("dk_sampler_dpmpp_2m", dtype_code(xin.dtype), ptr(x), ptr(d_prev), ptr(xin), ptr(out), x.numel(), sigma,
-            a, b, c, cfg_weight)
+    name, extra = _slg_entry("dk_sampler_dpmpp_2m", slg)
+    cx.call(name, dtype_code(xin.dtype), ptr(x), ptr(d_prev), ptr(xin), ptr(out), x.numel(), sigma, a, b, c,
+            cfg_weight, *extra)
     return x
 
 

@@ -15,6 +15,8 @@ Differences that are deliberate (documented in DESIGN.md):
     a scalar seed behaves exactly like the reference.
   * FLUX.1-dev's distilled guidance (`guidance=` of FluxPipeline.generate_image / denoise_latents) when the pipeline is
     built with mmdit_config=FLUX_DEV; the reference loads dev without its guidance embedder (quirk Q1).
+  * SD3.5 Medium (model_version "stabilityai/stable-diffusion-3.5-medium") and skip-layer guidance (`slg=` of
+    DiffusionPipeline.generate_image / denoise_latents, any SD3-family model under CFG), DESIGN.md §13.
 """
 from __future__ import annotations
 
@@ -29,7 +31,8 @@ from . import ops
 from ._lib import DkError
 from .config import MODEL_CONFIGS, T5_MAX_LENGTH, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig
 from .mmdit import MMDiT
-from .sampler import FluxSampler, ModelSamplingDiscreteFlow, dpmpp_2m_coefficients
+from .sampler import (FluxSampler, ModelSamplingDiscreteFlow, SkipLayerGuidance, check_skip_layer_guidance,
+                      dpmpp_2m_coefficients, skip_layer_guidance_steps)
 from .vae import VAEDecoder, VAEEncoder
 from .weights import init_params, mmdit_param_specs, vae_decoder_param_specs, vae_encoder_param_specs
 
@@ -40,6 +43,7 @@ MMDIT_CKPT = {  # reference mlx/__init__.py:37-44
     "argmaxinc/mlx-FLUX.1-schnell": "argmaxinc/mlx-FLUX.1-schnell",
     "argmaxinc/mlx-FLUX.1-schnell-4bit-quantized": "argmaxinc/mlx-FLUX.1-schnell-4bit-quantized",
     "argmaxinc/mlx-FLUX.1-dev": "argmaxinc/mlx-FLUX.1-dev",
+    "stabilityai/stable-diffusion-3.5-medium": "stabilityai/stable-diffusion-3.5-medium",
 }
 
 # FLUX.1-dev's guidance when the caller passes none (BFL's default for the dev checkpoint)
@@ -85,22 +89,36 @@ class CFGDenoiser:
 
     def __init__(self, model: "DiffusionPipeline"):
         self.model = model
+        # skip-layer guidance of the running denoise: (SkipLayerGuidance, its steps, [pos | neg | pos] conditioning)
+        self.slg = None
 
-    def cache_modulation_params(self, pooled_text_embeddings, sigmas, guidance=None):
-        """guidance: one FLUX.1-dev guidance value per row of pooled (None without a guidance embedder)"""
-        self.model.mmdit.cache_modulation_params(pooled_text_embeddings, sigmas, guidance)
+    def cache_modulation_params(self, pooled_text_embeddings, sigmas, guidance=None, skip_batch: int = 0):
+        """guidance: one FLUX.1-dev guidance value per row of pooled (None without a guidance embedder).
+        skip_batch: the trailing rows of pooled that condition skip-layer guidance's skip forwards"""
+        self.model.mmdit.cache_modulation_params(pooled_text_embeddings, sigmas, guidance, skip_batch=skip_batch)
+
+    def slg_scale(self, step) -> float:
+        """the skip-layer guidance scale of solver step `step` (0: plain CFG)"""
+        return self.slg[0].scale if self.slg is not None and step in self.slg[1] else 0.0
 
     def clear_cache(self):
         # the reference re-reads the adaLN weights it dropped (:686-689); nothing was dropped here
         pass
 
-    def __call__(self, x_t, timestep, sigma, conditioning, cfg_weight: float = 7.5, pooled_conditioning=None):
+    def __call__(self, x_t, timestep, sigma, conditioning, cfg_weight: float = 7.5, pooled_conditioning=None,
+                 step=None):
+        """step: the solver step this evaluation belongs to; inside the skip-layer guidance window the forward runs on
+        [pos | neg | pos] with the listed joint blocks skipped for the last third"""
         m = self.model
         reps = 1 if cfg_weight <= 0 else 2
         B = x_t.shape[0]
+        skip = {}
+        if self.slg is not None and step in self.slg[1]:
+            reps, conditioning = 3, self.slg[2]
+            skip = dict(skip_layers=self.slg[0].layers, skip_batch=B)
         xin = torch.empty((reps * B,) + tuple(x_t.shape[1:]), dtype=m.activation_dtype, device=x_t.device)
         ops.sampler_prepare(x_t, xin, reps)
-        out = m.mmdit(latent_image_embeddings=xin, token_level_text_embeddings=conditioning, timestep=timestep)
+        out = m.mmdit(latent_image_embeddings=xin, token_level_text_embeddings=conditioning, timestep=timestep, **skip)
         return xin, out
 
 
@@ -115,9 +133,17 @@ def _start_sampling(model: CFGDenoiser, sigmas, extra_args):
     timesteps = torch.from_numpy(np.asarray(pipe.sampler.timestep(sig), dtype=np.float32)).to(
         pipe.activation_dtype).to(torch.float32).tolist()
     pooled = extra_args.pop("pooled_conditioning")
-    model.cache_modulation_params(pooled, timesteps, extra_args.pop("guidance", None))
     cfg_weight = float(extra_args.get("cfg_weight", 0.0))
     conditioning = extra_args["conditioning"]
+    slg = extra_args.pop("slg", None)
+    steps = skip_layer_guidance_steps(slg, len(sig) - 1) if slg is not None else []
+    skip_batch = 0
+    if steps:
+        # rows [pos x B | neg x B | pos x B]: the forwards inside the window skip the listed blocks for the last B
+        skip_batch = pooled.shape[0] // 2
+        pooled = torch.cat([pooled, pooled[:skip_batch]])
+        model.slg = (slg, frozenset(steps), torch.cat([conditioning, conditioning[:skip_batch]]))
+    model.cache_modulation_params(pooled, timesteps, extra_args.pop("guidance", None), skip_batch)
     events = [torch.cuda.Event(enable_timing=True) for _ in range(len(sig))]
     events[0].record()
     return sig, timesteps, conditioning, cfg_weight, events
@@ -126,6 +152,7 @@ def _start_sampling(model: CFGDenoiser, sigmas, extra_args):
 def _finish_sampling(model: CFGDenoiser, events):
     """-> iter_time: seconds per step, from the events recorded after each step"""
     model.clear_cache()
+    model.slg = None
     torch.cuda.current_stream().synchronize()  # the reference syncs every step (mx.eval, :782); once is enough here
     return [round(events[i].elapsed_time(events[i + 1]) / 1e3, 3) for i in range(len(events) - 1)]
 
@@ -135,9 +162,9 @@ def sample_euler(model: CFGDenoiser, x, sigmas, extra_args=None):
     x: (B, H, W, 16) fp32 device tensor (updated in place); sigmas: 1-D float32 numpy/torch array."""
     sig, timesteps, conditioning, cfg_weight, events = _start_sampling(model, sigmas, extra_args)
     for i in range(len(sig) - 1):
-        xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight)
+        xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight, step=i)
         # denoised = xin - out * sigma; CFG mix; d = (x - denoised) / sigma; x += d * (sigma_next - sigma)
-        ops.sampler_step(x, xin, out, float(sig[i]), float(sig[i + 1]), cfg_weight)
+        ops.sampler_step(x, xin, out, float(sig[i]), float(sig[i + 1]), cfg_weight, slg=model.slg_scale(i))
         events[i + 1].record()
     return x, _finish_sampling(model, events)
 
@@ -150,15 +177,16 @@ def sample_heun(model: CFGDenoiser, x, sigmas, extra_args=None):
     d = x2 = None
     for i in range(len(sig) - 1):
         s, s_next = float(sig[i]), float(sig[i + 1])
-        xin, out = model(x, timesteps[i], s, conditioning, cfg_weight)
+        slg = model.slg_scale(i)                      # both evaluations of a step take that step's decision
+        xin, out = model(x, timesteps[i], s, conditioning, cfg_weight, step=i)
         if s_next == 0.0:
-            ops.sampler_step(x, xin, out, s, s_next, cfg_weight)
+            ops.sampler_step(x, xin, out, s, s_next, cfg_weight, slg=slg)
         else:
             if d is None:
                 d, x2 = torch.empty_like(x), torch.empty_like(x)
-            ops.sampler_heun_predict(x, xin, out, s, s_next, cfg_weight, d, x2)
-            xin, out = model(x2, timesteps[i + 1], s_next, conditioning, cfg_weight)
-            ops.sampler_heun_correct(x, d, x2, xin, out, s, s_next, cfg_weight)
+            ops.sampler_heun_predict(x, xin, out, s, s_next, cfg_weight, d, x2, slg=slg)
+            xin, out = model(x2, timesteps[i + 1], s_next, conditioning, cfg_weight, step=i)
+            ops.sampler_heun_correct(x, d, x2, xin, out, s, s_next, cfg_weight, slg=slg)
         events[i + 1].record()
     return x, _finish_sampling(model, events)
 
@@ -171,9 +199,9 @@ def sample_dpmpp_2m(model: CFGDenoiser, x, sigmas, extra_args=None):
     coef = dpmpp_2m_coefficients(sig)
     d_prev = torch.empty_like(x)
     for i in range(len(sig) - 1):
-        xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight)
+        xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight, step=i)
         a, b, c = (float(v) for v in coef[i])
-        ops.sampler_dpmpp_2m(x, d_prev, xin, out, float(sig[i]), a, b, c, cfg_weight)
+        ops.sampler_dpmpp_2m(x, d_prev, xin, out, float(sig[i]), a, b, c, cfg_weight, slg=model.slg_scale(i))
         events[i + 1].record()
     return x, _finish_sampling(model, events)
 
@@ -184,6 +212,15 @@ SOLVERS = {"euler": sample_euler, "heun": sample_heun, "dpmpp_2m": sample_dpmpp_
 def _check_solver(solver: str):
     if solver not in SOLVERS:
         raise ValueError(f"unknown solver {solver!r}: expected one of {', '.join(repr(k) for k in SOLVERS)}")
+
+
+def _check_slg(slg, cfg_weight: float, config: MMDiTConfig):
+    """skip-layer guidance arguments, refused with ValueError before any GPU work"""
+    if slg is None:
+        return
+    if config.depth_unified > 0:
+        raise ValueError("skip-layer guidance runs on SD3-family models only, not on a FLUX-shaped config")
+    check_skip_layer_guidance(slg, cfg_weight, config.depth_multimodal)
 
 
 class DiffusionPipeline:
@@ -272,7 +309,7 @@ class DiffusionPipeline:
                 params = model_io.flux_checkpoint_to_params(sd, self.config.hidden_size, self.config.mlp_ratio,
                                                             guidance_embed=self.config.guidance_embed)
             else:
-                params = model_io.sd3_checkpoint_to_params(sd)
+                params = model_io.sd3_checkpoint_to_params(sd, k_bias=self.config.attn_k_bias)
                 if "vae" not in paths and any("decoder." in k for k in sd):
                     out["vae"] = model_io.vae_decoder_checkpoint_to_params(sd)     # single-file SD3 checkpoints
                 if "vae" not in paths and any("encoder.down." in k for k in sd):
@@ -502,14 +539,16 @@ class DiffusionPipeline:
         *,
         noise: Optional[torch.Tensor] = None,
         solver: str = "euler",
+        slg: Optional[SkipLayerGuidance] = None,
     ):
         """-> (latent NHWC (B, H, W, 16) fp32 on the device, iter_time list).  `noise` (optional, device fp32
         (B, H, W, 16)) replaces the host-side numpy draw of get_noise for callers whose inputs already live in HBM.
         `image_path` (img2img): a file path, a PIL image or a uint8 HWC array; the latent size then follows the image
         (the reference ignores latent_size in that case too, :273).  `solver`: "euler" (the reference's sampler),
-        "heun" (two model evaluations per step but the last) or "dpmpp_2m" (one per step), DESIGN.md §11."""
+        "heun" (two model evaluations per step but the last) or "dpmpp_2m" (one per step), DESIGN.md §11.
+        `slg`: skip-layer guidance (sampler.SkipLayerGuidance, needs cfg_weight > 0; None: off), DESIGN.md §13."""
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
-                                     image_path, denoise, noise=noise, solver=solver, guidance=None)
+                                     image_path, denoise, noise=noise, solver=solver, guidance=None, slg=slg)
 
     def _guidance_values(self, guidance, n_images: int) -> Optional[List[float]]:
         """FluxPipeline's `guidance` -> one FLUX.1-dev guidance value per image, or None for a model without a
@@ -533,8 +572,9 @@ class DiffusionPipeline:
         return vals
 
     def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
-                         denoise, *, noise, solver, guidance):
+                         denoise, *, noise, solver, guidance, slg=None):
         _check_solver(solver)
+        _check_slg(slg, cfg_weight, self.config)
         if image_path is None:
             denoise = 1.0                                                   # :270-271
         elif not (0.0 <= denoise <= 1.0):
@@ -594,6 +634,8 @@ class DiffusionPipeline:
         if guidance is not None:
             # rows [positive x B | negative x B]: both rows of an image get its value
             extra_args["guidance"] = guidance * reps
+        if slg is not None:
+            extra_args["slg"] = slg
         latent, iter_time = SOLVERS[solver](CFGDenoiser(self), x, sigmas, extra_args=extra_args)
         latent = ops.axpb(latent, 1.0 / self.latent_format.scale_factor, self.latent_format.shift_factor)  # process_out
         return latent, iter_time
@@ -614,14 +656,18 @@ class DiffusionPipeline:
         conditioning=None,
         pooled_conditioning=None,
         solver: str = "euler",
+        slg: Optional[SkipLayerGuidance] = None,
     ):
+        """`slg`: skip-layer guidance as in denoise_latents; the log then holds its scale, layers and the steps it
+        applied to under log["denoising"]["skip_layer_guidance"]."""
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
-                                    solver=solver, guidance=None)
+                                    solver=solver, guidance=None, slg=slg)
 
     def _generate_image(self, text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
-                        denoise, *, conditioning, pooled_conditioning, solver, guidance):
+                        denoise, *, conditioning, pooled_conditioning, solver, guidance, slg=None):
         _check_solver(solver)
+        _check_slg(slg, cfg_weight, self.config)
         guidance = self._guidance_values(guidance, len(seed) if isinstance(seed, (list, tuple)) else 1)
         assert latent_size[0] % 2 == 0, f"Height must be divisible by 16 ({latent_size[0]*8}/16={latent_size[0]/2})"
         assert latent_size[1] % 2 == 0, f"Width must be divisible by 16 ({latent_size[1]*8}/16={latent_size[1]/2})"
@@ -652,7 +698,7 @@ class DiffusionPipeline:
         log["denoising"]["pre"] = mem()
         latents, iter_time = self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight,
                                                    latent_size, seed, image_path, denoise, noise=None, solver=solver,
-                                                   guidance=guidance)
+                                                   guidance=guidance, slg=slg)
         torch.cuda.synchronize(self.device)
         log["denoising"]["post"] = mem()
         log["denoising"]["time"] = round(time.time() - t0, 3)
@@ -664,6 +710,10 @@ class DiffusionPipeline:
             log["denoising"]["nfe"] = max(2 * n - 1, 0) if solver == "heun" else n
         if guidance is not None:
             log["denoising"]["guidance"] = guidance
+        if slg is not None:
+            log["denoising"]["skip_layer_guidance"] = {
+                "scale": slg.scale, "layers": list(slg.layers),
+                "steps": skip_layer_guidance_steps(slg, len(iter_time))}
         if self.mmdit.step_cache is not None:
             log["denoising"]["step_cache"] = [{"rel": rel, "skipped": skipped}
                                               for rel, skipped in self.mmdit.step_cache_log]

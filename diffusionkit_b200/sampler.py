@@ -5,6 +5,8 @@ fused CUDA sampler kernels (csrc/elementwise.cu: dk_sampler_prepare / dk_sampler
 DPM-Solver++(2M) updates, whose fp64 coefficients dpmpp_2m_coefficients computes).
 """
 import math
+from dataclasses import dataclass
+from typing import List, Tuple
 
 import numpy as np
 
@@ -91,3 +93,38 @@ def dpmpp_2m_coefficients(sigmas) -> np.ndarray:
         else:
             coef[i] = (s[i + 1] / s[i], b1, 0.0)
     return coef
+
+
+@dataclass(frozen=True)
+class SkipLayerGuidance:
+    """Skip-layer guidance (SLG) for SD3-family models under CFG, as Stability's SkipLayerCFGDenoiser applies it: on the
+    steps i of the n run with start·n < i < end·n, D = D_neg + w (D_pos - D_neg) + scale (D_pos - D_skip), where D_skip
+    is the positive prompt's estimate from a forward that skips the joint blocks `layers`.  The defaults are
+    Stability's published setting for SD3.5 Medium."""
+
+    scale: float = 2.5
+    layers: Tuple[int, ...] = (7, 8, 9)
+    start: float = 0.01
+    end: float = 0.20
+
+
+def check_skip_layer_guidance(slg: SkipLayerGuidance, cfg_weight: float, depth: int) -> None:
+    """Raise ValueError for a setting a model of `depth` joint blocks cannot run (before any GPU work)."""
+    if not isinstance(slg, SkipLayerGuidance):
+        raise ValueError(f"slg must be a SkipLayerGuidance or None, got {type(slg).__name__}")
+    if not cfg_weight > 0:
+        raise ValueError(f"skip-layer guidance needs CFG (cfg_weight > 0), got cfg_weight={cfg_weight}")
+    layers = tuple(slg.layers)
+    if not layers or len(set(layers)) != len(layers) or not all(
+            isinstance(i, (int, np.integer)) and 0 <= i < depth for i in layers):
+        raise ValueError(f"skip-layer guidance layers {layers} must be distinct joint block indices in [0, {depth})")
+    if not 0.0 <= slg.start < slg.end <= 1.0:
+        raise ValueError(f"skip-layer guidance window needs 0 <= start < end <= 1, got start={slg.start}, "
+                         f"end={slg.end}")
+    if not math.isfinite(slg.scale):
+        raise ValueError(f"skip-layer guidance scale must be finite, got {slg.scale}")
+
+
+def skip_layer_guidance_steps(slg: SkipLayerGuidance, n: int) -> List[int]:
+    """the steps i of n where SLG applies: start·n < i < end·n (Stability's window, in the steps actually run)"""
+    return [i for i in range(n) if slg.start * n < i < slg.end * n]

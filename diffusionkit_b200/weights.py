@@ -55,9 +55,10 @@ def mmdit_param_specs(cfg: MMDiTConfig) -> List[Spec]:
             specs.append((prefix + ".qk_norm.q_norm.weight", (d,), "g"))
             specs.append((prefix + ".qk_norm.k_norm.weight", (d,), "g"))
 
+    x_layers = set(cfg.x_block_self_attn_layers)
     for i in range(cfg.depth_multimodal):
         skip_text = (i == cfg.depth_multimodal - 1) and (cfg.depth_unified < 1)
-        block(f"multimodal_transformer_blocks.{i}.image_transformer_block", 6)
+        block(f"multimodal_transformer_blocks.{i}.image_transformer_block", 9 if i in x_layers else 6)
         block(f"multimodal_transformer_blocks.{i}.text_transformer_block", 2 if skip_text else 6, skip_post=skip_text)
     for i in range(cfg.depth_unified):
         block(f"unified_transformer_blocks.{i}.transformer_block", 3 if cfg.parallel_mlp_for_unified_blocks else 6)
@@ -68,6 +69,17 @@ def mmdit_param_specs(cfg: MMDiTConfig) -> List[Spec]:
         # by spec index) gives every other tensor the values it has without the embedder.
         lin("guidance_in.mlp.layers.0", h, cfg.frequency_embed_dim)
         lin("guidance_in.mlp.layers.2", h, h)
+    # MMDiT-X (SD3.5 Medium) and the kept k bias, appended for the same reason
+    for i in sorted(x_layers):
+        prefix = f"multimodal_transformer_blocks.{i}.image_transformer_block"
+        for n in "qkvo":
+            lin(f"{prefix}.attn2.{n}_proj", h, h, bias=n != "k" or cfg.attn_k_bias)
+        specs.append((prefix + ".qk_norm2.q_norm.weight", (d,), "g"))
+        specs.append((prefix + ".qk_norm2.k_norm.weight", (d,), "g"))
+    if cfg.attn_k_bias:
+        for name, _, _ in list(specs):
+            if name.endswith(".attn.k_proj.weight"):
+                specs.append((name[:-len("weight")] + "bias", (h,), "b"))
     return specs
 
 

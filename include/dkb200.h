@@ -192,6 +192,9 @@ int dk_copy_rows(dk_ctx* ctx, int dtype, const void* src, void* dst, int B, int 
  *                            d2 = (x2 - D(x2, sigma_next)) / sigma_next; x += (d + d2) / 2 * (sigma_next - sigma)
  *   dk_sampler_dpmpp_2m:     x = a x + b D + c d_prev; d_prev = D   (d_prev not read when c == 0; a, b, c from
  *                            sampler.dpmpp_2m_coefficients)
+ *   *_slg: the same updates with skip-layer guidance (DESIGN.md §13); xin / out hold [pos | neg | pos skipping joint
+ *          blocks] (reps = 3 in dk_sampler_prepare) and D = D_neg + w (D_pos - D_neg) + slg (D_pos - D_skip).
+ *          cfg_weight must be > 0 and slg finite.
  * ------------------------------------------------------------------------------------------- */
 int dk_sampler_prepare(dk_ctx* ctx, int dtype, const float* x, void* xin, long long n_per_rep, int reps, void* stream);
 int dk_sampler_step(dk_ctx* ctx, int dtype, float* x, const void* xin, const void* out, long long n, float sigma,
@@ -202,6 +205,17 @@ int dk_sampler_heun_correct(dk_ctx* ctx, int dtype, float* x, const float* d, co
                             const void* out, long long n, float sigma, float sigma_next, float cfg_weight, void* stream);
 int dk_sampler_dpmpp_2m(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin, const void* out, long long n,
                         float sigma, float a, float b, float c, float cfg_weight, void* stream);
+int dk_sampler_step_slg(dk_ctx* ctx, int dtype, float* x, const void* xin, const void* out, long long n, float sigma,
+                        float sigma_next, float cfg_weight, float slg, void* stream);
+int dk_sampler_heun_predict_slg(dk_ctx* ctx, int dtype, const float* x, const void* xin, const void* out, float* d,
+                                float* x2, long long n, float sigma, float sigma_next, float cfg_weight, float slg,
+                                void* stream);
+int dk_sampler_heun_correct_slg(dk_ctx* ctx, int dtype, float* x, const float* d, const float* x2, const void* xin,
+                                const void* out, long long n, float sigma, float sigma_next, float cfg_weight, float slg,
+                                void* stream);
+int dk_sampler_dpmpp_2m_slg(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin, const void* out,
+                            long long n, float sigma, float a, float b, float c, float cfg_weight, float slg,
+                            void* stream);
 /* y = x * a + b (fp32): latent_format.process_out (__init__.py:732-733) and noise scaling (sampler.py:41-42) */
 int dk_axpb_f32(dk_ctx* ctx, const float* x, float* y, long long n, float a, float b, void* stream);
 /* ---- text encoders (SURVEY.md §8 row f2): CLIP-L/G (mlx/clip.py) and the T5-XXL encoder (mlx/t5.py) ------------- */
