@@ -32,14 +32,6 @@ def _inputs(dtype, cfg, n, seed):
     return x, xin, out
 
 
-def ref_denoised(xin, out, sigma, cfg, n):
-    """D as dk_sampler_step computes it, in fp32 torch"""
-    den = xin.float() - out.float() * sigma
-    if cfg > 0:
-        den = den[n:] + cfg * (den[:n] - den[n:])
-    return den
-
-
 N_ODD = 3 * 4099          # not a multiple of the block or of any vector width
 
 
@@ -53,12 +45,12 @@ def test_heun_kernels(kc, dtype, cfg):
     x0 = x.clone()
     d, x2 = ops.sampler_heun_predict(x, xin, out, sigma, sigma_next, cfg)
     assert torch.equal(x, x0), "the predictor modified x"
-    d_ref = (x - ref_denoised(xin, out, sigma, cfg, n)) / sigma
+    d_ref = (x - kc.ref_denoised(xin, out, sigma, cfg, n)) / sigma
     x2_ref = x + d_ref * (sigma_next - sigma)
     kc._assert_close("heun_predict_d", d, d_ref, 1e-6)
     kc._assert_close("heun_predict_x2", x2, x2_ref, 1e-6)
     _, xin2, out2 = _inputs(dtype, cfg, n, 2)                   # the forward at (x2, sigma_next)
-    d2_ref = (x2 - ref_denoised(xin2, out2, sigma_next, cfg, n)) / sigma_next
+    d2_ref = (x2 - kc.ref_denoised(xin2, out2, sigma_next, cfg, n)) / sigma_next
     want = x + (d + d2_ref) / 2 * (sigma_next - sigma)
     got = ops.sampler_heun_correct(x.clone(), d, x2, xin2, out2, sigma, sigma_next, cfg)
     kc._assert_close("heun_correct", got, want, 1e-6)
@@ -80,7 +72,7 @@ def test_dpmpp_2m_kernel(kc, dtype, cfg):
         a, b, c = (float(v) for v in coef[i])
         sigma = float(sig[i])
         d_prev = torch.randn((n,), device=DEV)
-        den = ref_denoised(xin, out, sigma, cfg, n)
+        den = kc.ref_denoised(xin, out, sigma, cfg, n)
         want = a * x + b * den + c * d_prev
         got_prev = d_prev.clone()
         got = ops.sampler_dpmpp_2m(x.clone(), got_prev, xin, out, sigma, a, b, c, cfg)
@@ -97,7 +89,7 @@ def test_dpmpp_2m_does_not_read_d_prev_when_c_is_zero(kc):
     d_prev = torch.full((n,), float("nan"), device=DEV)
     got = ops.sampler_dpmpp_2m(x.clone(), d_prev, xin, out, 1.0, 0.75, 0.25, 0.0, 0.0)
     assert bool(torch.isfinite(got).all()) and bool(torch.isfinite(d_prev).all())
-    kc._assert_close("dpmpp_2m_first", got, 0.75 * x + 0.25 * ref_denoised(xin, out, 1.0, 0.0, n), 1e-6)
+    kc._assert_close("dpmpp_2m_first", got, 0.75 * x + 0.25 * kc.ref_denoised(xin, out, 1.0, 0.0, n), 1e-6)
 
 
 def test_heun_correct_refuses_sigma_next_zero(kc):

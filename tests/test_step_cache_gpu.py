@@ -24,18 +24,6 @@ def kc():
 
 
 # ------------------------------------------------------------------------------------------------ kernels
-def _delta_ref(x, base, nseq, rows, x_seq, b_seq, prev):
-    """fp64 sums of the fp32 residual, and the fp32 residual itself"""
-    h = x.shape[1]
-    xs = torch.stack([x[s * x_seq:s * x_seq + rows] for s in range(nseq)]).float()
-    bs = torch.stack([base[s * b_seq:s * b_seq + rows] for s in range(nseq)]).float()
-    r = (xs - bs).reshape(nseq * rows, h)
-    pv = prev.reshape(nseq, rows, h).double()
-    rd = r.reshape(nseq, rows, h).double()
-    sums = torch.stack([(rd - pv).abs().sum(dim=(1, 2)), pv.abs().sum(dim=(1, 2))], dim=1)
-    return r, sums
-
-
 @pytest.mark.parametrize("dtype", [bf16, fp16])
 @pytest.mark.parametrize("nseq,rows,h,x_seq,ldx", [(1, 4096, 3072, 4096, 3072), (8, 4096, 1536, 4096, 1536),
                                                    (3, 37, 128, 37, 128), (2, 1, 8, 1, 8),
@@ -53,7 +41,7 @@ def test_residual_delta(kc, dtype, nseq, rows, h, x_seq, ldx):
     r = torch.empty((nseq * rows, h), dtype=torch.float32, device=DEV)
     sums = ops.residual_delta(x, base, nseq, rows, x_seq_rows=x_seq, r_out=r, prev=prev)
     sums2 = ops.residual_delta(x, base, nseq, rows, x_seq_rows=x_seq, prev=prev)
-    want_r, want = _delta_ref(x, base, nseq, rows, x_seq, rows, prev)
+    want_r, want = kc.ref_residual_delta(x, base, nseq, rows, x_seq, rows, prev)
     assert torch.equal(r, want_r)
     assert torch.equal(sums, sums2)
     err = ((sums.double() - want) / want).abs().max()
