@@ -117,6 +117,8 @@ MODEL_CONFIGS = {
     "argmaxinc/mlx-stable-diffusion-3.5-large": SD3_8b,
     "argmaxinc/mlx-stable-diffusion-3.5-large-4bit-quantized": SD3_8b,
     "stabilityai/stable-diffusion-3.5-medium": SD35_MEDIUM,
+    # FLUX.1 Kontext [dev]: FLUX.1-dev's architecture and guidance embedder, run with reference tokens (DESIGN.md §14)
+    "black-forest-labs/FLUX.1-Kontext-dev": FLUX_DEV,
 }
 
 # T5 sequence lengths (mlx/__init__.py:46-53)
@@ -128,6 +130,7 @@ T5_MAX_LENGTH = {
     "argmaxinc/mlx-FLUX.1-schnell-4bit-quantized": 256,
     "argmaxinc/mlx-FLUX.1-dev": 512,
     "stabilityai/stable-diffusion-3.5-medium": 512,
+    "black-forest-labs/FLUX.1-Kontext-dev": 512,
 }
 
 

@@ -25,6 +25,9 @@ H100 layout decisions (vs. the reference's per-module MLX graph):
   * SD3.5 Medium's MMDiT-X blocks (`config.x_block_self_attn_layers`, DESIGN.md §13): the image stream's second
     self-attention is one more packed stream (attn2) run by the same kernels, and a forward can skip listed blocks
     for its trailing sequences (skip-layer guidance).
+  * FLUX.1 Kontext editing (`reference=` of __call__, DESIGN.md §14): a reference latent's tokens follow the target's
+    in the image stream at RoPE positions (1, r, c); every block runs unchanged on the longer stream and the final
+    layer reads the target rows.
 """
 from __future__ import annotations
 
@@ -515,6 +518,7 @@ class MMDiT:
 
     # ------------------------------------------------------------------------------------------ workspace
     def _workspace(self, st: dict, B: int, N: int, T: int):
+        """N: image-stream rows per sequence (target + reference tokens)"""
         if "ws" in st:
             return st["ws"]
         h, dt, dev = self.h, self.dtype, self.device
@@ -562,16 +566,23 @@ class MMDiT:
         st["ws8"] = w8
         return w8
 
-    def _rope_table(self, st: dict, T: int, hp: int, wp: int) -> torch.Tensor:
+    def _rope_table(self, st: dict, T: int, hp: int, wp: int,
+                    ref_grid: Optional[Tuple[int, int]] = None) -> torch.Tensor:
         """(S, d/2, 2) fp32 cos/sin; text tokens at position (0,0,0), image token (r, c) at (0, r, c)
-        (reference mmdit.py:865-911).  Cached across calls like the reference (:916-932)."""
+        (reference mmdit.py:865-911).  ref_grid (hpr, wpr): Kontext reference token (r, c) at (1, r, c), after the
+        target's.  Cached per input shape like the reference (:916-932)."""
         if "rope" in st:
             return st["rope"]
         axes = self.config.rope_axes_dim
-        S = T + hp * wp
-        pos = torch.zeros((S, 3), dtype=torch.float32)
-        pos[T:, 1] = torch.arange(hp, dtype=torch.float32)[:, None].expand(hp, wp).reshape(-1)
-        pos[T:, 2] = torch.arange(wp, dtype=torch.float32)[None, :].expand(hp, wp).reshape(-1)
+        grids = [(0, hp, wp)] + ([(1, *ref_grid)] if ref_grid is not None else [])
+        pos = torch.zeros((T + sum(a * b for _, a, b in grids), 3), dtype=torch.float32)
+        row = T
+        for axis0, gh, gw in grids:
+            n = gh * gw
+            pos[row:row + n, 0] = float(axis0)
+            pos[row:row + n, 1] = torch.arange(gh, dtype=torch.float32)[:, None].expand(gh, gw).reshape(-1)
+            pos[row:row + n, 2] = torch.arange(gw, dtype=torch.float32)[None, :].expand(gh, gw).reshape(-1)
+            row += n
         parts = []
         for a, dim in enumerate(axes):
             scale = torch.arange(0, dim, 2, dtype=torch.float32) / dim
@@ -624,10 +635,30 @@ class MMDiT:
         self._linear(self._lin_in(hid, hid8), s, "w_fc2", out=x, bias=s.b_fc2, gate=self._mod(s.mod_off, 5), res=x,
                      rows_per_batch=rows_per_batch, out_batch_rows=rows_per_batch)
 
+    def _check_reference(self, reference, B: int, Cl: int):
+        """raise ValueError, before any launch, for a Kontext reference latent this forward cannot take"""
+        if not self.is_flux:
+            raise ValueError("reference: Kontext reference tokens run on FLUX-shaped configs only, not on SD3-family "
+                             "models")
+        if reference.dim() != 4:
+            raise ValueError(f"reference must be an NHWC latent (B, Hr, Wr, {Cl}), got rank {reference.dim()}")
+        Br, Hr, Wr, Cr = reference.shape
+        if Br != B:
+            raise ValueError(f"reference has batch {Br}, the latent has batch {B}")
+        if Cr != Cl:
+            raise ValueError(f"reference has {Cr} channels, the latent has {Cl}")
+        p = self.config.patch_size
+        if Hr % p or Wr % p or Hr == 0 or Wr == 0:
+            raise ValueError(f"reference latent height and width must be positive multiples of {p}, got {Hr}x{Wr}")
+
     def __call__(self, latent_image_embeddings: torch.Tensor, token_level_text_embeddings: torch.Tensor,
-                 timestep=None, *, skip_layers=(), skip_batch: int = 0) -> torch.Tensor:
+                 timestep=None, *, reference: Optional[torch.Tensor] = None, skip_layers=(),
+                 skip_batch: int = 0) -> torch.Tensor:
         """latent (B, H, W, 16) NHWC, text (B, T, 1, 4096) or (B, T, 4096), timestep (B,) tensor / float
         (all entries equal, as in the reference which reads timestep[0], mmdit.py:445-447) -> (B, H, W, 16).
+        reference (FLUX.1 Kontext, FLUX-shaped configs only): a 16-bit (B, Hr, Wr, 16) latent already in the
+        process_in space, Hr and Wr even; its tokens join the image stream after the target's at RoPE positions
+        (1, r, c), and the output covers the target alone.
         skip_layers / skip_batch (skip-layer guidance): the last skip_batch sequences skip the listed joint blocks,
         both of their streams passing through them unchanged."""
         c = self.config
@@ -644,6 +675,8 @@ class MMDiT:
         B, H, W, Cl = x.shape
         if H % c.patch_size or W % c.patch_size:
             raise DkError("latent height/width must be divisible by the patch size")
+        if reference is not None:
+            self._check_reference(reference, B, Cl)
         text = token_level_text_embeddings
         if text.dim() == 4:
             text = text.squeeze(2)
@@ -664,31 +697,57 @@ class MMDiT:
         if self._mod_cur is None or B not in (self._mod_batch, lead):
             raise DkError(f"modulation cache holds batch {self._mod_batch}, forward got batch {B}")
         key = (B, H, W, Cl, T, skip_layers, skip_batch)
+        inputs = (x, text)
+        if reference is not None:
+            # the RoPE table, the workspaces and the graphs depend on the reference grid: part of the shape key
+            key += (tuple(reference.shape[1:3]),)
+            ref = reference.to(dtype=self.dtype)
+            inputs += (ref if ref.is_contiguous() else ref.contiguous(),)
         state = self._shapes.state(key, self.max_cached_shapes)
         state["skip"] = (frozenset(skip_layers), skip_batch)
+        state["ref_hw"] = tuple(reference.shape[1:3]) if reference is not None else None
         if self._step_cache is not None:
-            return self._cached_forward(state, key, x, text, B, H, W, Cl, T)
+            return self._cached_forward(state, key, inputs, B, H, W, Cl, T)
         return self._shapes.run(state, self.use_cuda_graphs,
-                                lambda xx, tt: self._forward_impl(state, xx, tt, B, H, W, Cl, T), x, text)
+                                lambda xx, tt, *rr: self._forward_impl(state, xx, tt, B, H, W, Cl, T, *rr), *inputs)
+
+    def _stream_rows(self, state, H, W) -> Tuple[int, int]:
+        """(target tokens Nx, image-stream rows N = Nx + Kontext reference tokens) per sequence"""
+        p, ref_hw = self.config.patch_size, state["ref_hw"]
+        Nx = (H // p) * (W // p)
+        return Nx, Nx + (0 if ref_hw is None else (ref_hw[0] // p) * (ref_hw[1] // p))
 
     def _geometry(self, state, B, H, W, T) -> dict:
-        """buffers and sizes of one input shape that the forward pieces below share"""
+        """buffers and sizes of one input shape that the forward pieces below share.  N is the image stream's length:
+        the target's Nx tokens, then a Kontext reference's (none without one: N = Nx)."""
         c = self.config
         hp, wp = H // c.patch_size, W // c.patch_size
-        N = hp * wp
-        g = {"B": B, "T": T, "N": N, "S": N + T, "hp": hp, "wp": wp, "ws": self._workspace(state, B, N, T),
+        Nx, N = self._stream_rows(state, H, W)
+        ref_hw = state["ref_hw"]
+        ref_grid = None if ref_hw is None else (ref_hw[0] // c.patch_size, ref_hw[1] // c.patch_size)
+        g = {"B": B, "T": T, "N": N, "Nx": Nx, "S": N + T, "hp": hp, "wp": wp, "ws": self._workspace(state, B, N, T),
              "w8": self._workspace8(state, B, N, T).get, "state": state,
              "skip_layers": state["skip"][0], "skip_batch": state["skip"][1]}
-        g["rope"] = self._rope_table(state, T, hp, wp) if c.pos_embed_type == PositionalEncoding.PreSDPARope else None
+        g["rope"] = (self._rope_table(state, T, hp, wp, ref_grid) if c.pos_embed_type == PositionalEncoding.PreSDPARope
+                     else None)
         # joint sequence order: FLUX [text, image] (mmdit.py:594-606), SD3 [image, text] (:608-625)
         g["off_img"], g["off_txt"], g["split"] = (T, 0, T) if self.is_flux else (0, N, N)
         return g
 
-    def _embed(self, g, x, text):
-        """input adapters (mmdit.py:195-206): text -> txt, latent -> img"""
+    def _embed(self, g, x, text, ref=None):
+        """input adapters (mmdit.py:195-206): text -> txt, latent -> img (and a Kontext reference -> its img rows)"""
         c, ws, state, N = self.config, g["ws"], g["state"], g["N"]
         ops.gemm(text, self.w_ctx, out=ws["txt"], bias=self.b_ctx)
-        if c.patchify_via_reshape:
+        if ref is not None:
+            # each sequence of img is [target Nx rows | reference N - Nx rows]; both embed through the output row remap
+            B, Nx = g["B"], g["Nx"]
+            rows_x, rows_r = ws["rows_in"][:B * Nx], ws["rows_in"][B * Nx:]
+            ops.patchify(x, 0, out=rows_x)
+            ops.gemm(rows_x, self.w_x, out=ws["img"], bias=self.b_x, rows_per_batch=Nx, out_batch_rows=N, out_row_off=0)
+            ops.patchify(ref, 0, out=rows_r)
+            ops.gemm(rows_r, self.w_x, out=ws["img"], bias=self.b_x, rows_per_batch=N - Nx, out_batch_rows=N,
+                     out_row_off=Nx)
+        elif c.patchify_via_reshape:
             ops.patchify(x, 0, out=ws["rows_in"])
             ops.gemm(ws["rows_in"], self.w_x, out=ws["img"], bias=self.b_x)
         else:
@@ -754,16 +813,22 @@ class MMDiT:
         ops.copy_rows(u, img, B, N, h, N, 0, S, T)                                     # image part (:245-247)
 
     def _final_layer(self, g, H, W, Cl):
-        """final layer (mmdit.py:780-796) on img + unpatchify / unpack"""
-        c, ws = self.config, g["ws"]
-        ops.ln_modulate(ws["img"], self._mod(self.final_mod_off, 0), self._mod(self.final_mod_off, 1), g["N"],
-                        c.layer_norm_eps, out=ws["m_img"])
-        ops.gemm(ws["m_img"], self.w_final, out=ws["rows_out"], bias=self.b_final)
-        return ops.unpatchify(ws["rows_out"], g["B"], H, W, Cl, 0 if c.patchify_via_reshape else 1)
+        """final layer (mmdit.py:780-796) on the target rows of img + unpatchify / unpack"""
+        c, ws, B, N, Nx = self.config, g["ws"], g["B"], g["N"], g["Nx"]
+        img, m_img, rows_out = ws["img"], ws["m_img"], ws["rows_out"]
+        if Nx != N:
+            # Kontext: the leading Nx rows of every N-row sequence (contiguous already for one sequence)
+            if B > 1:
+                img = ops.copy_rows(img, ws["o_img"], B, Nx, self.h, Nx, 0, N, 0)
+            img, m_img, rows_out = img[:B * Nx], m_img[:B * Nx], rows_out[:B * Nx]
+        ops.ln_modulate(img, self._mod(self.final_mod_off, 0), self._mod(self.final_mod_off, 1), Nx,
+                        c.layer_norm_eps, out=m_img)
+        ops.gemm(m_img, self.w_final, out=rows_out, bias=self.b_final)
+        return ops.unpatchify(rows_out, B, H, W, Cl, 0 if c.patchify_via_reshape else 1)
 
-    def _forward_impl(self, state, x, text, B, H, W, Cl, T):
+    def _forward_impl(self, state, x, text, B, H, W, Cl, T, ref=None):
         g = self._geometry(state, B, H, W, T)
-        self._embed(g, x, text)
+        self._embed(g, x, text, ref)
         for i in range(len(self.double)):
             self._double_block(g, i)
         self._single_blocks(g)
@@ -789,10 +854,10 @@ class MMDiT:
                        "host": torch.empty((B, 2), dtype=torch.float32, pin_memory=True)}
         return state["sc"]
 
-    def _head_impl(self, state, x, text, B, H, W, Cl, T):
+    def _head_impl(self, state, x, text, B, H, W, Cl, T, ref=None):
         g = self._geometry(state, B, H, W, T)
         sc, img, BN = state["sc"], g["ws"]["img"], B * g["N"]
-        self._embed(g, x, text)
+        self._embed(g, x, text, ref)
         ops.copy_rows(img, sc["snap"], 1, BN, self.h, BN, 0, BN, 0)                 # e
         self._double_block(g, 0)
         return ops.residual_delta(img, sc["snap"], B, g["N"], r_out=sc["r0"], prev=sc["r0prev"], sums=sc["sums"],
@@ -815,15 +880,15 @@ class MMDiT:
         ops.residual_apply(g["ws"]["img"], state["sc"]["R"], out=g["ws"]["img"])    # f = round16(a + R)
         return self._final_layer(g, H, W, Cl)
 
-    def _cached_forward(self, state, key, x, text, B, H, W, Cl, T):
+    def _cached_forward(self, state, key, inputs, B, H, W, Cl, T):
         policy = self._step_cache
         if key != self._step_cache_key:
             policy.reset()
             self._step_cache_key = key
-        sc = self._step_cache_buffers(state, B, (H // self.config.patch_size) * (W // self.config.patch_size))
+        sc = self._step_cache_buffers(state, B, self._stream_rows(state, H, W)[1])
         graphs = self.use_cuda_graphs
-        self._shapes.run(state, graphs, lambda xx, tt: self._head_impl(state, xx, tt, B, H, W, Cl, T), x, text,
-                         name="graph.head")
+        self._shapes.run(state, graphs, lambda xx, tt, *rr: self._head_impl(state, xx, tt, B, H, W, Cl, T, *rr),
+                         *inputs, name="graph.head")
         sc["host"].copy_(sc["sums"], non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()
         part = self._skip_impl if policy.step(sc["host"].tolist()) else self._tail_impl

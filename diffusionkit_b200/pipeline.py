@@ -17,6 +17,8 @@ Differences that are deliberate (documented in DESIGN.md):
     built with mmdit_config=FLUX_DEV; the reference loads dev without its guidance embedder (quirk Q1).
   * SD3.5 Medium (model_version "stabilityai/stable-diffusion-3.5-medium") and skip-layer guidance (`slg=` of
     DiffusionPipeline.generate_image / denoise_latents, any SD3-family model under CFG), DESIGN.md §13.
+  * FLUX.1 Kontext editing (model_version "black-forest-labs/FLUX.1-Kontext-dev"; `reference_image=` /
+    `reference_latents=` of FluxPipeline.generate_image / denoise_latents), DESIGN.md §14.
 """
 from __future__ import annotations
 
@@ -44,6 +46,7 @@ MMDIT_CKPT = {  # reference mlx/__init__.py:37-44
     "argmaxinc/mlx-FLUX.1-schnell-4bit-quantized": "argmaxinc/mlx-FLUX.1-schnell-4bit-quantized",
     "argmaxinc/mlx-FLUX.1-dev": "argmaxinc/mlx-FLUX.1-dev",
     "stabilityai/stable-diffusion-3.5-medium": "stabilityai/stable-diffusion-3.5-medium",
+    "black-forest-labs/FLUX.1-Kontext-dev": "black-forest-labs/FLUX.1-Kontext-dev",
 }
 
 # FLUX.1-dev's guidance when the caller passes none (BFL's default for the dev checkpoint)
@@ -91,6 +94,8 @@ class CFGDenoiser:
         self.model = model
         # skip-layer guidance of the running denoise: (SkipLayerGuidance, its steps, [pos | neg | pos] conditioning)
         self.slg = None
+        # FLUX.1 Kontext reference latent of the running denoise, one row per forward row (None: no reference)
+        self.reference = None
 
     def cache_modulation_params(self, pooled_text_embeddings, sigmas, guidance=None, skip_batch: int = 0):
         """guidance: one FLUX.1-dev guidance value per row of pooled (None without a guidance embedder).
@@ -118,13 +123,14 @@ class CFGDenoiser:
             skip = dict(skip_layers=self.slg[0].layers, skip_batch=B)
         xin = torch.empty((reps * B,) + tuple(x_t.shape[1:]), dtype=m.activation_dtype, device=x_t.device)
         ops.sampler_prepare(x_t, xin, reps)
-        out = m.mmdit(latent_image_embeddings=xin, token_level_text_embeddings=conditioning, timestep=timestep, **skip)
+        out = m.mmdit(latent_image_embeddings=xin, token_level_text_embeddings=conditioning, timestep=timestep,
+                      reference=self.reference, **skip)
         return xin, out
 
 
 def _start_sampling(model: CFGDenoiser, sigmas, extra_args):
     """What every sampler does first: the timesteps of the schedule (and, for FLUX.1-dev, the per-row guidance values
-    extra_args["guidance"]) into the modulation cache.
+    extra_args["guidance"]) into the modulation cache; a Kontext reference extra_args["reference"] onto the denoiser.
     -> (sigmas fp32, timesteps, conditioning, cfg_weight, events (one per sigma, the first recorded))"""
     extra_args = {} if extra_args is None else dict(extra_args)
     pipe = model.model
@@ -136,6 +142,7 @@ def _start_sampling(model: CFGDenoiser, sigmas, extra_args):
     cfg_weight = float(extra_args.get("cfg_weight", 0.0))
     conditioning = extra_args["conditioning"]
     slg = extra_args.pop("slg", None)
+    model.reference = extra_args.pop("reference", None)
     steps = skip_layer_guidance_steps(slg, len(sig) - 1) if slg is not None else []
     skip_batch = 0
     if steps:
@@ -153,6 +160,7 @@ def _finish_sampling(model: CFGDenoiser, events):
     """-> iter_time: seconds per step, from the events recorded after each step"""
     model.clear_cache()
     model.slg = None
+    model.reference = None
     torch.cuda.current_stream().synchronize()  # the reference syncs every step (mx.eval, :782); once is enough here
     return [round(events[i].elapsed_time(events[i + 1]) / 1e3, 3) for i in range(len(events) - 1)]
 
@@ -571,8 +579,45 @@ class DiffusionPipeline:
             raise ValueError(f"guidance must be finite, got {vals}")
         return vals
 
+    def _reference_input(self, reference_image, reference_latents, n_images: int):
+        """FluxPipeline's Kontext reference -> None, or (uint8 HWC image or fp32 latents, its (Hr, Wr) latent size).
+        Raises ValueError, before any GPU work, for a reference the pipeline cannot take."""
+        if reference_image is None and reference_latents is None:
+            return None
+        if reference_image is not None and reference_latents is not None:
+            raise ValueError("pass reference_image or reference_latents, not both")
+        if self.config.depth_unified == 0:
+            raise ValueError("a Kontext reference runs on FLUX-shaped configs only")
+        if reference_image is not None:
+            arr = self._load_image_u8(reference_image)
+            return arr, (arr.shape[0] // 8, arr.shape[1] // 8)
+        r = reference_latents
+        if not torch.is_tensor(r) or r.dtype != torch.float32 or r.dim() != 4 or r.shape[3] != 16:
+            raise ValueError("reference_latents must be an fp32 (1 or B, Hr, Wr, 16) latent in the process_in space, got "
+                             f"{tuple(r.shape) if torch.is_tensor(r) else type(r).__name__}"
+                             f"{' ' + str(r.dtype) if torch.is_tensor(r) else ''}")
+        Br, Hr, Wr = (int(v) for v in r.shape[:3])
+        if Br not in (1, n_images):
+            raise ValueError(f"reference_latents has batch {Br}: pass one reference, or one per seed ({n_images})")
+        if Hr % 2 or Wr % 2 or Hr == 0 or Wr == 0:
+            raise ValueError(f"reference latent height and width must be positive and even, got {Hr}x{Wr}")
+        return r, (Hr, Wr)
+
+    def _reference_latent(self, ref, rows: int) -> torch.Tensor:
+        """a checked Kontext reference -> the (rows, Hr, Wr, 16) activation-dtype latent every forward row takes.
+        An image is encoded once and represented by its posterior mean (zero noise), as diffusers' Kontext pipeline
+        does; BFL's reference code samples the posterior instead (DESIGN.md §14)."""
+        if isinstance(ref, np.ndarray):
+            hidden = self._encode_u8(ref)
+            zero = torch.zeros(tuple(hidden.shape[:3]) + (hidden.shape[3] // 2,), dtype=torch.float32,
+                               device=self.device)
+            lf = self.latent_format
+            ref = ops.vae_sample_latent(hidden, zero, lf.shift_factor, lf.scale_factor)
+        ref16 = ops.cast_to_16(ref.to(self.device).contiguous(), self.activation_dtype)
+        return ref16.repeat(rows // ref16.shape[0], 1, 1, 1)     # rows [positive x B | negative x B]
+
     def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
-                         denoise, *, noise, solver, guidance, slg=None):
+                         denoise, *, noise, solver, guidance, slg=None, reference_image=None, reference_latents=None):
         _check_solver(solver)
         _check_slg(slg, cfg_weight, self.config)
         if image_path is None:
@@ -588,6 +633,7 @@ class DiffusionPipeline:
             seeds = [int(seed)]
         B = len(seeds)
         guidance = self._guidance_values(guidance, B)
+        reference = self._reference_input(reference_image, reference_latents, B)
         H, W = latent_size
         conditioning = torch.as_tensor(conditioning).to(device=self.device, dtype=self.activation_dtype)
         pooled_conditioning = torch.as_tensor(pooled_conditioning).to(device=self.device, dtype=self.activation_dtype)
@@ -636,6 +682,8 @@ class DiffusionPipeline:
             extra_args["guidance"] = guidance * reps
         if slg is not None:
             extra_args["slg"] = slg
+        if reference is not None:
+            extra_args["reference"] = self._reference_latent(reference[0], reps * B)
         latent, iter_time = SOLVERS[solver](CFGDenoiser(self), x, sigmas, extra_args=extra_args)
         latent = ops.axpb(latent, 1.0 / self.latent_format.scale_factor, self.latent_format.shift_factor)  # process_out
         return latent, iter_time
@@ -665,10 +713,17 @@ class DiffusionPipeline:
                                     solver=solver, guidance=None, slg=slg)
 
     def _generate_image(self, text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
-                        denoise, *, conditioning, pooled_conditioning, solver, guidance, slg=None):
+                        denoise, *, conditioning, pooled_conditioning, solver, guidance, slg=None, reference_image=None,
+                        reference_latents=None):
         _check_solver(solver)
         _check_slg(slg, cfg_weight, self.config)
-        guidance = self._guidance_values(guidance, len(seed) if isinstance(seed, (list, tuple)) else 1)
+        n_images = len(seed) if isinstance(seed, (list, tuple)) else 1
+        guidance = self._guidance_values(guidance, n_images)
+        reference = self._reference_input(reference_image, reference_latents, n_images)
+        if reference is not None:                   # the checked image array goes on, so the file is read once
+            ref_kw = {"reference_image" if isinstance(reference[0], np.ndarray) else "reference_latents": reference[0]}
+        else:
+            ref_kw = {}
         assert latent_size[0] % 2 == 0, f"Height must be divisible by 16 ({latent_size[0]*8}/16={latent_size[0]/2})"
         assert latent_size[1] % 2 == 0, f"Width must be divisible by 16 ({latent_size[1]*8}/16={latent_size[1]/2})"
         self.check_and_load_models()
@@ -698,7 +753,7 @@ class DiffusionPipeline:
         log["denoising"]["pre"] = mem()
         latents, iter_time = self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight,
                                                    latent_size, seed, image_path, denoise, noise=None, solver=solver,
-                                                   guidance=guidance, slg=slg)
+                                                   guidance=guidance, slg=slg, **ref_kw)
         torch.cuda.synchronize(self.device)
         log["denoising"]["post"] = mem()
         log["denoising"]["time"] = round(time.time() - t0, 3)
@@ -710,6 +765,9 @@ class DiffusionPipeline:
             log["denoising"]["nfe"] = max(2 * n - 1, 0) if solver == "heun" else n
         if guidance is not None:
             log["denoising"]["guidance"] = guidance
+        if reference is not None:
+            Hr, Wr = reference[1]
+            log["denoising"]["reference"] = {"latent_size": (Hr, Wr), "tokens": (Hr // 2) * (Wr // 2)}
         if slg is not None:
             log["denoising"]["skip_layer_guidance"] = {
                 "scale": slg.scale, "layers": list(slg.layers),
@@ -797,9 +855,12 @@ class DiffusionPipeline:
         return (torch.from_numpy(arr[:, :, :3].astype(np.float32)) / 255 * 2 - 1.0).unsqueeze(0)
 
     def _encode_image_hidden(self, image_path) -> torch.Tensor:
+        return self._encode_u8(self._load_image_u8(image_path))
+
+    def _encode_u8(self, arr: np.ndarray) -> torch.Tensor:
+        """a _load_image_u8 array -> the VAE encoder's (1, H/8, W/8, 32) (mean | logvar)"""
         if not hasattr(self, "encoder"):
             self.load_encoder()
-        arr = self._load_image_u8(image_path)
         host = torch.from_numpy(arr).unsqueeze(0).pin_memory()
         return self.encoder(host.to(self.device, non_blocking=True))       # the /255*2-1 runs in dk_image_pre
 
@@ -869,22 +930,33 @@ class FluxPipeline(DiffusionPipeline):
     def denoise_latents(self, conditioning, pooled_conditioning, num_steps: int = 2, cfg_weight: float = 0.0,
                         latent_size: Tuple[int, int] = (64, 64), seed=None, image_path: Optional[str] = None,
                         denoise: float = 1.0, *, noise: Optional[torch.Tensor] = None, solver: str = "euler",
-                        guidance=None):
+                        guidance=None, reference_image=None, reference_latents: Optional[torch.Tensor] = None):
         """DiffusionPipeline.denoise_latents, plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
         float for every image or one per seed, and None means DEFAULT_GUIDANCE (3.5) when the model has a guidance
-        embedder (mmdit_config=FLUX_DEV).  A model without one refuses any value but None."""
+        embedder (mmdit_config=FLUX_DEV).  A model without one refuses any value but None.
+
+        FLUX.1 Kontext editing (DESIGN.md §14): `reference_image` (a path, a PIL image or a uint8 HWC RGB array, sides
+        cut to multiples of 64 like image_path) is encoded once by the VAE encoder into its posterior mean;
+        `reference_latents` is a device fp32 (1 or B, Hr, Wr, 16) latent already in the process_in space (B: one
+        reference per seed).  Every forward then sees the reference tokens after the target's; the result covers the
+        target alone.  Pass at most one of the two.  `image_path` still sets the target's starting point."""
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
-                                     image_path, denoise, noise=noise, solver=solver, guidance=guidance)
+                                     image_path, denoise, noise=noise, solver=solver, guidance=guidance,
+                                     reference_image=reference_image, reference_latents=reference_latents)
 
     def generate_image(self, text: str, num_steps: int = 2, cfg_weight: float = 0.0, negative_text: str = "",
                        latent_size: Tuple[int, int] = (64, 64), seed=None, verbose: bool = True,
                        image_path: Optional[str] = None, denoise: float = 1.0, *, conditioning=None,
-                       pooled_conditioning=None, solver: str = "euler", guidance=None):
-        """DiffusionPipeline.generate_image with `guidance` as in denoise_latents; with a guidance embedder the log
-        holds the value of each image under log["denoising"]["guidance"]."""
+                       pooled_conditioning=None, solver: str = "euler", guidance=None, reference_image=None,
+                       reference_latents: Optional[torch.Tensor] = None):
+        """DiffusionPipeline.generate_image with `guidance`, `reference_image` and `reference_latents` as in
+        denoise_latents; with a guidance embedder the log holds the value of each image under
+        log["denoising"]["guidance"], and with a reference its latent size and token count under
+        log["denoising"]["reference"]."""
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
-                                    solver=solver, guidance=guidance)
+                                    solver=solver, guidance=guidance, reference_image=reference_image,
+                                    reference_latents=reference_latents)
 
     def encode_text(self, text: str, cfg_weight: float = 7.5, negative_text: str = ""):
         """reference :642-671: CLIP-L pooled output + T5 sequence of the POSITIVE prompt only, T5 padded with zeros to
