@@ -8,8 +8,9 @@ DiffusionPipeline / FluxPipeline API (reference: argmaxinc/DiffusionKit, python/
                                      conditioning=cond, pooled_conditioning=pooled)
 """
 from ._lib import DkError  # noqa: F401
-from .config import (FLUX_DEV, FLUX_SCHNELL, SD3_2b, SD3_8b, SD35_MEDIUM, MMDiTConfig, VAEDecoderConfig,  # noqa: F401
-                     VAEEncoderConfig)
+from .config import (FLUX_DEV, FLUX_SCHNELL, SD3_2b, SD3_8b, SD35_MEDIUM, SIGLIP_SO400M_PATCH14_384,  # noqa: F401
+                     MMDiTConfig, SiglipVisionConfig, VAEDecoderConfig, VAEEncoderConfig)
+from .image_encoders import ReduxImageEncoder, SiglipVisionModel  # noqa: F401
 from .lora import LoRA, load_lora  # noqa: F401
 from .mmdit import MMDiT  # noqa: F401
 from .pipeline import (CFGDenoiser, DiffusionPipeline, FluxLatentFormat, FluxPipeline, LatentFormat,  # noqa: F401

@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "libdkb200.so")
 HEADER_PATH = os.path.join(_HERE, "..", "include", "dkb200.h")
 
 DK_BF16, DK_FP16 = 0, 1
-ACT_NONE, ACT_GELU_ERF, ACT_SILU, ACT_QUICK_GELU = 0, 1, 2, 3
+ACT_NONE, ACT_GELU_ERF, ACT_SILU, ACT_QUICK_GELU, ACT_GELU_TANH = 0, 1, 2, 3, 4
 
 vp = C.c_void_p
 i32 = C.c_int
@@ -80,6 +80,7 @@ SIGNATURES = {
     "dk_attention_small": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, i32, f32, i32, vp]),
     "dk_dequant_q4": (i32, [vp, i32, vp, vp, vp, vp, i64, i32, i32, vp]),
     "dk_image_pre": (i32, [vp, i32, vp, vp, i64, i32, i32, vp]),
+    "dk_image_patches": (i32, [vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
     "dk_axpby_f32": (i32, [vp, vp, vp, vp, i64, f32, f32, vp]),
     "dk_vae_sample_latent": (i32, [vp, i32, vp, vp, vp, i64, i32, f32, f32, vp]),
     "dk_cast_f32_to_16": (i32, [vp, i32, vp, vp, i64, vp]),

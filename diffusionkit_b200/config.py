@@ -199,6 +199,39 @@ class T5EncoderConfig:
     feed_forward_proj: str = "gated-gelu"
 
 
+@dataclass
+class SiglipVisionConfig:
+    """The fields of transformers.SiglipVisionConfig the FLUX.1 Redux image encoder reads (DESIGN.md §15)."""
+
+    hidden_size: int = 1152
+    num_attention_heads: int = 16
+    intermediate_size: int = 4304
+    num_hidden_layers: int = 27
+    patch_size: int = 14
+    image_size: int = 384
+    layer_norm_eps: float = 1e-6
+    hidden_act: str = "gelu_pytorch_tanh"
+
+    @property
+    def head_dim(self) -> int:
+        return self.hidden_size // self.num_attention_heads
+
+    @property
+    def num_patches(self) -> int:
+        """tokens per image: the stride-p convolution without padding drops image_size % patch_size pixels"""
+        return (self.image_size // self.patch_size) ** 2
+
+
+# google/siglip-so400m-patch14-384, the vision tower of BFL's FLUX.1 Redux [dev] (prepare_redux)
+SIGLIP_SO400M_PATCH14_384 = SiglipVisionConfig()
+
+
+def tiny_siglip_config(image_size: int = 98, layers: int = 2) -> SiglipVisionConfig:
+    """Small SigLIP for tests: 2 heads of SigLIP's head dim 72, so the attention padding is exercised."""
+    return SiglipVisionConfig(hidden_size=144, num_attention_heads=2, intermediate_size=304, num_hidden_layers=layers,
+                              image_size=image_size)
+
+
 def tiny_clip_config(projection: bool = True, act: str = "quick_gelu") -> CLIPTextModelConfig:
     return CLIPTextModelConfig(num_layers=3, model_dims=128, num_heads=2, max_length=77, vocab_size=1000,
                                projection_dim=64 if projection else None, hidden_act=act)

@@ -298,6 +298,13 @@ __device__ __forceinline__ float quick_gelu_f(float v) {
   return __fdividef(v, 1.0f + e);
 }
 
+// 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))): torch's gelu(approximate="tanh"), SigLIP's "gelu_pytorch_tanh".
+// The accurate tanhf, not tanh.approx.f32 (relative error about 2^-11), like torch's fp32 tanh.
+__device__ __forceinline__ float gelu_tanh_f(float v) {
+  const float inner = 0.7978845608028654f * (v + 0.044715f * v * v * v);
+  return 0.5f * v * (1.0f + tanhf(inner));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

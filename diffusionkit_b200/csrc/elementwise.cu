@@ -310,7 +310,12 @@ __global__ void act_kernel(const T* __restrict__ x, T* __restrict__ y, long long
     float a[8];
     load8(x + i * 8, a);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) a[j] = act == DK_ACT_SILU ? silu_f(a[j]) : (act == DK_ACT_GELU_ERF ? gelu_erf(a[j]) : (act == DK_ACT_QUICK_GELU ? quick_gelu_f(a[j]) : a[j]));
+    for (int j = 0; j < 8; ++j)
+      a[j] = act == DK_ACT_SILU ? silu_f(a[j])
+             : act == DK_ACT_GELU_ERF ? gelu_erf(a[j])
+             : act == DK_ACT_QUICK_GELU ? quick_gelu_f(a[j])
+             : act == DK_ACT_GELU_TANH ? gelu_tanh_f(a[j])
+             : a[j];
     store8(y + i * 8, a);
   }
 }
@@ -506,8 +511,14 @@ __global__ void dequant_q4_kernel(const uint32_t* __restrict__ wq, const T* __re
   }
 }
 
+// u8 / 255 * 2 - 1 as three separately rounded fp32 ops like the reference's (x / 255) * 2 - 1 (no FMA contraction);
+// it is also SigLIP's (x / 255 - 0.5) / 0.5.  dk_image_pre and dk_image_patches both normalise through it.
+__device__ __forceinline__ float u8_to_unit(uint8_t u) {
+  return __fsub_rn(__fmul_rn(__fdiv_rn(static_cast<float>(u), 255.f), 2.f), 1.f);
+}
+
 // read_image (reference mlx/__init__.py:536-551): uint8 [pixels, src_c >= 3] -> 16-bit [pixels, cpad], channels 0..2 =
-// u8 / 255 * 2 - 1 (fp32 arithmetic, then rounded to T), channels 3.. = 0 (the tensor-core conv wants Cin % 64 == 0)
+// u8_to_unit (fp32 arithmetic, then rounded to T), channels 3.. = 0 (the tensor-core conv wants Cin % 64 == 0)
 template <typename T>
 __global__ void image_pre_kernel(const uint8_t* __restrict__ img, T* __restrict__ out, long long pixels, int src_c,
                                  int cpad) {
@@ -520,14 +531,41 @@ __global__ void image_pre_kernel(const uint8_t* __restrict__ img, T* __restrict_
     uint4 w = make_uint4(0u, 0u, 0u, 0u);
     if (v == 0) {
       const uint8_t* px = img + p * src_c;
-      // three separately rounded fp32 ops like the reference's (x / 255) * 2 - 1 (no FMA contraction)
-      const float r = __fsub_rn(__fmul_rn(__fdiv_rn(static_cast<float>(px[0]), 255.f), 2.f), 1.f);
-      const float g = __fsub_rn(__fmul_rn(__fdiv_rn(static_cast<float>(px[1]), 255.f), 2.f), 1.f);
-      const float b = __fsub_rn(__fmul_rn(__fdiv_rn(static_cast<float>(px[2]), 255.f), 2.f), 1.f);
-      w.x = Half16<T>::pack(r, g);
-      w.y = Half16<T>::pack(b, 0.f);
+      w.x = Half16<T>::pack(u8_to_unit(px[0]), u8_to_unit(px[1]));
+      w.y = Half16<T>::pack(u8_to_unit(px[2]), 0.f);
     }
     *reinterpret_cast<uint4*>(out + p * cpad + v * 8) = w;
+  }
+}
+
+// Patch rows of a stride-p, p x p, unpadded convolution (SigLIP's patch embedding): uint8 NHWC [B, H, W, src_c >= 3] ->
+// 16-bit [B * (H / p) * (W / p), kp].  Column k < 3p^2 of the row of patch (hp, wp) is u8_to_unit of channel k % 3 of
+// pixel (hp * p + k / (3p), wp * p + (k / 3) % p), i.e. (kh, kw, c) order; columns 3p^2.. are zero.  The floor of H / p
+// and W / p drops the last pixel rows and columns, as the convolution does.  One thread per 8-column vector.
+template <typename T>
+__global__ void image_patches_kernel(const uint8_t* __restrict__ img, T* __restrict__ out, int B, int H, int W,
+                                     int src_c, int p, int kp) {
+  const int hp_n = H / p, wp_n = W / p, vpr = kp / 8, kreal = 3 * p * p;
+  const long long nvec = static_cast<long long>(B) * hp_n * wp_n * vpr;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long row = i / vpr;
+    const int v = static_cast<int>(i - row * vpr);
+    const int wp = static_cast<int>(row % wp_n);
+    const int hp = static_cast<int>((row / wp_n) % hp_n);
+    const int b = static_cast<int>(row / (static_cast<long long>(wp_n) * hp_n));
+    float o[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = v * 8 + j;
+      o[j] = 0.f;
+      if (k < kreal) {
+        const int kh = k / (3 * p), kw = (k / 3) % p, c = k % 3;
+        const long long px = (static_cast<long long>(b) * H + hp * p + kh) * W + wp * p + kw;
+        o[j] = u8_to_unit(img[px * src_c + c]);
+      }
+    }
+    store8(out + row * kp + v * 8, o);
   }
 }
 __global__ void axpby_kernel(const float* __restrict__ x, const float* __restrict__ y, float* __restrict__ o,
@@ -1303,6 +1341,24 @@ extern "C" int dk_image_pre(dk_ctx* ctx, int dtype, const uint8_t* img, void* ou
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DK_DISPATCH(dtype, (image_pre_kernel<T><<<dk_grid_for(pixels * (cpad / 8), 256, ctx->sm_count), 256, 0, stream>>>(
                          img, static_cast<T*>(out), pixels, src_channels, cpad)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_image_patches(dk_ctx* ctx, int dtype, const uint8_t* img, void* out, int B, int H, int W,
+                                int src_channels, int p, int kp, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(src_channels >= 3, "dk_image_patches: image needs at least 3 channels (got %d)", src_channels);
+  DK_REQUIRE(B > 0 && p > 0 && H >= p && W >= p, "dk_image_patches: image %dx%d (batch %d) has no %dx%d patch", H, W, B,
+             p, p);
+  DK_REQUIRE(kp % 8 == 0 && kp >= 3 * p * p, "dk_image_patches: kp (%d) must be a multiple of 8 and >= 3p^2 (%d)", kp,
+             3 * p * p);
+  DK_REQUIRE(dk_aligned16(out), "dk_image_patches: out must be 16-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long nvec = static_cast<long long>(B) * (H / p) * (W / p) * (kp / 8);
+  DK_DISPATCH(dtype, (image_patches_kernel<T><<<dk_grid_for(nvec, 256, ctx->sm_count), 256, 0, stream>>>(
+                         img, static_cast<T*>(out), B, H, W, src_channels, p, kp)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }

@@ -82,8 +82,9 @@ __device__ __forceinline__ void cluster_tile(int ct, const GemmShape& s, uint32_
 // B_MN: W operand given as [K, N] row-major (MN-major wgmma operand, transposed B).
 // T: 16-bit type of the epilogue's operands and of out.  E: element of A and W, T itself or E4m3 (K-major only,
 // MODE 0 only; the epilogue then applies the row and column scales).
+// GELU_TANH: the instance whose epilogue has the DK_ACT_GELU_TANH case (gemm_epilogue_tile).
 // Launched in clusters of 2 along x with an even grid of at most (resident clusters) x 2 CTAs.
-template <typename T, int BN, bool B_MN, int MODE, typename E>
+template <typename T, int BN, bool B_MN, int MODE, typename E, bool GELU_TANH>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmShape s,
                   const GemmEpi e, const ConvGeom g) {
@@ -226,7 +227,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         mbar_arrive_cluster(&empty_bar[prev], 0);
         mbar_arrive_cluster(&empty_bar[prev], 1);
       }
-      gemm_epilogue_tile<T, BN, MODE, FP8>(acc, s, e, g, m_blk, n_blk, cw, stg + cw * (Cfg::EPI_BYTES / 2), rstd + cw * 128);
+      gemm_epilogue_tile<T, BN, MODE, FP8, GELU_TANH>(acc, s, e, g, m_blk, n_blk, cw, stg + cw * (Cfg::EPI_BYTES / 2),
+                                                      rstd + cw * 128);
     }
   }
   // no CTA may leave while its partner can still multicast into its shared memory or arrive on its barriers
@@ -236,11 +238,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-template <typename T, int BN, bool B_MN, int MODE, typename E = T>
+template <typename T, int BN, bool B_MN, int MODE, typename E = T, bool GELU_TANH = false>
 static int launch_gemm_inst(const char* fn, dk_ctx* ctx, const CUtensorMap& tmA, const CUtensorMap& tmB,
                             const GemmShape& s, const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_wgmma_kernel<T, BN, B_MN, MODE, E>;
+  auto kern = gemm_wgmma_kernel<T, BN, B_MN, MODE, E, GELU_TANH>;
   cudaLaunchAttribute cluster;
   cluster.id = cudaLaunchAttributeClusterDimension;
   cluster.val.clusterDim.x = CLUSTER;
@@ -269,12 +271,12 @@ static int launch_gemm_inst(const char* fn, dk_ctx* ctx, const CUtensorMap& tmA,
   return 0;
 }
 
-template <typename T, bool B_MN, int MODE, typename E = T>
+template <typename T, bool B_MN, int MODE, typename E = T, bool GELU_TANH = false>
 static int launch_gemm_bn(const char* fn, dk_ctx* ctx, int bn, const CUtensorMap& tmA, const CUtensorMap& tmB,
                           const GemmShape& s, const GemmEpi& e, const ConvGeom& g, cudaStream_t stream) {
-  if (bn == 256) return launch_gemm_inst<T, 256, B_MN, MODE, E>(fn, ctx, tmA, tmB, s, e, g, stream);
-  if (bn == 128) return launch_gemm_inst<T, 128, B_MN, MODE, E>(fn, ctx, tmA, tmB, s, e, g, stream);
-  return launch_gemm_inst<T, 64, B_MN, MODE, E>(fn, ctx, tmA, tmB, s, e, g, stream);
+  if (bn == 256) return launch_gemm_inst<T, 256, B_MN, MODE, E, GELU_TANH>(fn, ctx, tmA, tmB, s, e, g, stream);
+  if (bn == 128) return launch_gemm_inst<T, 128, B_MN, MODE, E, GELU_TANH>(fn, ctx, tmA, tmB, s, e, g, stream);
+  return launch_gemm_inst<T, 64, B_MN, MODE, E, GELU_TANH>(fn, ctx, tmA, tmB, s, e, g, stream);
 }
 
 // Tile-N choice: 256 wide tiles keep the shared-memory operand traffic per MMA lowest; fall back to narrower tiles
@@ -349,6 +351,8 @@ static int gemm_impl(const char* fn, dk_ctx* ctx, const dk_gemm_args* a, const f
                "%s: fused QK epilogue excludes act/gate/residual", fn);
     DK_REQUIRE(a->qk_rope == nullptr || dk_aligned16(a->qk_rope), "%s: rope table alignment", fn);
   }
+  DK_REQUIRE(a->act != DK_ACT_GELU_TANH || (!fp8 && !a->w_n_major),
+             "%s: the tanh-GELU epilogue runs on 16-bit K-major operands only", fn);
   ConvGeom g = {};
 
   CUtensorMap tmA, tmB;
@@ -373,6 +377,7 @@ static int gemm_impl(const char* fn, dk_ctx* ctx, const dk_gemm_args* a, const f
   DK_DISPATCH(a->dtype, {
     if (fp8) return launch_gemm_bn<T, false, 0, E4m3>(fn, ctx, bn, tmA, tmB, s, e, g, stream);
     if (a->w_n_major) return launch_gemm_inst<T, 128, true, 0>(fn, ctx, tmA, tmB, s, e, g, stream);
+    if (a->act == DK_ACT_GELU_TANH) return launch_gemm_bn<T, false, 0, T, true>(fn, ctx, bn, tmA, tmB, s, e, g, stream);
     return launch_gemm_bn<T, false, 0>(fn, ctx, bn, tmA, tmB, s, e, g, stream);
   });
 }

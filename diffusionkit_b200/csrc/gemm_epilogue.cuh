@@ -1,5 +1,6 @@
 // Shared pieces of the wgmma GEMM kernel: problem/epilogue descriptors and the accumulator -> global
-// epilogue (bias / GELU-erf / SiLU / adaLN gate / residual, or QK-RMSNorm + RoPE on a packed QKV projection).
+// epilogue (bias / GELU-erf / SiLU / quick-GELU / tanh-GELU / adaLN gate / residual, or QK-RMSNorm + RoPE on a packed
+// QKV projection).
 #pragma once
 
 #include "common.cuh"
@@ -90,7 +91,10 @@ __device__ __forceinline__ uint32_t ld_u32(const T* p) {
 // Per element the fp32 order is that of the reference: bias, activation, gate, residual, one rounding; the QK path
 // rounds (acc + bias) to 16 bits for the head's sum of squares, which one thread per (row, head) adds in column order.
 // SCALED (e4m3 operands): "acc" above is the accumulator times a_scale[row] * w_scale[column].
-template <typename T, int BN, int MODE, bool SCALED>
+// GELU_TANH: the instances that can apply DK_ACT_GELU_TANH (SigLIP's fc1).  The inlined tanhf makes the kernel a fifth
+// larger; with the case in every instance, bench.py's FLUX.1-schnell images/s measured 1.5 % lower on an H100, so the
+// other instances leave it out and compile to the code they had without it.
+template <typename T, int BN, int MODE, bool SCALED, bool GELU_TANH = false>
 __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], const GemmShape& s, const GemmEpi& e,
                                                    const ConvGeom& g, int m_blk, int n_blk, int cw, uint8_t* stg,
                                                    float* rstd) {
@@ -343,6 +347,11 @@ __device__ __forceinline__ void gemm_epilogue_tile(const float (&acc)[BN / 2], c
           for (int u = 0; u < G; ++u)
 #pragma unroll
             for (int k = 0; k < 4; ++k) v[u][k >> 1][k & 1] = quick_gelu_f(v[u][k >> 1][k & 1]);
+        } else if (GELU_TANH && e.act == DK_ACT_GELU_TANH) {
+#pragma unroll
+          for (int u = 0; u < G; ++u)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) v[u][k >> 1][k & 1] = gelu_tanh_f(v[u][k >> 1][k & 1]);
         }
         if (gate != nullptr) {
 #pragma unroll

@@ -352,3 +352,54 @@ def check_against_specs(params: Dict[str, Tensor], specs: Iterable[Tuple[str, Tu
     if missing or extra or bad:
         raise ValueError(f"checkpoint does not match the model: missing {missing[:5]} (+{max(0, len(missing) - 5)}), "
                          f"unexpected {extra[:5]} (+{max(0, len(extra) - 5)}), wrong shape {bad[:5]}")
+
+
+# ------------------------------------------------------------------------------------------------ FLUX.1 Redux
+_SIGLIP_DROPPED = ("text_model.", "logit_scale", "logit_bias", "vision_model.head.", "head.")
+
+
+def siglip_checkpoint_to_params(sd: Dict[str, Tensor], config=None) -> Dict[str, Tensor]:
+    """Hugging Face SigLIP safetensors -> the engine's SiglipVisionModel tree (image_encoders.pack_siglip_params).
+    Takes the full SiglipModel file (`vision_model.*` beside `text_model.*`, `logit_scale`, `logit_bias`) or a
+    vision-only export (with or without the `vision_model.` prefix).  The text tower, the logit scalars and the pooling
+    head (`vision_model.head.*`, not part of last_hidden_state) are dropped; the `position_ids` buffer older exports carry
+    is skipped.  A missing key, an unexpected one or a wrong shape raises ValueError naming it.  config: a
+    SiglipVisionConfig (default google/siglip-so400m-patch14-384)."""
+    from .config import SIGLIP_SO400M_PATCH14_384
+    from .image_encoders import pack_siglip_params, siglip_param_specs
+
+    cfg = config if config is not None else SIGLIP_SO400M_PATCH14_384
+    out: Dict[str, Tensor] = {}
+    for key, v in sd.items():
+        if key.startswith(_SIGLIP_DROPPED) or key.endswith("position_ids"):
+            continue
+        out[key[len("vision_model."):] if key.startswith("vision_model.") else key] = v
+    want = {n: tuple(s) for n, s, _ in siglip_param_specs(cfg)}
+    for n, s in want.items():
+        if n not in out:
+            raise ValueError(f"SigLIP checkpoint: missing vision_model.{n}")
+        if tuple(out[n].shape) != s:
+            raise ValueError(f"SigLIP checkpoint: vision_model.{n} has shape {tuple(out[n].shape)}, expected {s}")
+    extra = sorted(set(out) - set(want))
+    if extra:
+        raise ValueError(f"SigLIP checkpoint: unexpected keys {extra[:5]} (+{max(0, len(extra) - 5)})")
+    return pack_siglip_params(out, cfg)
+
+
+def redux_checkpoint_to_params(sd: Dict[str, Tensor], token_level_text_embed_dim: int = 4096,
+                               siglip_hidden: int = 1152) -> Dict[str, Tensor]:
+    """BFL `flux1-redux-dev.safetensors` (redux_up / redux_down .weight / .bias) -> ReduxImageEncoder's tree, the same
+    names.  Shapes are checked against the FLUX config's token_level_text_embed_dim and the SigLIP width; a missing,
+    unexpected or misshaped key raises ValueError naming it."""
+    from .image_encoders import redux_param_specs
+
+    want = {n: tuple(s) for n, s, _ in redux_param_specs(siglip_hidden, token_level_text_embed_dim)}
+    for n, s in want.items():
+        if n not in sd:
+            raise ValueError(f"Redux checkpoint: missing {n}")
+        if tuple(sd[n].shape) != s:
+            raise ValueError(f"Redux checkpoint: {n} has shape {tuple(sd[n].shape)}, expected {s}")
+    extra = sorted(set(sd) - set(want))
+    if extra:
+        raise ValueError(f"Redux checkpoint: unexpected keys {extra}")
+    return {n: sd[n] for n in want}

@@ -19,6 +19,8 @@ Differences that are deliberate (documented in DESIGN.md):
     DiffusionPipeline.generate_image / denoise_latents, any SD3-family model under CFG), DESIGN.md §13.
   * FLUX.1 Kontext editing (model_version "black-forest-labs/FLUX.1-Kontext-dev"; `reference_image=` /
     `reference_latents=` of FluxPipeline.generate_image / denoise_latents), DESIGN.md §14.
+  * FLUX.1 Redux image prompts (FluxPipeline.load_redux / encode_redux, `redux_image=` of generate_image /
+    denoise_latents): SigLIP + Redux tokens appended to the T5 sequence, DESIGN.md §15.
 """
 from __future__ import annotations
 
@@ -616,8 +618,69 @@ class DiffusionPipeline:
         ref16 = ops.cast_to_16(ref.to(self.device).contiguous(), self.activation_dtype)
         return ref16.repeat(rows // ref16.shape[0], 1, 1, 1)     # rows [positive x B | negative x B]
 
+    def _redux_input(self, redux_image, cfg_weight: float, n_images: int):
+        """FluxPipeline's `redux_image` -> None, or the list of 1 or n_images uint8 (S, S, 3) host arrays to encode.
+        Raises, before any GPU work, for an image prompt the pipeline cannot take."""
+        if redux_image is None:
+            return None
+        if cfg_weight > 0:
+            raise ValueError("redux_image needs cfg_weight == 0: every row of a batch shares one text length and there is "
+                             "no attention mask, so a negative row without image tokens cannot run beside it")
+        self._need_redux()
+        if not isinstance(redux_image, (list, tuple)):
+            redux_image = [redux_image]
+        elif len(redux_image) != n_images:
+            raise ValueError(f"redux_image has {len(redux_image)} images for {n_images} seed(s): pass one image, or a "
+                             "list with one per seed")
+        return [self._redux_image_u8(im) for im in redux_image]
+
+    def _need_redux(self):
+        missing = [n for n in ("siglip", "redux") if getattr(self, n, None) is None]
+        if missing:
+            raise DkError(
+                f"redux_image needs {', '.join(missing)}: call load_redux(...) with local weights first (nothing can be "
+                "downloaded here), or pass `conditioning` with the image tokens appended")
+
+    def _redux_image_u8(self, image) -> np.ndarray:
+        """a path, PIL image or uint8 (H, W), (H, W, 3) or (H, W, 4) array -> uint8 (S, S, 3), S = the SigLIP image
+        size: converted to RGB as BFL does, resized with PIL bicubic to exactly S x S (aspect ratio not kept,
+        reducing_gap=None), as the SigLIP image processor BFL calls resizes"""
+        from PIL import Image
+
+        if isinstance(image, (str, bytes)) or hasattr(image, "__fspath__"):
+            image = Image.open(image)
+        if isinstance(image, np.ndarray):
+            if image.dtype != np.uint8 or not (image.ndim == 2 or (image.ndim == 3 and image.shape[2] in (3, 4))):
+                raise ValueError(f"redux_image array must be uint8 (H, W), (H, W, 3) or (H, W, 4), got {image.dtype} "
+                                 f"{image.shape}")
+            image = Image.fromarray(image)
+        S = self.siglip.config.image_size
+        image = image.convert("RGB").resize((S, S), Image.BICUBIC, reducing_gap=None)
+        return np.ascontiguousarray(np.asarray(image))
+
+    def _redux_tokens(self, arrs, out: torch.Tensor, T: int):
+        """SigLIP + Redux of the n checked host images, one batch: image i's tokens go to rows [T, T + tokens) of
+        sequence i of out (>= n, T + tokens, txt_dim)"""
+        host = torch.from_numpy(np.stack(arrs)).pin_memory()
+        h = self.siglip(host.to(self.device, non_blocking=True))
+        P = h.shape[1]
+        self.redux(h.reshape(-1, h.shape[2]), P, out=out.view(-1, out.shape[2]), out_seq_rows=T + P, out_row_off=T)
+
+    def _redux_conditioning(self, conditioning: torch.Tensor, arrs) -> torch.Tensor:
+        """(B, T, E) conditioning + checked images -> (B, T + tokens, E): each sequence's T5 rows, then its image's
+        tokens (BFL's txt = cat(txt, img_cond)); one shared image is encoded once and its tokens copied"""
+        B, T, E = conditioning.shape
+        P = self.siglip.config.num_patches
+        out = torch.empty((B, T + P, E), dtype=self.activation_dtype, device=self.device)
+        ops.copy_rows(conditioning.contiguous(), out, B, T, E, T + P, 0, T, 0)
+        self._redux_tokens(arrs, out, T)
+        if len(arrs) < B:
+            ops.copy_rows(out, out, B - 1, P, E, T + P, T + P + T, 0, T)
+        return out
+
     def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
-                         denoise, *, noise, solver, guidance, slg=None, reference_image=None, reference_latents=None):
+                         denoise, *, noise, solver, guidance, slg=None, reference_image=None, reference_latents=None,
+                         redux_image=None, redux_log=None):
         _check_solver(solver)
         _check_slg(slg, cfg_weight, self.config)
         if image_path is None:
@@ -634,6 +697,7 @@ class DiffusionPipeline:
         B = len(seeds)
         guidance = self._guidance_values(guidance, B)
         reference = self._reference_input(reference_image, reference_latents, B)
+        redux = self._redux_input(redux_image, cfg_weight, B)
         H, W = latent_size
         conditioning = torch.as_tensor(conditioning).to(device=self.device, dtype=self.activation_dtype)
         pooled_conditioning = torch.as_tensor(pooled_conditioning).to(device=self.device, dtype=self.activation_dtype)
@@ -649,6 +713,13 @@ class DiffusionPipeline:
             raise DkError(
                 f"conditioning has batch {conditioning.shape[0]}, expected {reps * B} "
                 f"({'[positive | negative] x ' if reps == 2 else ''}{B} image(s)) for cfg_weight={cfg_weight}")
+        if redux is not None:
+            t0 = time.time()
+            conditioning = self._redux_conditioning(conditioning, redux)
+            if redux_log is not None:
+                torch.cuda.synchronize(self.device)
+                redux_log.update(images=len(redux), tokens=self.siglip.config.num_patches,
+                                 time=round(time.time() - t0, 3))
 
         hidden = None
         if image_path is not None:
@@ -714,12 +785,13 @@ class DiffusionPipeline:
 
     def _generate_image(self, text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                         denoise, *, conditioning, pooled_conditioning, solver, guidance, slg=None, reference_image=None,
-                        reference_latents=None):
+                        reference_latents=None, redux_image=None):
         _check_solver(solver)
         _check_slg(slg, cfg_weight, self.config)
         n_images = len(seed) if isinstance(seed, (list, tuple)) else 1
         guidance = self._guidance_values(guidance, n_images)
         reference = self._reference_input(reference_image, reference_latents, n_images)
+        redux = self._redux_input(redux_image, cfg_weight, n_images)   # the checked 384^2 arrays go on: read once
         if reference is not None:                   # the checked image array goes on, so the file is read once
             ref_kw = {"reference_image" if isinstance(reference[0], np.ndarray) else "reference_latents": reference[0]}
         else:
@@ -751,9 +823,12 @@ class DiffusionPipeline:
         torch.cuda.reset_peak_memory_stats(self.device)
         t0 = time.time()
         log["denoising"]["pre"] = mem()
+        redux_log = {}
         latents, iter_time = self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight,
                                                    latent_size, seed, image_path, denoise, noise=None, solver=solver,
-                                                   guidance=guidance, slg=slg, **ref_kw)
+                                                   guidance=guidance, slg=slg, redux_log=redux_log,
+                                                   redux_image=redux if redux is None or len(redux) == n_images
+                                                   else redux[0], **ref_kw)
         torch.cuda.synchronize(self.device)
         log["denoising"]["post"] = mem()
         log["denoising"]["time"] = round(time.time() - t0, 3)
@@ -768,6 +843,8 @@ class DiffusionPipeline:
         if reference is not None:
             Hr, Wr = reference[1]
             log["denoising"]["reference"] = {"latent_size": (Hr, Wr), "tokens": (Hr // 2) * (Wr // 2)}
+        if redux is not None:
+            log["denoising"]["redux"] = redux_log
         if slg is not None:
             log["denoising"]["skip_layer_guidance"] = {
                 "scale": slg.scale, "layers": list(slg.layers),
@@ -930,7 +1007,8 @@ class FluxPipeline(DiffusionPipeline):
     def denoise_latents(self, conditioning, pooled_conditioning, num_steps: int = 2, cfg_weight: float = 0.0,
                         latent_size: Tuple[int, int] = (64, 64), seed=None, image_path: Optional[str] = None,
                         denoise: float = 1.0, *, noise: Optional[torch.Tensor] = None, solver: str = "euler",
-                        guidance=None, reference_image=None, reference_latents: Optional[torch.Tensor] = None):
+                        guidance=None, reference_image=None, reference_latents: Optional[torch.Tensor] = None,
+                        redux_image=None):
         """DiffusionPipeline.denoise_latents, plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
         float for every image or one per seed, and None means DEFAULT_GUIDANCE (3.5) when the model has a guidance
         embedder (mmdit_config=FLUX_DEV).  A model without one refuses any value but None.
@@ -939,24 +1017,66 @@ class FluxPipeline(DiffusionPipeline):
         cut to multiples of 64 like image_path) is encoded once by the VAE encoder into its posterior mean;
         `reference_latents` is a device fp32 (1 or B, Hr, Wr, 16) latent already in the process_in space (B: one
         reference per seed).  Every forward then sees the reference tokens after the target's; the result covers the
-        target alone.  Pass at most one of the two.  `image_path` still sets the target's starting point."""
+        target alone.  Pass at most one of the two.  `image_path` still sets the target's starting point.
+
+        FLUX.1 Redux image prompt (DESIGN.md §15, after load_redux): `redux_image` is one image for every seed or a list
+        with one per seed (each as encode_redux takes it).  It is encoded once per call, and its tokens are appended to
+        each image's conditioning rows, which then hold T + tokens rows.  Needs cfg_weight == 0."""
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
                                      image_path, denoise, noise=noise, solver=solver, guidance=guidance,
-                                     reference_image=reference_image, reference_latents=reference_latents)
+                                     reference_image=reference_image, reference_latents=reference_latents,
+                                     redux_image=redux_image)
 
     def generate_image(self, text: str, num_steps: int = 2, cfg_weight: float = 0.0, negative_text: str = "",
                        latent_size: Tuple[int, int] = (64, 64), seed=None, verbose: bool = True,
                        image_path: Optional[str] = None, denoise: float = 1.0, *, conditioning=None,
                        pooled_conditioning=None, solver: str = "euler", guidance=None, reference_image=None,
-                       reference_latents: Optional[torch.Tensor] = None):
-        """DiffusionPipeline.generate_image with `guidance`, `reference_image` and `reference_latents` as in
-        denoise_latents; with a guidance embedder the log holds the value of each image under
-        log["denoising"]["guidance"], and with a reference its latent size and token count under
-        log["denoising"]["reference"]."""
+                       reference_latents: Optional[torch.Tensor] = None, redux_image=None):
+        """DiffusionPipeline.generate_image with `guidance`, `reference_image`, `reference_latents` and `redux_image`
+        as in denoise_latents; with a guidance embedder the log holds the value of each image under
+        log["denoising"]["guidance"], with a reference its latent size and token count under
+        log["denoising"]["reference"], and with an image prompt {"images", "tokens", "time"} of its encode under
+        log["denoising"]["redux"]."""
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
                                     solver=solver, guidance=guidance, reference_image=reference_image,
-                                    reference_latents=reference_latents)
+                                    reference_latents=reference_latents, redux_image=redux_image)
+
+    def load_redux(self, siglip=None, redux=None, *, siglip_config=None):
+        """Build FLUX.1 Redux's image encoder on the device: SigLIP (siglip_config, default
+        google/siglip-so400m-patch14-384) and the Redux projector.  siglip / redux: parameter dicts in the engine's names
+        (model_io.siglip_checkpoint_to_params / redux_checkpoint_to_params convert the upstream safetensors), or None for
+        the deterministic synthetic initialiser.  Weights are 16-bit in the pipeline's dtype."""
+        from .config import SIGLIP_SO400M_PATCH14_384
+        from .image_encoders import (ReduxImageEncoder, SiglipVisionModel, init_siglip_params, redux_param_specs)
+
+        cfg = siglip_config or SIGLIP_SO400M_PATCH14_384
+        txt_dim = self.config.token_level_text_embed_dim
+        if siglip is None:
+            siglip = init_siglip_params(cfg, seed=self._weight_seed + 6, dtype=self.dtype, device=self.device)
+        if redux is None:
+            redux = init_params(redux_param_specs(cfg.hidden_size, txt_dim), seed=self._weight_seed + 7,
+                                dtype=self.dtype, device=self.device)
+        enc = ReduxImageEncoder({k: v.to(device=self.device, dtype=self.dtype) for k, v in redux.items()},
+                                device=self.device)
+        if (enc.siglip_hidden, enc.txt_dim) != (cfg.hidden_size, txt_dim):
+            raise ValueError(f"Redux projector maps {enc.siglip_hidden} -> {enc.txt_dim}; this pipeline needs "
+                             f"{cfg.hidden_size} (SigLIP) -> {txt_dim} (token_level_text_embed_dim)")
+        self.siglip = SiglipVisionModel({k: v.to(device=self.device, dtype=self.dtype) for k, v in siglip.items()}, cfg,
+                                        device=self.device)
+        self.redux = enc
+
+    def encode_redux(self, images) -> torch.Tensor:
+        """FLUX.1 Redux tokens of one image or a list (paths, PIL images or uint8 HWC arrays; converted to RGB and
+        resized to SigLIP's square size on the host), encoded as one batch -> (n, tokens, token_level_text_embed_dim)
+        on the device in the activation dtype.  Appending them to the T5 rows of `conditioning` is what
+        `redux_image=` does."""
+        self._need_redux()
+        arrs = [self._redux_image_u8(im) for im in (images if isinstance(images, (list, tuple)) else [images])]
+        out = torch.empty((len(arrs), self.siglip.config.num_patches, self.redux.txt_dim), dtype=self.activation_dtype,
+                          device=self.device)
+        self._redux_tokens(arrs, out, 0)
+        return out
 
     def encode_text(self, text: str, cfg_weight: float = 7.5, negative_text: str = ""):
         """reference :642-671: CLIP-L pooled output + T5 sequence of the POSITIVE prompt only, T5 padded with zeros to

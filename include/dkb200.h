@@ -50,6 +50,8 @@ extern "C" {
 #define DK_ACT_GELU_ERF 1 /* mlx nn.GELU() exact erf — mmdit.py:421,835 */
 #define DK_ACT_SILU 2
 #define DK_ACT_QUICK_GELU 3 /* x * sigmoid(1.702 x): mlx nn.gelu_fast_approx, CLIP-L "quick_gelu" — clip.py:11 */
+#define DK_ACT_GELU_TANH 4  /* 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))), accurate tanhf: SigLIP's
+                               "gelu_pytorch_tanh" (FLUX.1 Redux image encoder, DESIGN.md §15) */
 
 typedef struct dk_ctx dk_ctx;
 
@@ -247,6 +249,13 @@ int dk_dequant_q4(dk_ctx* ctx, int dtype, const uint32_t* wq, const void* scales
  * u8 / 255 * 2 - 1, the padding channels are zero */
 int dk_image_pre(dk_ctx* ctx, int dtype, const uint8_t* img, void* out, long long pixels, int src_channels, int cpad,
                  void* stream);
+/* FLUX.1 Redux's SigLIP patch embedding (DESIGN.md §15): uint8 NHWC [B, H, W, src_channels >= 3] -> 16-bit patch rows
+ * [B * (H/p) * (W/p), kp] of the stride-p, p x p convolution without padding (the last H % p rows and W % p columns are
+ * dropped).  Column k < 3p^2 holds channel k % 3 of pixel (k / 3p, (k / 3) % p) of the patch, normalised like
+ * dk_image_pre (u8 / 255 * 2 - 1, SigLIP's (x / 255 - 0.5) / 0.5); columns 3p^2 .. kp are zero.  kp % 8 == 0, so the
+ * rows feed dk_gemm with the conv weight permuted to (O, kh, kw, c) and zero-padded to kp. */
+int dk_image_patches(dk_ctx* ctx, int dtype, const uint8_t* img, void* out, int B, int H, int W, int src_channels,
+                     int p, int kp, void* stream);
 /* out = a * x + b * y (fp32): img2img noise scaling sigma * noise + (1 - sigma) * latent (sampler.py:41-42) */
 int dk_axpby_f32(dk_ctx* ctx, const float* x, const float* y, float* out, long long n, float a, float b, void* stream);
 /* VAE-encoder posterior sample + process_in: hidden [pixels, 2C] 16-bit = (mean | logvar);
