@@ -14,9 +14,10 @@ from .image_encoders import ReduxImageEncoder, SiglipVisionModel  # noqa: F401
 from .lora import LoRA, load_lora  # noqa: F401
 from .mmdit import MMDiT  # noqa: F401
 from .pipeline import (CFGDenoiser, DiffusionPipeline, FluxLatentFormat, FluxPipeline, LatentFormat,  # noqa: F401
-                       SD3LatentFormat, sample_dpmpp_2m, sample_euler, sample_heun)
+                       SD3LatentFormat, sample_dpmpp_2m, sample_dpmpp_2m_sde, sample_euler, sample_euler_ancestral,
+                       sample_heun)
 from .sampler import (FluxSampler, ModelSamplingDiscreteFlow, SkipLayerGuidance, dpmpp_2m_coefficients,  # noqa: F401
-                      flux_resolution_shift)
+                      dpmpp_2m_sde_coefficients, euler_ancestral_coefficients, flux_resolution_shift)
 from .vae import VAEDecoder, VAEEncoder  # noqa: F401
 
 __version__ = "0.1.0"

@@ -71,6 +71,8 @@ SIGNATURES = {
     "dk_sampler_heun_predict_slg": (i32, [vp, i32, vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, vp]),
     "dk_sampler_heun_correct_slg": (i32, [vp, i32, vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, vp]),
     "dk_sampler_dpmpp_2m_slg": (i32, [vp, i32, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, vp]),
+    "dk_sampler_sde_step": (i32, [vp, i32, vp, vp, vp, vp, i64, i32, i32, f32, f32, f32, f32, f32, f32, f32, vp, i32,
+                                  vp]),
     "dk_axpb_f32": (i32, [vp, vp, vp, i64, f32, f32, vp]),
     "dk_embedding": (i32, [vp, i32, vp, vp, vp, vp, i64, i32, i32, i32, vp]),
     "dk_layernorm": (i32, [vp, i32, vp, vp, vp, vp, i32, i32, f32, vp]),

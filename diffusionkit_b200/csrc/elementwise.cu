@@ -479,6 +479,83 @@ __global__ void sampler_dpmpp_2m_kernel(float* __restrict__ x, float* __restrict
     d_prev[i] = den;
   }
 }
+// Philox4x32-10 (Salmon et al. 2011, "Parallel random numbers: as easy as 1, 2, 3"): ten rounds of two 32 x 32 -> 64-bit
+// multiplies, the key bumped by the Weyl constants between rounds.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r > 0) {
+      k0 += 0x9E3779B9u;
+      k1 += 0xBB67AE85u;
+    }
+    const uint32_t lo0 = 0xD2511F53u * ctr.x, hi0 = __umulhi(0xD2511F53u, ctr.x);
+    const uint32_t lo1 = 0xCD9E8D57u * ctr.z, hi1 = __umulhi(0xCD9E8D57u, ctr.z);
+    ctr = make_uint4(hi1 ^ ctr.y ^ k0, lo1, hi0 ^ ctr.w ^ k1, lo0);
+  }
+  return ctr;
+}
+// The top 23 bits of a Philox word as ((v >> 9) + 0.5) 2^-23: exact in fp32 and strictly inside (0, 1), so logf is
+// finite.  (Taking 24 bits, (k + 0.5) 2^-24 needs 25 significant bits for k >= 2^23 and rounds, up to 1.0 at the top.)
+__device__ __forceinline__ float philox_uniform(uint32_t v) {
+  return (static_cast<float>(v >> 9) + 0.5f) * 0x1p-23f;
+}
+// Box-Muller with the accurate logf / sqrtf / sincospif: (r cos 2 pi u_t, r sin 2 pi u_t), r = sqrt(-2 log u_r)
+__device__ __forceinline__ float2 box_muller(float u_r, float u_t) {
+  const float r = sqrtf(-2.f * logf(u_r));
+  float s, c;
+  sincospif(2.f * u_t, &s, &c);
+  return make_float2(r * c, r * s);
+}
+// Stochastic samplers (DESIGN.md §16): x <- a x + b D + c D_prev + noise z, then D_prev <- D when d_prev is given.
+// Each thread owns 4 consecutive elements e = 4q .. 4q + 3 of image blockIdx.y (n_img elements per image; the rows of
+// xin / out sit n = B n_img apart per replica, as cfg_denoised expects).  z comes from one Philox call with counter
+// (q, step, 0, 0) and key (lo32(seed), hi32(seed)) of that image's seed: Box-Muller on (u0, u1) gives elements 0 and 1,
+// on (u2, u3) elements 2 and 3, so an image's noise depends only on its seed, the step and the element.  With
+// noise == 0 nothing is drawn and each element's arithmetic is sampler_dpmpp_2m_kernel's, in the same order.
+template <typename T, bool SLG>
+__global__ void __launch_bounds__(256) sampler_sde_step_kernel(float* __restrict__ x, float* __restrict__ d_prev,
+                                                               const T* __restrict__ xin, const T* __restrict__ out,
+                                                               long long n_img, long long n, float sigma, float a,
+                                                               float b, float c, float noise, float cfg, float slg,
+                                                               const uint64_t* __restrict__ seeds, uint32_t step) {
+  const long long img = blockIdx.y;
+  uint32_t k0 = 0, k1 = 0;
+  if (noise != 0.f) {
+    const uint64_t s = seeds[img];
+    k0 = static_cast<uint32_t>(s);
+    k1 = static_cast<uint32_t>(s >> 32);
+  }
+  const long long n4 = n_img >> 2;
+  for (long long q = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; q < n4;
+       q += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long i0 = img * n_img + 4 * q;
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (noise != 0.f) {
+      const uint4 v = philox4x32_10(make_uint4(static_cast<uint32_t>(q), step, 0u, 0u), k0, k1);
+      const float2 z01 = box_muller(philox_uniform(v.x), philox_uniform(v.y));
+      const float2 z23 = box_muller(philox_uniform(v.z), philox_uniform(v.w));
+      z[0] = z01.x, z[1] = z01.y, z[2] = z23.x, z[3] = z23.y;
+    }
+    const float4 x4 = *reinterpret_cast<const float4*>(x + i0);
+    const float xs[4] = {x4.x, x4.y, x4.z, x4.w};
+    float ps[4] = {0.f, 0.f, 0.f, 0.f};
+    if (c != 0.f) {
+      const float4 p4 = *reinterpret_cast<const float4*>(d_prev + i0);
+      ps[0] = p4.x, ps[1] = p4.y, ps[2] = p4.z, ps[3] = p4.w;
+    }
+    float res[4], den[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      den[k] = cfg_denoised<SLG>(xin, out, n, i0 + k, sigma, cfg, slg);
+      float v = a * xs[k] + b * den[k];
+      if (c != 0.f) v += c * ps[k];
+      if (noise != 0.f) v += noise * z[k];
+      res[k] = v;
+    }
+    *reinterpret_cast<float4*>(x + i0) = make_float4(res[0], res[1], res[2], res[3]);
+    if (d_prev != nullptr) *reinterpret_cast<float4*>(d_prev + i0) = make_float4(den[0], den[1], den[2], den[3]);
+  }
+}
 __global__ void axpb_kernel(const float* __restrict__ x, float* __restrict__ y, long long n, float a, float b) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
@@ -1307,6 +1384,44 @@ extern "C" int dk_sampler_dpmpp_2m_slg(dk_ctx* ctx, int dtype, float* x, float* 
   return 0;
 }
 #undef DK_SLG_REQUIRE
+
+extern "C" int dk_sampler_sde_step(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin, const void* out,
+                                   long long n_per_image, int B, int reps, float sigma, float a, float b, float c,
+                                   float noise, float cfg_weight, float slg, const uint64_t* seeds, int step,
+                                   void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(reps >= 1 && reps <= 3, "dk_sampler_sde_step: reps must be 1 (no CFG), 2 (CFG) or 3 (CFG + SLG), got %d",
+             reps);
+  DK_REQUIRE((reps >= 2) == (cfg_weight > 0.f),
+             "dk_sampler_sde_step: reps = %d does not match cfg_weight = %g (CFG needs reps 2 or 3)", reps, cfg_weight);
+  DK_REQUIRE(reps == 3 || slg == 0.f, "dk_sampler_sde_step: skip-layer guidance needs reps = 3 (CFG + SLG)");
+  DK_REQUIRE(isfinite(sigma) && isfinite(a) && isfinite(b) && isfinite(c) && isfinite(noise) && isfinite(cfg_weight) &&
+                 isfinite(slg),
+             "dk_sampler_sde_step: sigma, a, b, c, noise, cfg_weight and slg must be finite");
+  DK_REQUIRE(d_prev != nullptr || c == 0.f, "dk_sampler_sde_step: c != 0 needs d_prev");
+  DK_REQUIRE(noise == 0.f || seeds != nullptr, "dk_sampler_sde_step: noise != 0 needs seeds");
+  DK_REQUIRE(B >= 1 && B <= 65535, "dk_sampler_sde_step: B must be in [1, 65535], got %d", B);
+  DK_REQUIRE(step >= 0, "dk_sampler_sde_step: step must be >= 0, got %d", step);
+  DK_REQUIRE(n_per_image > 0 && n_per_image % 4 == 0 && n_per_image / 4 <= 0xFFFFFFFFll,
+             "dk_sampler_sde_step: n_per_image must be a positive multiple of 4 below 2^34, got %lld", n_per_image);
+  DK_REQUIRE(dk_aligned16(x) && dk_aligned16(d_prev) && dk_aligned16(xin) && dk_aligned16(out),
+             "dk_sampler_sde_step: x, d_prev, xin and out must be 16-byte aligned");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long n = n_per_image * B;
+  const dim3 grid(dk_grid_for(n_per_image / 4, 256, ctx->sm_count), B);
+  if (reps == 3) {
+    DK_DISPATCH(dtype, (sampler_sde_step_kernel<T, true><<<grid, 256, 0, stream>>>(
+                           x, d_prev, static_cast<const T*>(xin), static_cast<const T*>(out), n_per_image, n, sigma, a,
+                           b, c, noise, cfg_weight, slg, seeds, static_cast<uint32_t>(step))));
+  } else {
+    DK_DISPATCH(dtype, (sampler_sde_step_kernel<T, false><<<grid, 256, 0, stream>>>(
+                           x, d_prev, static_cast<const T*>(xin), static_cast<const T*>(out), n_per_image, n, sigma, a,
+                           b, c, noise, cfg_weight, 0.f, seeds, static_cast<uint32_t>(step))));
+  }
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
 
 extern "C" int dk_axpb_f32(dk_ctx* ctx, const float* x, float* y, long long n, float a, float b, void* stream_) {
   DK_ENTRY(ctx);

@@ -21,6 +21,8 @@ Differences that are deliberate (documented in DESIGN.md):
     `reference_latents=` of FluxPipeline.generate_image / denoise_latents), DESIGN.md §14.
   * FLUX.1 Redux image prompts (FluxPipeline.load_redux / encode_redux, `redux_image=` of generate_image /
     denoise_latents): SigLIP + Redux tokens appended to the T5 sequence, DESIGN.md §15.
+  * stochastic samplers (solver="euler_ancestral" / "dpmpp_2m_sde", `eta=`): per-image Philox noise drawn inside the
+    fused CFG + solver kernel, DESIGN.md §16.
 """
 from __future__ import annotations
 
@@ -32,11 +34,12 @@ import numpy as np
 import torch
 
 from . import ops
-from ._lib import DkError
+from ._lib import DkError, dtype_code, ptr
 from .config import MODEL_CONFIGS, T5_MAX_LENGTH, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig
 from .mmdit import MMDiT
-from .sampler import (FluxSampler, ModelSamplingDiscreteFlow, SkipLayerGuidance, check_skip_layer_guidance,
-                      dpmpp_2m_coefficients, skip_layer_guidance_steps)
+from .sampler import (FluxSampler, ModelSamplingDiscreteFlow, SkipLayerGuidance, check_eta, check_skip_layer_guidance,
+                      dpmpp_2m_coefficients, dpmpp_2m_sde_coefficients, euler_ancestral_coefficients,
+                      skip_layer_guidance_steps)
 from .vae import VAEDecoder, VAEEncoder
 from .weights import init_params, mmdit_param_specs, vae_decoder_param_specs, vae_encoder_param_specs
 
@@ -216,12 +219,79 @@ def sample_dpmpp_2m(model: CFGDenoiser, x, sigmas, extra_args=None):
     return x, _finish_sampling(model, events)
 
 
+def seeds_tensor(seeds, device) -> torch.Tensor:
+    """per-image 64-bit noise seeds -> the (B,) uint64 device array dk_sampler_sde_step reads"""
+    vals = [int(s) for s in seeds]
+    if not all(0 <= s < 2 ** 64 for s in vals):
+        raise ValueError(f"noise seeds must be in [0, 2^64), got {vals}")
+    return torch.from_numpy(np.asarray(vals, dtype=np.uint64)).to(device)
+
+
+def sampler_sde_step(x, d_prev, xin, out, sigma: float, a: float, b: float, c: float, noise: float, cfg_weight: float,
+                     slg: float, seeds: torch.Tensor, step: int):
+    """dk_sampler_sde_step: x = a x + b D + c d_prev + noise z, then d_prev = D (both in place; d_prev None: neither
+    read nor written, c must be 0).  x (B, ...) fp32; xin / out hold 1, 2 or 3 replicas of x's rows (no CFG, CFG, CFG +
+    skip-layer guidance); z is image b's Philox normal of `step` under seeds[b] (DESIGN.md §16).  Kept beside its
+    callers rather than in ops: the launch census of the shipped models requires a reference for every launching op
+    there, and this one runs only under a stochastic solver, whose GPU test runs a census of its own that wraps it."""
+    assert x.dtype == torch.float32 and x.is_contiguous() and xin.is_contiguous() and out.is_contiguous()
+    assert d_prev is None or (d_prev.dtype == torch.float32 and d_prev.is_contiguous() and d_prev.shape == x.shape)
+    B = x.shape[0]
+    assert seeds.dtype == torch.uint64 and tuple(seeds.shape) == (B,) and seeds.device == x.device
+    cx = ops.ctx(x.device.index)
+    cx.call("dk_sampler_sde_step", dtype_code(xin.dtype), ptr(x), ptr(d_prev), ptr(xin), ptr(out), x.numel() // B, B,
+            xin.numel() // x.numel(), sigma, a, b, c, noise, cfg_weight, slg, ptr(seeds), step)
+    return x
+
+
+def _sample_sde(model: CFGDenoiser, x, sigmas, extra_args, coefficients, keep_d: bool):
+    """the loop both stochastic samplers share: one forward and one dk_sampler_sde_step per step.  extra_args["eta"]
+    (None: 1.0) scales the noise, extra_args["seeds"] holds one noise seed per image of x."""
+    extra_args = dict(extra_args or {})
+    if "seeds" not in extra_args:
+        raise ValueError("a stochastic sampler needs extra_args['seeds']: one noise seed per image")
+    eta = extra_args.pop("eta", None)
+    coef = coefficients(np.asarray(sigmas, dtype=np.float32), 1.0 if eta is None else eta)
+    seeds = seeds_tensor(extra_args.pop("seeds"), x.device)            # one upload per call
+    sig, timesteps, conditioning, cfg_weight, events = _start_sampling(model, sigmas, extra_args)
+    d_prev = torch.empty_like(x) if keep_d else None
+    for i in range(len(sig) - 1):
+        xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight, step=i)
+        a, b, c, n = (float(v) for v in coef[i])
+        sampler_sde_step(x, d_prev, xin, out, float(sig[i]), a, b, c, n, cfg_weight, model.slg_scale(i), seeds, i)
+        events[i + 1].record()
+    return x, _finish_sampling(model, events)
+
+
+def sample_euler_ancestral(model: CFGDenoiser, x, sigmas, extra_args=None):
+    """Euler ancestral for the rectified-flow ODE sample_euler integrates (sampler.euler_ancestral_coefficients): an
+    Euler step to sigma_down, rescaled, plus fresh noise, one forward per step.  extra_args as for sample_euler, plus
+    "seeds" (one per image, required) and "eta" (None: 1.0; 0: Euler).  Same return value as sample_euler."""
+    return _sample_sde(model, x, sigmas, extra_args, euler_ancestral_coefficients, keep_d=False)
+
+
+def sample_dpmpp_2m_sde(model: CFGDenoiser, x, sigmas, extra_args=None):
+    """DPM-Solver++(2M) SDE (Lu et al. 2022; sampler.dpmpp_2m_sde_coefficients), one forward per step, the previous
+    step's denoised estimate kept on the device.  extra_args as for sample_euler_ancestral; eta = 0 is sample_dpmpp_2m
+    bit for bit.  Same return value as sample_euler."""
+    return _sample_sde(model, x, sigmas, extra_args, dpmpp_2m_sde_coefficients, keep_d=True)
+
+
+# the deterministic (ODE) solvers, and the stochastic ones, which take `eta` and draw per-image noise every step
 SOLVERS = {"euler": sample_euler, "heun": sample_heun, "dpmpp_2m": sample_dpmpp_2m}
+SDE_SOLVERS = {"euler_ancestral": sample_euler_ancestral, "dpmpp_2m_sde": sample_dpmpp_2m_sde}
 
 
-def _check_solver(solver: str):
-    if solver not in SOLVERS:
-        raise ValueError(f"unknown solver {solver!r}: expected one of {', '.join(repr(k) for k in SOLVERS)}")
+def _check_solver(solver: str, eta=None):
+    """the solver name and its eta, refused with ValueError before any GPU work"""
+    if solver not in SOLVERS and solver not in SDE_SOLVERS:
+        raise ValueError(f"unknown solver {solver!r}: expected one of "
+                         f"{', '.join(repr(k) for k in (*SOLVERS, *SDE_SOLVERS))}")
+    if eta is not None:
+        if solver not in SDE_SOLVERS:
+            raise ValueError(f"eta scales the noise of the stochastic solvers ({', '.join(map(repr, SDE_SOLVERS))}); "
+                             f"solver {solver!r} is deterministic")
+        check_eta(eta)
 
 
 def _check_slg(slg, cfg_weight: float, config: MMDiTConfig):
@@ -550,15 +620,19 @@ class DiffusionPipeline:
         noise: Optional[torch.Tensor] = None,
         solver: str = "euler",
         slg: Optional[SkipLayerGuidance] = None,
+        eta: Optional[float] = None,
     ):
         """-> (latent NHWC (B, H, W, 16) fp32 on the device, iter_time list).  `noise` (optional, device fp32
         (B, H, W, 16)) replaces the host-side numpy draw of get_noise for callers whose inputs already live in HBM.
         `image_path` (img2img): a file path, a PIL image or a uint8 HWC array; the latent size then follows the image
         (the reference ignores latent_size in that case too, :273).  `solver`: "euler" (the reference's sampler),
-        "heun" (two model evaluations per step but the last) or "dpmpp_2m" (one per step), DESIGN.md §11.
+        "heun" (two model evaluations per step but the last) or "dpmpp_2m" (one per step), DESIGN.md §11; or the
+        stochastic "euler_ancestral" and "dpmpp_2m_sde" (one per step, fresh noise drawn on the device every step from
+        each image's seed), DESIGN.md §16.  `eta`: the stochastic solvers' noise scale, >= 0 (None: 1.0; 0: the
+        deterministic step, for "dpmpp_2m_sde" exactly "dpmpp_2m"); a deterministic solver refuses it.
         `slg`: skip-layer guidance (sampler.SkipLayerGuidance, needs cfg_weight > 0; None: off), DESIGN.md §13."""
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
-                                     image_path, denoise, noise=noise, solver=solver, guidance=None, slg=slg)
+                                     image_path, denoise, noise=noise, solver=solver, guidance=None, slg=slg, eta=eta)
 
     def _guidance_values(self, guidance, n_images: int) -> Optional[List[float]]:
         """FluxPipeline's `guidance` -> one FLUX.1-dev guidance value per image, or None for a model without a
@@ -680,8 +754,8 @@ class DiffusionPipeline:
 
     def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
                          denoise, *, noise, solver, guidance, slg=None, reference_image=None, reference_latents=None,
-                         redux_image=None, redux_log=None):
-        _check_solver(solver)
+                         redux_image=None, redux_log=None, eta=None, sde_log=None):
+        _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
         if image_path is None:
             denoise = 1.0                                                   # :270-271
@@ -755,7 +829,13 @@ class DiffusionPipeline:
             extra_args["slg"] = slg
         if reference is not None:
             extra_args["reference"] = self._reference_latent(reference[0], reps * B)
-        latent, iter_time = SOLVERS[solver](CFGDenoiser(self), x, sigmas, extra_args=extra_args)
+        if solver in SDE_SOLVERS:
+            extra_args.update(eta=eta, seeds=seeds)
+            if sde_log is not None:
+                sde_log.update(solver=solver, eta=1.0 if eta is None else float(eta), seeds=seeds)
+            latent, iter_time = SDE_SOLVERS[solver](CFGDenoiser(self), x, sigmas, extra_args=extra_args)
+        else:
+            latent, iter_time = SOLVERS[solver](CFGDenoiser(self), x, sigmas, extra_args=extra_args)
         latent = ops.axpb(latent, 1.0 / self.latent_format.scale_factor, self.latent_format.shift_factor)  # process_out
         return latent, iter_time
 
@@ -776,17 +856,20 @@ class DiffusionPipeline:
         pooled_conditioning=None,
         solver: str = "euler",
         slg: Optional[SkipLayerGuidance] = None,
+        eta: Optional[float] = None,
     ):
         """`slg`: skip-layer guidance as in denoise_latents; the log then holds its scale, layers and the steps it
-        applied to under log["denoising"]["skip_layer_guidance"]."""
+        applied to under log["denoising"]["skip_layer_guidance"].  `solver` and `eta` as in denoise_latents; under a
+        stochastic solver the log holds {"solver", "eta", "seeds"} under log["denoising"]["sde"] (the seeds also when
+        seed=None picked one from the clock), which reproduces the run."""
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
-                                    solver=solver, guidance=None, slg=slg)
+                                    solver=solver, guidance=None, slg=slg, eta=eta)
 
     def _generate_image(self, text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                         denoise, *, conditioning, pooled_conditioning, solver, guidance, slg=None, reference_image=None,
-                        reference_latents=None, redux_image=None):
-        _check_solver(solver)
+                        reference_latents=None, redux_image=None, eta=None):
+        _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
         n_images = len(seed) if isinstance(seed, (list, tuple)) else 1
         guidance = self._guidance_values(guidance, n_images)
@@ -823,10 +906,11 @@ class DiffusionPipeline:
         torch.cuda.reset_peak_memory_stats(self.device)
         t0 = time.time()
         log["denoising"]["pre"] = mem()
-        redux_log = {}
+        redux_log, sde_log = {}, {}
         latents, iter_time = self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight,
                                                    latent_size, seed, image_path, denoise, noise=None, solver=solver,
-                                                   guidance=guidance, slg=slg, redux_log=redux_log,
+                                                   guidance=guidance, slg=slg, redux_log=redux_log, eta=eta,
+                                                   sde_log=sde_log,
                                                    redux_image=redux if redux is None or len(redux) == n_images
                                                    else redux[0], **ref_kw)
         torch.cuda.synchronize(self.device)
@@ -838,6 +922,8 @@ class DiffusionPipeline:
             n = len(iter_time)
             log["denoising"]["solver"] = solver
             log["denoising"]["nfe"] = max(2 * n - 1, 0) if solver == "heun" else n
+        if sde_log:
+            log["denoising"]["sde"] = sde_log
         if guidance is not None:
             log["denoising"]["guidance"] = guidance
         if reference is not None:
@@ -1008,8 +1094,8 @@ class FluxPipeline(DiffusionPipeline):
                         latent_size: Tuple[int, int] = (64, 64), seed=None, image_path: Optional[str] = None,
                         denoise: float = 1.0, *, noise: Optional[torch.Tensor] = None, solver: str = "euler",
                         guidance=None, reference_image=None, reference_latents: Optional[torch.Tensor] = None,
-                        redux_image=None):
-        """DiffusionPipeline.denoise_latents, plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
+                        redux_image=None, eta: Optional[float] = None):
+        """DiffusionPipeline.denoise_latents (`solver` and `eta` included), plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
         float for every image or one per seed, and None means DEFAULT_GUIDANCE (3.5) when the model has a guidance
         embedder (mmdit_config=FLUX_DEV).  A model without one refuses any value but None.
 
@@ -1025,14 +1111,14 @@ class FluxPipeline(DiffusionPipeline):
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
                                      image_path, denoise, noise=noise, solver=solver, guidance=guidance,
                                      reference_image=reference_image, reference_latents=reference_latents,
-                                     redux_image=redux_image)
+                                     redux_image=redux_image, eta=eta)
 
     def generate_image(self, text: str, num_steps: int = 2, cfg_weight: float = 0.0, negative_text: str = "",
                        latent_size: Tuple[int, int] = (64, 64), seed=None, verbose: bool = True,
                        image_path: Optional[str] = None, denoise: float = 1.0, *, conditioning=None,
                        pooled_conditioning=None, solver: str = "euler", guidance=None, reference_image=None,
-                       reference_latents: Optional[torch.Tensor] = None, redux_image=None):
-        """DiffusionPipeline.generate_image with `guidance`, `reference_image`, `reference_latents` and `redux_image`
+                       reference_latents: Optional[torch.Tensor] = None, redux_image=None, eta: Optional[float] = None):
+        """DiffusionPipeline.generate_image (`solver`, `eta` and the log of a stochastic solver included) with `guidance`, `reference_image`, `reference_latents` and `redux_image`
         as in denoise_latents; with a guidance embedder the log holds the value of each image under
         log["denoising"]["guidance"], with a reference its latent size and token count under
         log["denoising"]["reference"], and with an image prompt {"images", "tokens", "time"} of its encode under
@@ -1040,7 +1126,7 @@ class FluxPipeline(DiffusionPipeline):
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
                                     solver=solver, guidance=guidance, reference_image=reference_image,
-                                    reference_latents=reference_latents, redux_image=redux_image)
+                                    reference_latents=reference_latents, redux_image=redux_image, eta=eta)
 
     def load_redux(self, siglip=None, redux=None, *, siglip_config=None):
         """Build FLUX.1 Redux's image encoder on the device: SigLIP (siglip_config, default

@@ -2,7 +2,8 @@
 
 Host-side scalar arithmetic (numpy fp32, like the reference's fp32 mx arrays); the per-step tensor math runs in the
 fused CUDA sampler kernels (csrc/elementwise.cu: dk_sampler_prepare / dk_sampler_step, and the Heun and
-DPM-Solver++(2M) updates, whose fp64 coefficients dpmpp_2m_coefficients computes).
+DPM-Solver++(2M) updates, whose fp64 coefficients dpmpp_2m_coefficients computes, and the stochastic samplers' update
+dk_sampler_sde_step, whose coefficients euler_ancestral_coefficients / dpmpp_2m_sde_coefficients compute).
 """
 import math
 from dataclasses import dataclass
@@ -92,6 +93,81 @@ def dpmpp_2m_coefficients(sigmas) -> np.ndarray:
             coef[i] = (s[i + 1] / s[i], b1 * (1.0 + half_r), -b1 * half_r)
         else:
             coef[i] = (s[i + 1] / s[i], b1, 0.0)
+    return coef
+
+
+def check_eta(eta) -> float:
+    """the noise scale of a stochastic sampler: finite and >= 0 (ValueError otherwise)"""
+    e = float(eta)
+    if not (math.isfinite(e) and e >= 0.0):
+        raise ValueError(f"eta must be finite and >= 0, got {eta}")
+    return e
+
+
+def euler_ancestral_coefficients(sigmas, eta: float = 1.0) -> np.ndarray:
+    """The rectified-flow ancestral Euler step as per-step coefficients of x_{i+1} = a x_i + b D_i + c D_{i-1} + n z_i
+    (dk_sampler_sde_step), in fp64 -> (steps, 4) for steps + 1 sigmas; c is always 0.
+
+    sigma_down = sigma_{i+1} (1 + (sigma_{i+1} / sigma_i - 1) eta), alpha = 1 - sigma.  A deterministic Euler step to
+    sigma_down, rescaled by alpha_{i+1} / alpha_down, plus noise of standard deviation
+    sqrt(sigma_{i+1}^2 - (sigma_down alpha_{i+1} / alpha_down)^2):
+        a = (alpha_{i+1} / alpha_down) sigma_down / sigma_i,  b = (alpha_{i+1} / alpha_down) (1 - sigma_down / sigma_i).
+    eta = 0 gives Euler, (sigma_{i+1} / sigma_i, 1 - sigma_{i+1} / sigma_i, 0, 0).  An eta large enough to push
+    sigma_down below 0 is held at sigma_down = 0 (D re-noised to sigma_{i+1}).  A step to sigma = 0 returns D: (0, 1, 0, 0).
+
+    Check (fp64): with the exact denoiser D = x0 and x_i = alpha_i x0 + sigma_i eps, the coefficients of x0,
+    a alpha_i + b + c, sum to alpha_{i+1}, and the independent noise a sigma_i eps + n z has standard deviation
+    sqrt(a^2 sigma_i^2 + n^2) = sigma_{i+1}: each step lands on the marginal of x_{i+1}."""
+    s = np.asarray(sigmas, dtype=np.float64)
+    eta = check_eta(eta)
+    coef = np.zeros((len(s) - 1, 4), dtype=np.float64)
+    for i in range(len(s) - 1):
+        sn = s[i + 1]
+        if sn == 0.0:
+            coef[i] = (0.0, 1.0, 0.0, 0.0)
+            continue
+        ratio = sn / s[i]
+        sd = max(sn * (1.0 + (ratio - 1.0) * eta), 0.0)
+        scale = (1.0 - sn) / (1.0 - sd)
+        dn = sd * scale                                 # sigma_down alpha_{i+1} / alpha_down
+        coef[i] = (scale * (sd / s[i]), scale * (1.0 - sd / s[i]), 0.0, math.sqrt(max(sn * sn - dn * dn, 0.0)))
+    return coef
+
+
+def dpmpp_2m_sde_coefficients(sigmas, eta: float = 1.0) -> np.ndarray:
+    """DPM-Solver++(2M) SDE (Lu et al. 2022, data prediction, midpoint form) for x = (1 - sigma) x0 + sigma eps, as
+    per-step coefficients of x_{i+1} = a x_i + b D_i + c D_{i-1} + n z_i (dk_sampler_sde_step), in fp64 -> (steps, 4).
+
+    With h_i = lambda_{i+1} - lambda_i (lambda = log(alpha / sigma)):
+        a = (sigma_{i+1} / sigma_i) e^{-eta h},  b1 = alpha_{i+1} (1 - e^{-(1 + eta) h}),
+        n = sigma_{i+1} sqrt(1 - e^{-2 eta h}),
+    and b1 is split into b and c by dpmpp_2m_coefficients' second-order rule D' = (1 + 1/(2r)) D_i - 1/(2r) D_{i-1}, on
+    the same steps (not the first, not after an interval with h = inf, not the last two).  eta = 0 gives
+    dpmpp_2m_coefficients exactly (n = 0).  A step from sigma = 1 (h = inf) has a = 0 for eta > 0; a step to sigma = 0
+    returns D: (0, 1, 0, 0).
+
+    Check (fp64): with D = x0, a alpha_i + b + c = alpha_{i+1} (since (sigma_{i+1} / sigma_i) alpha_i = alpha_{i+1} e^{-h})
+    and sqrt(a^2 sigma_i^2 + n^2) = sigma_{i+1}, as for euler_ancestral_coefficients."""
+    s = np.asarray(sigmas, dtype=np.float64)
+    eta = check_eta(eta)
+    n = len(s) - 1
+    with np.errstate(divide="ignore"):
+        lam = np.log1p(-s) - np.log(s)
+    h = lam[1:] - lam[:-1]
+    coef = np.zeros((n, 4), dtype=np.float64)
+    for i in range(n):
+        if s[i + 1] == 0.0:
+            coef[i] = (0.0, 1.0, 0.0, 0.0)
+            continue
+        eh = eta * h[i] if eta > 0.0 else 0.0          # eta = 0 at h = inf is 0, not 0 * inf
+        a = s[i + 1] / s[i] * math.exp(-eh)
+        b1 = -(1.0 - s[i + 1]) * np.expm1(-(1.0 + eta) * h[i])
+        noise = s[i + 1] * math.sqrt(-math.expm1(-2.0 * eh))
+        if 1 <= i < n - 2 and np.isfinite(h[i - 1]):
+            half_r = 0.5 * h[i] / h[i - 1]              # 1 / (2r)
+            coef[i] = (a, b1 * (1.0 + half_r), -b1 * half_r, noise)
+        else:
+            coef[i] = (a, b1, 0.0, noise)
     return coef
 
 

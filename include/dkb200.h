@@ -218,6 +218,19 @@ int dk_sampler_heun_correct_slg(dk_ctx* ctx, int dtype, float* x, const float* d
 int dk_sampler_dpmpp_2m_slg(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin, const void* out,
                             long long n, float sigma, float a, float b, float c, float cfg_weight, float slg,
                             void* stream);
+/* Stochastic samplers (Euler ancestral, DPM-Solver++(2M) SDE; DESIGN.md §16), one step of B images of n_per_image
+ * elements each: x = a x + b D + c d_prev + noise z, then d_prev = D.  a, b, c, noise from
+ * sampler.euler_ancestral_coefficients / dpmpp_2m_sde_coefficients (Lu et al. 2022, data-prediction SDE solver; the
+ * rectified-flow ancestral step).  reps 1 (no CFG), 2 (CFG) or 3 (CFG + skip-layer guidance, slg the scale): D as in the
+ * updates above.  d_prev NULL: neither read nor written (then c must be 0); d_prev is not read when c == 0.
+ * z of element e of image b at solver step `step`: (v0..v3) = Philox4x32-10(counter (e / 4, step, 0, 0),
+ * key (lo32(seeds[b]), hi32(seeds[b]))), u_j = ((v_j >> 9) + 0.5) 2^-23, Box-Muller (sqrtf(-2 logf u), sincospif(2 u'))
+ * on (u0, u1) for e % 4 in {0, 1} and on (u2, u3) for {2, 3}: independent of B, the image's batch position and reps.
+ * noise == 0 draws nothing (seeds may be NULL) and computes what dk_sampler_dpmpp_2m computes, bit for bit.
+ * n_per_image % 4 == 0; x, d_prev, xin, out 16-byte aligned; seeds a device array of B values. */
+int dk_sampler_sde_step(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin, const void* out,
+                        long long n_per_image, int B, int reps, float sigma, float a, float b, float c, float noise,
+                        float cfg_weight, float slg, const uint64_t* seeds, int step, void* stream);
 /* y = x * a + b (fp32): latent_format.process_out (__init__.py:732-733) and noise scaling (sampler.py:41-42) */
 int dk_axpb_f32(dk_ctx* ctx, const float* x, float* y, long long n, float a, float b, void* stream);
 /* ---- text encoders (SURVEY.md §8 row f2): CLIP-L/G (mlx/clip.py) and the T5-XXL encoder (mlx/t5.py) ------------- */
