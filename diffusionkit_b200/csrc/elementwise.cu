@@ -556,6 +556,47 @@ __global__ void __launch_bounds__(256) sampler_sde_step_kernel(float* __restrict
     if (d_prev != nullptr) *reinterpret_cast<float4*>(d_prev + i0) = make_float4(den[0], den[1], den[2], den[3]);
   }
 }
+// Masked inpainting (DESIGN.md §17), after a solver step to sigma: every latent position the mask keeps (mask byte 0)
+// is reset to the re-noised source a eps + b x0 (a = sigma, b = 1 - sigma), rounded as axpby_kernel rounds it,
+// fma(a, eps, b x0); a repainted position (mask byte != 0) is neither read nor written.  x, eps, x0 are (B, HW, C)
+// fp32 and mask is (HW) uint8; one thread per 4-channel vector of image blockIdx.y, which lies within one position
+// since C % 4 == 0 (c4 = C / 4 vectors per position).
+__global__ void __launch_bounds__(256) inpaint_blend_kernel(float* __restrict__ x, const float* __restrict__ eps,
+                                                            const float* __restrict__ x0,
+                                                            const uint8_t* __restrict__ mask, unsigned n4_img,
+                                                            unsigned c4, float a, float b) {
+  const long long base = static_cast<long long>(blockIdx.y) * n4_img;
+  for (unsigned q = blockIdx.x * blockDim.x + threadIdx.x; q < n4_img; q += gridDim.x * blockDim.x) {
+    if (mask[q / c4] != 0) continue;
+    const float4 e = reinterpret_cast<const float4*>(eps)[base + q];
+    const float4 z = reinterpret_cast<const float4*>(x0)[base + q];
+    reinterpret_cast<float4*>(x)[base + q] =
+        make_float4(__fmaf_rn(a, e.x, __fmul_rn(b, z.x)), __fmaf_rn(a, e.y, __fmul_rn(b, z.y)),
+                    __fmaf_rn(a, e.z, __fmul_rn(b, z.z)), __fmaf_rn(a, e.w, __fmul_rn(b, z.w)));
+  }
+}
+// Inpainting paste-back: every pixel of the uint8 (B, P, 3) image whose mask byte is 0 becomes the source's (P, 3)
+// pixel.  One thread per 4 pixels = 12 bytes = 3 words of image blockIdx.y; four repainted pixels are left untouched,
+// four kept ones are stored without reading the image.
+__global__ void __launch_bounds__(256) inpaint_paste_kernel(uint8_t* __restrict__ img, const uint8_t* __restrict__ src,
+                                                            const uint8_t* __restrict__ mask, unsigned n4_img) {
+  uint32_t* dst = reinterpret_cast<uint32_t*>(img) + 3ll * blockIdx.y * n4_img;
+  const uint32_t* from = reinterpret_cast<const uint32_t*>(src);
+  for (unsigned q = blockIdx.x * blockDim.x + threadIdx.x; q < n4_img; q += gridDim.x * blockDim.x) {
+    const uint32_t m = reinterpret_cast<const uint32_t*>(mask)[q];
+    uint32_t keep[3] = {0u, 0u, 0u};  // byte k of the 12 belongs to pixel k / 3
+#pragma unroll
+    for (int k = 0; k < 12; ++k)
+      if (((m >> (8 * (k / 3))) & 0xFFu) == 0u) keep[k / 4] |= 0xFFu << (8 * (k % 4));
+    if ((keep[0] | keep[1] | keep[2]) == 0u) continue;
+    const bool all = (keep[0] & keep[1] & keep[2]) == 0xFFFFFFFFu;
+#pragma unroll
+    for (int w = 0; w < 3; ++w) {
+      const uint32_t s = from[3ll * q + w];
+      dst[3ll * q + w] = all ? s : (dst[3ll * q + w] & ~keep[w]) | (s & keep[w]);
+    }
+  }
+}
 __global__ void axpb_kernel(const float* __restrict__ x, float* __restrict__ y, long long n, float a, float b) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
@@ -1419,6 +1460,44 @@ extern "C" int dk_sampler_sde_step(dk_ctx* ctx, int dtype, float* x, float* d_pr
                            x, d_prev, static_cast<const T*>(xin), static_cast<const T*>(out), n_per_image, n, sigma, a,
                            b, c, noise, cfg_weight, 0.f, seeds, static_cast<uint32_t>(step))));
   }
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_inpaint_blend(dk_ctx* ctx, float* x, const float* eps, const float* x0, const uint8_t* mask, int B,
+                                long long HW, int C, float a, float b, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_REQUIRE(x != nullptr && eps != nullptr && x0 != nullptr && mask != nullptr,
+             "dk_inpaint_blend: x, eps, x0 and mask are required");
+  DK_REQUIRE(dk_aligned16(x) && dk_aligned16(eps) && dk_aligned16(x0),
+             "dk_inpaint_blend: x, eps and x0 must be 16-byte aligned");
+  DK_REQUIRE(B >= 1 && B <= 65535, "dk_inpaint_blend: B must be in [1, 65535], got %d", B);
+  DK_REQUIRE(C > 0 && C % 4 == 0, "dk_inpaint_blend: C must be a positive multiple of 4, got %d", C);
+  DK_REQUIRE(HW > 0 && HW * C / 4 < (1ll << 31), "dk_inpaint_blend: HW * C / 4 must be in [1, 2^31), got HW = %lld",
+             HW);
+  DK_REQUIRE(isfinite(a) && isfinite(b), "dk_inpaint_blend: a and b must be finite");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long n4 = HW * C / 4;
+  const dim3 grid(dk_grid_for(n4, 256, ctx->sm_count), B);
+  inpaint_blend_kernel<<<grid, 256, 0, stream>>>(x, eps, x0, mask, static_cast<unsigned>(n4),
+                                                 static_cast<unsigned>(C / 4), a, b);
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_inpaint_paste(dk_ctx* ctx, uint8_t* img, const uint8_t* src, const uint8_t* mask, int B,
+                                long long pixels, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_REQUIRE(img != nullptr && src != nullptr && mask != nullptr, "dk_inpaint_paste: img, src and mask are required");
+  DK_REQUIRE(((reinterpret_cast<uintptr_t>(img) | reinterpret_cast<uintptr_t>(src) |
+               reinterpret_cast<uintptr_t>(mask)) & 3u) == 0,
+             "dk_inpaint_paste: img, src and mask must be 4-byte aligned");
+  DK_REQUIRE(B >= 1 && B <= 65535, "dk_inpaint_paste: B must be in [1, 65535], got %d", B);
+  DK_REQUIRE(pixels > 0 && pixels % 4 == 0 && pixels / 4 < (1ll << 31),
+             "dk_inpaint_paste: pixels must be a positive multiple of 4 below 2^33, got %lld", pixels);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const dim3 grid(dk_grid_for(pixels / 4, 256, ctx->sm_count), B);
+  inpaint_paste_kernel<<<grid, 256, 0, stream>>>(img, src, mask, static_cast<unsigned>(pixels / 4));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }

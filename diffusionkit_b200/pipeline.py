@@ -23,6 +23,9 @@ Differences that are deliberate (documented in DESIGN.md):
     denoise_latents): SigLIP + Redux tokens appended to the T5 sequence, DESIGN.md §15.
   * stochastic samplers (solver="euler_ancestral" / "dpmpp_2m_sde", `eta=`): per-image Philox noise drawn inside the
     fused CFG + solver kernel, DESIGN.md §16.
+  * masked inpainting (`mask_image=` with `image_path`), DESIGN.md §17: diffusers' masked img2img blend after every
+    full solver step (after Heun's corrector), except that a latent position is repainted when ANY pixel of its 8 x 8
+    block is masked (diffusers samples one pixel), and generate_image always pastes the unmasked source pixels back.
 """
 from __future__ import annotations
 
@@ -33,7 +36,7 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 import torch
 
-from . import ops
+from . import inpaint, ops
 from ._lib import DkError, dtype_code, ptr
 from .config import MODEL_CONFIGS, T5_MAX_LENGTH, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig
 from .mmdit import MMDiT
@@ -101,6 +104,8 @@ class CFGDenoiser:
         self.slg = None
         # FLUX.1 Kontext reference latent of the running denoise, one row per forward row (None: no reference)
         self.reference = None
+        # masked inpainting of the running denoise (inpaint.InpaintBlend; None: no mask)
+        self.inpaint = None
 
     def cache_modulation_params(self, pooled_text_embeddings, sigmas, guidance=None, skip_batch: int = 0):
         """guidance: one FLUX.1-dev guidance value per row of pooled (None without a guidance embedder).
@@ -110,6 +115,12 @@ class CFGDenoiser:
     def slg_scale(self, step) -> float:
         """the skip-layer guidance scale of solver step `step` (0: plain CFG)"""
         return self.slg[0].scale if self.slg is not None and step in self.slg[1] else 0.0
+
+    def inpaint_step(self, x, sigma_next: float):
+        """after a full solver step to sigma_next: reset the latent positions a mask keeps to the re-noised source
+        (DESIGN.md §17); nothing, and no launch, without a mask"""
+        if self.inpaint is not None:
+            self.inpaint.blend(x, sigma_next)
 
     def clear_cache(self):
         # the reference re-reads the adaLN weights it dropped (:686-689); nothing was dropped here
@@ -148,6 +159,7 @@ def _start_sampling(model: CFGDenoiser, sigmas, extra_args):
     conditioning = extra_args["conditioning"]
     slg = extra_args.pop("slg", None)
     model.reference = extra_args.pop("reference", None)
+    model.inpaint = extra_args.pop("inpaint", None)
     steps = skip_layer_guidance_steps(slg, len(sig) - 1) if slg is not None else []
     skip_batch = 0
     if steps:
@@ -166,6 +178,7 @@ def _finish_sampling(model: CFGDenoiser, events):
     model.clear_cache()
     model.slg = None
     model.reference = None
+    model.inpaint = None
     torch.cuda.current_stream().synchronize()  # the reference syncs every step (mx.eval, :782); once is enough here
     return [round(events[i].elapsed_time(events[i + 1]) / 1e3, 3) for i in range(len(events) - 1)]
 
@@ -178,6 +191,7 @@ def sample_euler(model: CFGDenoiser, x, sigmas, extra_args=None):
         xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight, step=i)
         # denoised = xin - out * sigma; CFG mix; d = (x - denoised) / sigma; x += d * (sigma_next - sigma)
         ops.sampler_step(x, xin, out, float(sig[i]), float(sig[i + 1]), cfg_weight, slg=model.slg_scale(i))
+        model.inpaint_step(x, float(sig[i + 1]))
         events[i + 1].record()
     return x, _finish_sampling(model, events)
 
@@ -200,6 +214,7 @@ def sample_heun(model: CFGDenoiser, x, sigmas, extra_args=None):
             ops.sampler_heun_predict(x, xin, out, s, s_next, cfg_weight, d, x2, slg=slg)
             xin, out = model(x2, timesteps[i + 1], s_next, conditioning, cfg_weight, step=i)
             ops.sampler_heun_correct(x, d, x2, xin, out, s, s_next, cfg_weight, slg=slg)
+        model.inpaint_step(x, s_next)                 # after the full step: the predictor's x2 is not blended
         events[i + 1].record()
     return x, _finish_sampling(model, events)
 
@@ -215,6 +230,7 @@ def sample_dpmpp_2m(model: CFGDenoiser, x, sigmas, extra_args=None):
         xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight, step=i)
         a, b, c = (float(v) for v in coef[i])
         ops.sampler_dpmpp_2m(x, d_prev, xin, out, float(sig[i]), a, b, c, cfg_weight, slg=model.slg_scale(i))
+        model.inpaint_step(x, float(sig[i + 1]))      # d_prev stays the unblended history
         events[i + 1].record()
     return x, _finish_sampling(model, events)
 
@@ -259,6 +275,7 @@ def _sample_sde(model: CFGDenoiser, x, sigmas, extra_args, coefficients, keep_d:
         xin, out = model(x, timesteps[i], float(sig[i]), conditioning, cfg_weight, step=i)
         a, b, c, n = (float(v) for v in coef[i])
         sampler_sde_step(x, d_prev, xin, out, float(sig[i]), a, b, c, n, cfg_weight, model.slg_scale(i), seeds, i)
+        model.inpaint_step(x, float(sig[i + 1]))
         events[i + 1].record()
     return x, _finish_sampling(model, events)
 
@@ -301,6 +318,29 @@ def _check_slg(slg, cfg_weight: float, config: MMDiTConfig):
     if config.depth_unified > 0:
         raise ValueError("skip-layer guidance runs on SD3-family models only, not on a FLUX-shaped config")
     check_skip_layer_guidance(slg, cfg_weight, config.depth_multimodal)
+
+
+def _load_image_sized(image) -> Tuple[np.ndarray, Tuple[int, int]]:
+    """-> (uint8 (H, W, >=3) with H, W multiples of 64 (read_image's resize rule, :540-546), (width, height) of the
+    image as given)"""
+    from PIL import Image
+
+    if isinstance(image, (str, bytes)) or hasattr(image, "__fspath__"):
+        image = Image.open(image)
+    if isinstance(image, np.ndarray):
+        if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] < 3:
+            raise ValueError("image array must be uint8 (H, W, >=3)")
+        image = Image.fromarray(image[:, :, :3])
+    size = (image.width, image.height)
+    W, H = (dim - dim % 64 for dim in size)
+    if W == 0 or H == 0:
+        raise ValueError(f"image {image.width}x{image.height} is smaller than 64x64")
+    if W != image.width or H != image.height:
+        image = image.resize((W, H), Image.LANCZOS)
+    arr = np.asarray(image)
+    if arr.ndim == 2:
+        raise ValueError("greyscale images are not supported (the reference indexes img[:, :, :3])")
+    return np.ascontiguousarray(arr), size
 
 
 class DiffusionPipeline:
@@ -621,6 +661,7 @@ class DiffusionPipeline:
         solver: str = "euler",
         slg: Optional[SkipLayerGuidance] = None,
         eta: Optional[float] = None,
+        mask_image=None,
     ):
         """-> (latent NHWC (B, H, W, 16) fp32 on the device, iter_time list).  `noise` (optional, device fp32
         (B, H, W, 16)) replaces the host-side numpy draw of get_noise for callers whose inputs already live in HBM.
@@ -630,9 +671,14 @@ class DiffusionPipeline:
         stochastic "euler_ancestral" and "dpmpp_2m_sde" (one per step, fresh noise drawn on the device every step from
         each image's seed), DESIGN.md §16.  `eta`: the stochastic solvers' noise scale, >= 0 (None: 1.0; 0: the
         deterministic step, for "dpmpp_2m_sde" exactly "dpmpp_2m"); a deterministic solver refuses it.
-        `slg`: skip-layer guidance (sampler.SkipLayerGuidance, needs cfg_weight > 0; None: off), DESIGN.md §13."""
+        `slg`: skip-layer guidance (sampler.SkipLayerGuidance, needs cfg_weight > 0; None: off), DESIGN.md §13.
+        `mask_image` (masked inpainting, needs image_path; DESIGN.md §17): a path, a PIL image or a uint8 (H, W) /
+        (H, W, 1|3|4) array of the source image's size; white (>= 128 in grayscale) marks what to regenerate.  After
+        every solver step the other latent positions are reset to the re-noised source, so the returned latent holds
+        the encoded source there exactly; one mask for all seeds."""
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
-                                     image_path, denoise, noise=noise, solver=solver, guidance=None, slg=slg, eta=eta)
+                                     image_path, denoise, noise=noise, solver=solver, guidance=None, slg=slg, eta=eta,
+                                     mask_image=mask_image)
 
     def _guidance_values(self, guidance, n_images: int) -> Optional[List[float]]:
         """FluxPipeline's `guidance` -> one FLUX.1-dev guidance value per image, or None for a model without a
@@ -754,13 +800,17 @@ class DiffusionPipeline:
 
     def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
                          denoise, *, noise, solver, guidance, slg=None, reference_image=None, reference_latents=None,
-                         redux_image=None, redux_log=None, eta=None, sde_log=None):
+                         redux_image=None, redux_log=None, eta=None, sde_log=None, mask_image=None):
         _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
         if image_path is None:
             denoise = 1.0                                                   # :270-271
         elif not (0.0 <= denoise <= 1.0):
             raise ValueError(f"denoise must be in [0, 1], got {denoise}")
+        source = None
+        if mask_image is not None:
+            # generate_image passes the source array and the mask it prepared; the source is read once either way
+            source, mask_image = self._inpaint_input(image_path, mask_image)
         seeds: List[int]
         if seed is None:
             seeds = [int(time.time())]
@@ -796,7 +846,10 @@ class DiffusionPipeline:
                                  time=round(time.time() - t0, 3))
 
         hidden = None
-        if image_path is not None:
+        if source is not None:
+            hidden = self._encode_u8(source)
+            H, W = hidden.shape[1], hidden.shape[2]
+        elif image_path is not None:
             hidden = self._encode_image_hidden(image_path)                  # (1, H, W, 32) = (mean | logvar)
             H, W = hidden.shape[1], hidden.shape[2]
         x_T = self.get_empty_latent(H, W)                                   # (1, H, W, 16) host
@@ -829,6 +882,10 @@ class DiffusionPipeline:
             extra_args["slg"] = slg
         if reference is not None:
             extra_args["reference"] = self._reference_latent(reference[0], reps * B)
+        if source is not None:
+            # eps = the seeded noise and x0 = the encoded source of the start above, both (B, H, W, 16) in process_in
+            lm = torch.from_numpy(mask_image.latent).to(self.device)
+            extra_args["inpaint"] = inpaint.InpaintBlend(noise, x_T, lm)
         if solver in SDE_SOLVERS:
             extra_args.update(eta=eta, seeds=seeds)
             if sde_log is not None:
@@ -857,24 +914,31 @@ class DiffusionPipeline:
         solver: str = "euler",
         slg: Optional[SkipLayerGuidance] = None,
         eta: Optional[float] = None,
+        mask_image=None,
     ):
         """`slg`: skip-layer guidance as in denoise_latents; the log then holds its scale, layers and the steps it
         applied to under log["denoising"]["skip_layer_guidance"].  `solver` and `eta` as in denoise_latents; under a
         stochastic solver the log holds {"solver", "eta", "seeds"} under log["denoising"]["sde"] (the seeds also when
-        seed=None picked one from the clock), which reproduces the run."""
+        seed=None picked one from the clock), which reproduces the run.  `mask_image` as in denoise_latents; every
+        unmasked pixel of the returned images is then the source pixel (the resized image that was encoded), bit for
+        bit, and the log holds {"latent_size", "masked_fraction"} under log["denoising"]["inpaint"]."""
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
-                                    solver=solver, guidance=None, slg=slg, eta=eta)
+                                    solver=solver, guidance=None, slg=slg, eta=eta, mask_image=mask_image)
 
     def _generate_image(self, text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                         denoise, *, conditioning, pooled_conditioning, solver, guidance, slg=None, reference_image=None,
-                        reference_latents=None, redux_image=None, eta=None):
+                        reference_latents=None, redux_image=None, eta=None, mask_image=None):
         _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
         n_images = len(seed) if isinstance(seed, (list, tuple)) else 1
         guidance = self._guidance_values(guidance, n_images)
         reference = self._reference_input(reference_image, reference_latents, n_images)
         redux = self._redux_input(redux_image, cfg_weight, n_images)   # the checked 384^2 arrays go on: read once
+        source = None
+        if mask_image is not None:                  # the source array goes on to the encoder and the paste-back
+            source, mask_image = self._inpaint_input(image_path, mask_image)
+            image_path = source
         if reference is not None:                   # the checked image array goes on, so the file is read once
             ref_kw = {"reference_image" if isinstance(reference[0], np.ndarray) else "reference_latents": reference[0]}
         else:
@@ -910,7 +974,7 @@ class DiffusionPipeline:
         latents, iter_time = self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight,
                                                    latent_size, seed, image_path, denoise, noise=None, solver=solver,
                                                    guidance=guidance, slg=slg, redux_log=redux_log, eta=eta,
-                                                   sde_log=sde_log,
+                                                   sde_log=sde_log, mask_image=mask_image,
                                                    redux_image=redux if redux is None or len(redux) == n_images
                                                    else redux[0], **ref_kw)
         torch.cuda.synchronize(self.device)
@@ -931,6 +995,9 @@ class DiffusionPipeline:
             log["denoising"]["reference"] = {"latent_size": (Hr, Wr), "tokens": (Hr // 2) * (Wr // 2)}
         if redux is not None:
             log["denoising"]["redux"] = redux_log
+        if source is not None:
+            log["denoising"]["inpaint"] = {"latent_size": tuple(mask_image.latent.shape),
+                                           "masked_fraction": mask_image.masked_fraction}
         if slg is not None:
             log["denoising"]["skip_layer_guidance"] = {
                 "scale": slg.scale, "layers": list(slg.layers),
@@ -945,6 +1012,9 @@ class DiffusionPipeline:
         log["decoding"]["pre"] = mem()
         latents16 = ops.cast_to_16(latents, self.activation_dtype)          # latents.astype(activation_dtype) (:459)
         _, u8 = self._decode(latents16, want_u8=True)
+        if source is not None:                      # unmasked pixels: the source, without the VAE round trip
+            inpaint.inpaint_paste(u8, torch.from_numpy(np.ascontiguousarray(source[:, :, :3])).to(self.device),
+                                  torch.from_numpy(mask_image.pixels).to(self.device))
         host = getattr(self, "_host_u8", None)                              # pinned staging, reused across calls
         if host is None or host.shape != u8.shape:
             host = self._host_u8 = torch.empty(u8.shape, dtype=torch.uint8, pin_memory=True)
@@ -994,23 +1064,18 @@ class DiffusionPipeline:
 
     def _load_image_u8(self, image) -> np.ndarray:
         """-> uint8 (H, W, >=3) with H, W multiples of 64 (read_image's resize rule, :540-546)"""
-        from PIL import Image
+        return _load_image_sized(image)[0]
 
-        if isinstance(image, (str, bytes)) or hasattr(image, "__fspath__"):
-            image = Image.open(image)
-        if isinstance(image, np.ndarray):
-            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] < 3:
-                raise ValueError("image array must be uint8 (H, W, >=3)")
-            image = Image.fromarray(image[:, :, :3])
-        W, H = (dim - dim % 64 for dim in (image.width, image.height))
-        if W == 0 or H == 0:
-            raise ValueError(f"image {image.width}x{image.height} is smaller than 64x64")
-        if W != image.width or H != image.height:
-            image = image.resize((W, H), Image.LANCZOS)
-        arr = np.asarray(image)
-        if arr.ndim == 2:
-            raise ValueError("greyscale images are not supported (the reference indexes img[:, :, :3])")
-        return np.ascontiguousarray(arr)
+    def _inpaint_input(self, image_path, mask_image):
+        """-> (the source as _load_image_u8 returns it, inpaint.InpaintMask); a prepared mask passes through with
+        image_path, which is then that source array.  Raises ValueError, before any GPU work, for a mask the pipeline
+        cannot take."""
+        if image_path is None:
+            raise ValueError("mask_image needs image_path: the mask marks what to regenerate in that source image")
+        if isinstance(mask_image, inpaint.InpaintMask):
+            return image_path, mask_image
+        source, size = _load_image_sized(image_path)
+        return source, inpaint.prepare_mask(mask_image, size)
 
     def read_image(self, image_path):
         """-> (1, H, W, 3) float32 in [-1, 1] on the host (reference :536-551)"""
@@ -1094,8 +1159,8 @@ class FluxPipeline(DiffusionPipeline):
                         latent_size: Tuple[int, int] = (64, 64), seed=None, image_path: Optional[str] = None,
                         denoise: float = 1.0, *, noise: Optional[torch.Tensor] = None, solver: str = "euler",
                         guidance=None, reference_image=None, reference_latents: Optional[torch.Tensor] = None,
-                        redux_image=None, eta: Optional[float] = None):
-        """DiffusionPipeline.denoise_latents (`solver` and `eta` included), plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
+                        redux_image=None, eta: Optional[float] = None, mask_image=None):
+        """DiffusionPipeline.denoise_latents (`solver`, `eta` and `mask_image` included), plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
         float for every image or one per seed, and None means DEFAULT_GUIDANCE (3.5) when the model has a guidance
         embedder (mmdit_config=FLUX_DEV).  A model without one refuses any value but None.
 
@@ -1111,14 +1176,15 @@ class FluxPipeline(DiffusionPipeline):
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
                                      image_path, denoise, noise=noise, solver=solver, guidance=guidance,
                                      reference_image=reference_image, reference_latents=reference_latents,
-                                     redux_image=redux_image, eta=eta)
+                                     redux_image=redux_image, eta=eta, mask_image=mask_image)
 
     def generate_image(self, text: str, num_steps: int = 2, cfg_weight: float = 0.0, negative_text: str = "",
                        latent_size: Tuple[int, int] = (64, 64), seed=None, verbose: bool = True,
                        image_path: Optional[str] = None, denoise: float = 1.0, *, conditioning=None,
                        pooled_conditioning=None, solver: str = "euler", guidance=None, reference_image=None,
-                       reference_latents: Optional[torch.Tensor] = None, redux_image=None, eta: Optional[float] = None):
-        """DiffusionPipeline.generate_image (`solver`, `eta` and the log of a stochastic solver included) with `guidance`, `reference_image`, `reference_latents` and `redux_image`
+                       reference_latents: Optional[torch.Tensor] = None, redux_image=None, eta: Optional[float] = None,
+                       mask_image=None):
+        """DiffusionPipeline.generate_image (`solver`, `eta`, `mask_image` and their logs included) with `guidance`, `reference_image`, `reference_latents` and `redux_image`
         as in denoise_latents; with a guidance embedder the log holds the value of each image under
         log["denoising"]["guidance"], with a reference its latent size and token count under
         log["denoising"]["reference"], and with an image prompt {"images", "tokens", "time"} of its encode under
@@ -1126,7 +1192,8 @@ class FluxPipeline(DiffusionPipeline):
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
                                     solver=solver, guidance=guidance, reference_image=reference_image,
-                                    reference_latents=reference_latents, redux_image=redux_image, eta=eta)
+                                    reference_latents=reference_latents, redux_image=redux_image, eta=eta,
+                                    mask_image=mask_image)
 
     def load_redux(self, siglip=None, redux=None, *, siglip_config=None):
         """Build FLUX.1 Redux's image encoder on the device: SigLIP (siglip_config, default

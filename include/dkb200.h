@@ -231,6 +231,12 @@ int dk_sampler_dpmpp_2m_slg(dk_ctx* ctx, int dtype, float* x, float* d_prev, con
 int dk_sampler_sde_step(dk_ctx* ctx, int dtype, float* x, float* d_prev, const void* xin, const void* out,
                         long long n_per_image, int B, int reps, float sigma, float a, float b, float c, float noise,
                         float cfg_weight, float slg, const uint64_t* seeds, int step, void* stream);
+/* Masked inpainting (DESIGN.md §17), run after each solver step to sigma: at every position hw whose mask[hw] == 0
+ * (kept), x[b, hw, :] = a * eps[b, hw, :] + b * x0[b, hw, :] with a = sigma, b = 1 - sigma, rounded as dk_axpby_f32
+ * rounds it (fma(a, eps, b * x0)); positions with mask[hw] != 0 (repainted) are neither read nor written.
+ * x, eps, x0 fp32 (B, HW, C), 16-byte aligned, C % 4 == 0; mask uint8 (HW), shared by the B images. */
+int dk_inpaint_blend(dk_ctx* ctx, float* x, const float* eps, const float* x0, const uint8_t* mask, int B, long long HW,
+                     int C, float a, float b, void* stream);
 /* y = x * a + b (fp32): latent_format.process_out (__init__.py:732-733) and noise scaling (sampler.py:41-42) */
 int dk_axpb_f32(dk_ctx* ctx, const float* x, float* y, long long n, float a, float b, void* stream);
 /* ---- text encoders (SURVEY.md §8 row f2): CLIP-L/G (mlx/clip.py) and the T5-XXL encoder (mlx/t5.py) ------------- */
@@ -342,6 +348,10 @@ int dk_softmax_rows(dk_ctx* ctx, int dtype, void* x, long long rows, int n, long
  * x NHWC [.., C_in_stride] 16-bit, takes the first 3 channels. */
 int dk_image_post(dk_ctx* ctx, int dtype, const void* x, int c_stride, float* img_f32, uint8_t* img_u8, long long pixels,
                   void* stream);
+/* Inpainting paste-back (DESIGN.md §17): img uint8 (B, pixels, 3) in place; every pixel p with mask[p] == 0 becomes
+ * src[p] (uint8 (pixels, 3)), bit for bit; the others are not touched.  pixels % 4 == 0; img, src, mask 4-byte aligned. */
+int dk_inpaint_paste(dk_ctx* ctx, uint8_t* img, const uint8_t* src, const uint8_t* mask, int B, long long pixels,
+                     void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * one-time weight broadcast for multi-GPU batch sharding (no per-step collective).
