@@ -51,6 +51,9 @@ class MMDiTConfig:
     # keep the k bias of the q/k/v projections; False drops it (quirk Q3), which SD3.5 Medium cannot: with QK-RMSNorm
     # the bias enters before the norm and changes the output
     attn_k_bias: bool = False
+    # FLUX.1 Fill: input channels of the x-embedder beyond the packed latent's, the masked-image latent (64) and the
+    # mask (256) of every token (DESIGN.md §18); 0 for every other model
+    x_embedder_cond_channels: int = 0
 
     @property
     def head_dim(self) -> int:
@@ -84,6 +87,9 @@ SD35_MEDIUM = replace(SD3_2b, use_qk_norm=True, max_latent_resolution=384, x_blo
 # Defined by the reference but never used: FLUX.1-dev is loaded with FLUX_SCHNELL (mlx/model_io.py:109,756; quirk Q1).
 # Here mmdit_config=FLUX_DEV opts in to the guidance embedder (DESIGN.md §12); MODEL_CONFIGS keeps the quirk.
 FLUX_DEV = replace(FLUX_SCHNELL, guidance_embed=True)
+
+# FLUX.1 Fill [dev]: FLUX.1-dev with 320 conditioning channels per token in the x-embedder input (DESIGN.md §18)
+FLUX_FILL_DEV = replace(FLUX_DEV, x_embedder_cond_channels=320)
 
 
 @dataclass
@@ -119,6 +125,8 @@ MODEL_CONFIGS = {
     "stabilityai/stable-diffusion-3.5-medium": SD35_MEDIUM,
     # FLUX.1 Kontext [dev]: FLUX.1-dev's architecture and guidance embedder, run with reference tokens (DESIGN.md §14)
     "black-forest-labs/FLUX.1-Kontext-dev": FLUX_DEV,
+    # FLUX.1 Fill [dev]: masked-image and mask channels in the x-embedder input (DESIGN.md §18)
+    "black-forest-labs/FLUX.1-Fill-dev": FLUX_FILL_DEV,
 }
 
 # T5 sequence lengths (mlx/__init__.py:46-53)
@@ -131,6 +139,7 @@ T5_MAX_LENGTH = {
     "argmaxinc/mlx-FLUX.1-dev": 512,
     "stabilityai/stable-diffusion-3.5-medium": 512,
     "black-forest-labs/FLUX.1-Kontext-dev": 512,
+    "black-forest-labs/FLUX.1-Fill-dev": 512,
 }
 
 

@@ -656,6 +656,63 @@ __global__ void image_pre_kernel(const uint8_t* __restrict__ img, T* __restrict_
   }
 }
 
+// FLUX.1 Fill's masked image (DESIGN.md §18): image_pre_kernel for one (H, W) image whose pixels with a nonzero mask
+// byte are written as 0 in every channel, BFL's (x / 255 * 2 - 1) * (1 - mask) with +0 for the masked pixels.  Kept
+// pixels round through the same u8_to_unit.  One thread per 8-channel vector of the [pixels, cpad] output.
+template <typename T>
+__global__ void image_pre_masked_kernel(const uint8_t* __restrict__ img, const uint8_t* __restrict__ mask,
+                                        T* __restrict__ out, long long pixels, int src_c, int cpad) {
+  const int vpp = cpad / 8;
+  const long long nvec = pixels * vpp;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long p = i / vpp;
+    const int v = static_cast<int>(i - p * vpp);
+    uint4 w = make_uint4(0u, 0u, 0u, 0u);
+    if (v == 0 && mask[p] == 0) {
+      const uint8_t* px = img + p * src_c;
+      w.x = Half16<T>::pack(u8_to_unit(px[0]), u8_to_unit(px[1]));
+      w.y = Half16<T>::pack(u8_to_unit(px[2]), 0.f);
+    }
+    *reinterpret_cast<uint4*>(out + p * cpad + v * 8) = w;
+  }
+}
+
+// FLUX.1 Fill's conditioning rows (DESIGN.md §18): row n = (h, w) of the (H/16, W/16) token grid gets
+// [lat[n, 0:64] | 256 mask channels], 320 columns.  Mask channel j = c * 4 + ph * 2 + pw with c = ph1 * 8 + pw1 holds
+// mask[(2h + ph) * 8 + ph1, (2w + pw) * 8 + pw1] != 0 as 1 or 0: BFL's "b (h ph1) (w pw1) -> b (ph1 pw1) h w" then
+// "b c (h ph) (w pw) -> b (h w) (c ph pw)".  One thread per 8-column output vector (40 per row): vectors 0-7 copy the
+// latent, vector 8 + q holds channels c = 2q and 2q + 1.
+template <typename T>
+__global__ void fill_cond_rows_kernel(const T* __restrict__ lat, const uint8_t* __restrict__ mask, T* __restrict__ out,
+                                      int H, int W) {
+  const int wt = W / 16;
+  const long long nvec = static_cast<long long>(H / 16) * wt * 40;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long row = i / 40;
+    const int v = static_cast<int>(i - row * 40);
+    uint4 o;
+    if (v < 8) {
+      o = *reinterpret_cast<const uint4*>(lat + row * 64 + v * 8);
+    } else {
+      const int h = static_cast<int>(row / wt), w = static_cast<int>(row - static_cast<long long>(h) * wt);
+      float m[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const int c = 2 * (v - 8) + k / 4, ph = (k >> 1) & 1, pw = k & 1;
+        const long long y = (2 * h + ph) * 8 + (c >> 3), x = (2 * w + pw) * 8 + (c & 7);
+        m[k] = mask[y * W + x] != 0 ? 1.f : 0.f;
+      }
+      o.x = Half16<T>::pack(m[0], m[1]);
+      o.y = Half16<T>::pack(m[2], m[3]);
+      o.z = Half16<T>::pack(m[4], m[5]);
+      o.w = Half16<T>::pack(m[6], m[7]);
+    }
+    *reinterpret_cast<uint4*>(out + row * 320 + v * 8) = o;
+  }
+}
+
 // Patch rows of a stride-p, p x p, unpadded convolution (SigLIP's patch embedding): uint8 NHWC [B, H, W, src_c >= 3] ->
 // 16-bit [B * (H / p) * (W / p), kp].  Column k < 3p^2 of the row of patch (hp, wp) is u8_to_unit of channel k % 3 of
 // pixel (hp * p + k / (3p), wp * p + (k / 3) % p), i.e. (kh, kw, c) order; columns 3p^2.. are zero.  The floor of H / p
@@ -1535,6 +1592,41 @@ extern "C" int dk_image_pre(dk_ctx* ctx, int dtype, const uint8_t* img, void* ou
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DK_DISPATCH(dtype, (image_pre_kernel<T><<<dk_grid_for(pixels * (cpad / 8), 256, ctx->sm_count), 256, 0, stream>>>(
                          img, static_cast<T*>(out), pixels, src_channels, cpad)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_image_pre_masked(dk_ctx* ctx, int dtype, const uint8_t* img, const uint8_t* mask, void* out, int H,
+                                   int W, int src_channels, int cpad, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(img != nullptr && mask != nullptr && out != nullptr, "dk_image_pre_masked: img, mask and out are required");
+  DK_REQUIRE(dk_aligned16(out), "dk_image_pre_masked: out must be 16-byte aligned");
+  DK_REQUIRE(H > 0 && W > 0 && H % 16 == 0 && W % 16 == 0,
+             "dk_image_pre_masked: H and W must be positive multiples of 16, got %dx%d", H, W);
+  DK_REQUIRE(src_channels >= 3, "dk_image_pre_masked: image needs at least 3 channels (got %d)", src_channels);
+  DK_REQUIRE(cpad >= 8 && cpad % 8 == 0, "dk_image_pre_masked: cpad (%d) must be a positive multiple of 8", cpad);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long pixels = static_cast<long long>(H) * W;
+  DK_DISPATCH(dtype, (image_pre_masked_kernel<T><<<dk_grid_for(pixels * (cpad / 8), 256, ctx->sm_count), 256, 0,
+                                                   stream>>>(img, mask, static_cast<T*>(out), pixels, src_channels,
+                                                             cpad)));
+  DK_LAUNCH_CHECK(ctx);
+  return 0;
+}
+
+extern "C" int dk_fill_cond_rows(dk_ctx* ctx, int dtype, const void* lat, const uint8_t* mask, void* out, int H, int W,
+                                 void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  DK_REQUIRE(lat != nullptr && mask != nullptr && out != nullptr, "dk_fill_cond_rows: lat, mask and out are required");
+  DK_REQUIRE(dk_aligned16(lat) && dk_aligned16(out), "dk_fill_cond_rows: lat and out must be 16-byte aligned");
+  DK_REQUIRE(H > 0 && W > 0 && H % 16 == 0 && W % 16 == 0,
+             "dk_fill_cond_rows: H and W must be positive multiples of 16, got %dx%d", H, W);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long nvec = static_cast<long long>(H / 16) * (W / 16) * 40;
+  DK_DISPATCH(dtype, (fill_cond_rows_kernel<T><<<dk_grid_for(nvec, 256, ctx->sm_count), 256, 0, stream>>>(
+                         static_cast<const T*>(lat), mask, static_cast<T*>(out), H, W)));
   DK_LAUNCH_CHECK(ctx);
   return 0;
 }

@@ -28,6 +28,9 @@ H100 layout decisions (vs. the reference's per-module MLX graph):
   * FLUX.1 Kontext editing (`reference=` of __call__, DESIGN.md §14): a reference latent's tokens follow the target's
     in the image stream at RoPE positions (1, r, c); every block runs unchanged on the longer stream and the final
     layer reads the target rows.
+  * FLUX.1 Fill (`config.x_embedder_cond_channels`, DESIGN.md §18): the x-embedder's conditioning columns run once per
+    call (cache_fill_conditioning); every forward adds their product to the latent columns' through the x-embedder
+    GEMM's broadcast residual, so the per-step launches are FLUX.1-dev's.
 """
 from __future__ import annotations
 
@@ -110,6 +113,11 @@ class MMDiT:
         if self.d not in (64, 128):
             raise DkError(f"MMDiT: head dim {self.d} unsupported by the attention kernel (64 or 128)")
         self.is_flux = c.depth_unified > 0
+        self.cond_channels = int(c.x_embedder_cond_channels)
+        if self.cond_channels and not (self.is_flux and c.patchify_via_reshape):
+            raise ValueError("MMDiT: x_embedder_cond_channels (FLUX.1 Fill) needs a FLUX-shaped config")
+        if self.cond_channels % 8:
+            raise ValueError(f"MMDiT: x_embedder_cond_channels must be a multiple of 8, got {self.cond_channels}")
         self._pack(params)
         self._mod_index: Dict[float, int] = {}
         self._mod_all: Optional[torch.Tensor] = None
@@ -128,6 +136,11 @@ class MMDiT:
         # set_step_cache: the skip policy (None: off) and the input shape its residuals belong to
         self._step_cache: Optional[StepCachePolicy] = None
         self._step_cache_key = None
+        # FLUX.1 Fill: (rows, h) conditioning term of the x-embedder, written once per call by cache_fill_conditioning
+        # at a fixed address (captured graphs read it); _fill_rows = its valid rows, 0 until computed or after a LoRA
+        # merge changed the x-embedder
+        self._fill_cond: Optional[torch.Tensor] = None
+        self._fill_rows = 0
 
     # ------------------------------------------------------------------------------------------ weight packing
     def _pack(self, P: Dict[str, torch.Tensor]):
@@ -140,7 +153,9 @@ class MMDiT:
                 t = t.to(device=dev, dtype=dt)
             return t.contiguous()
 
-        self.w_x = get("x_embedder.proj.weight").reshape(h, -1).contiguous()          # (h, 64)
+        # (h, 64 + cond_channels): the latent columns, then FLUX.1 Fill's conditioning columns
+        self.w_x = get("x_embedder.proj.weight").reshape(h, -1).contiguous()
+        self.x_in = self.w_x.shape[1] - self.cond_channels
         self.b_x = get("x_embedder.proj.bias")
         self.pos_table = get("x_pos_embedder.pos_embed.weight") if "x_pos_embedder.pos_embed.weight" in P else None
         self.y0 = (get("y_embedder.mlp.layers.0.weight"), get("y_embedder.mlp.layers.0.bias"))
@@ -309,6 +324,25 @@ class MMDiT:
         for i, t in enumerate(ts):
             self._mod_index.setdefault(t, i)
         self._cur_t = None
+
+    def cache_fill_conditioning(self, rows: torch.Tensor):
+        """FLUX.1 Fill (DESIGN.md §18): rows (N, cond_channels) 16-bit, the [masked-image latent | mask] columns of the
+        N target tokens of one sequence, shared by every forward row -> the conditioning term
+        round16(rows @ W_c^T + b_x) of the x-embedder, W_c its conditioning columns, in a buffer every later forward
+        adds through the x-embedder GEMM's residual (one rounding of the sum).  Call once per denoise, after any LoRA
+        change; the buffer keeps its address while N does."""
+        if not self.cond_channels:
+            raise ValueError("cache_fill_conditioning: this model has no conditioning channels (not FLUX.1 Fill)")
+        if rows.dim() != 2 or rows.shape[1] != self.cond_channels or rows.dtype != self.dtype:
+            raise ValueError(f"cache_fill_conditioning: rows must be (N, {self.cond_channels}) {self.dtype}, got "
+                             f"{tuple(rows.shape)} {rows.dtype}")
+        N = rows.shape[0]
+        if self._fill_cond is None or self._fill_cond.shape[0] != N:
+            self._fill_cond = torch.empty((N, self.h), dtype=self.dtype, device=self.device)
+            self._shapes.drop_graphs()
+        ops.gemm(rows.contiguous(), self.w_x[:, self.x_in:], out=self._fill_cond, bias=self.b_x)
+        self._fill_rows = N
+        self._reset_step_cache()
 
     def clear_modulation_params_cache(self):
         self._mod_index, self._mod_all = {}, None
@@ -498,6 +532,8 @@ class MMDiT:
         if rebound:
             self._shapes.drop_graphs()
         self._reset_step_cache()
+        if any(attr == "w_x" for _, attr, _ in changed):
+            self._fill_rows = 0                          # the conditioning term was computed from the old W_c
         if mod_changed:
             self.clear_modulation_params_cache()
             self._cur_t = None
@@ -534,7 +570,7 @@ class MMDiT:
             "qkv": buf(B * S, 3 * h),
             "o_img": buf(B * N, h), "o_txt": buf(B * T, h),
             "hid_img": buf(B * N, r * h), "hid_txt": buf(B * T, r * h),
-            "rows_in": buf(B * N, self.w_x.shape[1]), "rows_out": buf(B * N, self.w_final.shape[0]),
+            "rows_in": buf(B * N, self.x_in), "rows_out": buf(B * N, self.w_final.shape[0]),
         }
         if self.attn2:                                 # MMDiT-X: attn2's packed q/k/v and its attention output
             ws["qkv2"] = buf(B * N, 3 * h)
@@ -677,6 +713,13 @@ class MMDiT:
             raise DkError("latent height/width must be divisible by the patch size")
         if reference is not None:
             self._check_reference(reference, B, Cl)
+        if self.cond_channels:
+            if reference is not None:
+                raise ValueError("reference: a FLUX.1 Fill model takes no Kontext reference")
+            Nx = (H // c.patch_size) * (W // c.patch_size)
+            if self._fill_rows != Nx:
+                raise ValueError(f"FLUX.1 Fill: the conditioning holds {self._fill_rows} tokens, the latent has {Nx}: "
+                                 "call cache_fill_conditioning for this latent first")
         text = token_level_text_embeddings
         if text.dim() == 4:
             text = text.squeeze(2)
@@ -747,6 +790,11 @@ class MMDiT:
             ops.patchify(ref, 0, out=rows_r)
             ops.gemm(rows_r, self.w_x, out=ws["img"], bias=self.b_x, rows_per_batch=N - Nx, out_batch_rows=N,
                      out_row_off=Nx)
+        elif self.cond_channels:
+            # FLUX.1 Fill: the latent columns plus the per-call conditioning term, broadcast over the batch
+            ops.patchify(x, 0, out=ws["rows_in"])
+            ops.gemm(ws["rows_in"], self.w_x[:, :self.x_in], out=ws["img"], res=self._fill_cond, rows_per_batch=N,
+                     out_batch_rows=N, res_batch_rows=0)
         elif c.patchify_via_reshape:
             ops.patchify(x, 0, out=ws["rows_in"])
             ops.gemm(ws["rows_in"], self.w_x, out=ws["img"], bias=self.b_x)

@@ -38,7 +38,7 @@ _FLUX_GUIDANCE_KEYS = {f"guidance_in.{layer}.{leaf}": f"guidance_in.mlp.layers.{
 
 
 def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, mlp_ratio: int = 4, *,
-                              guidance_embed: bool = False) -> Dict[str, Tensor]:
+                              guidance_embed: bool = False, cond_channels: int = 0) -> Dict[str, Tensor]:
     """BFL `flux1-*.safetensors` -> MMDiT parameter tree (reference model_io.py:130-311).
 
     double_blocks.i.{img,txt}_attn.qkv        -> split 3 (rows)  -> ...{image,text}_transformer_block.attn.{q,k,v}_proj
@@ -53,6 +53,8 @@ def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, ml
     guidance_in.{in,out}_layer                -> guidance_in.mlp.layers.{0,2}  (guidance_embed only)
     The K-projection bias is dropped (quirk Q3).  Without `guidance_embed` guidance_in.* is ignored, as the reference
     does (quirk Q1); with it, FLUX.1-dev's guidance embedder is loaded and must be present.
+    `cond_channels` (MMDiTConfig.x_embedder_cond_channels): img_in.weight must have 64 + cond_channels columns, 384 for
+    FLUX.1 Fill's `flux1-fill-dev.safetensors` (DESIGN.md §18); a ValueError names the key otherwise.
     """
     h = hidden_size
     out: Dict[str, Tensor] = {}
@@ -112,6 +114,10 @@ def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, ml
             continue
         if key.startswith("img_in."):
             leaf = key[7:]
+            if leaf == "weight" and v.shape[1] != 64 + cond_channels:
+                kind = "a FLUX.1 Fill" if cond_channels else "a plain FLUX"
+                raise ValueError(f"{key} has {v.shape[1]} input columns, {kind} config takes {64 + cond_channels} "
+                                 f"(x_embedder_cond_channels = {cond_channels})")
             out[f"x_embedder.proj.{leaf}"] = v.reshape(v.shape[0], 1, 1, v.shape[1]).contiguous() if leaf == "weight" else v
         elif key.startswith("txt_in."):
             out["context_embedder." + key[7:]] = v

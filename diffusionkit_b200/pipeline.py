@@ -26,6 +26,9 @@ Differences that are deliberate (documented in DESIGN.md):
   * masked inpainting (`mask_image=` with `image_path`), DESIGN.md §17: diffusers' masked img2img blend after every
     full solver step (after Heun's corrector), except that a latent position is repainted when ANY pixel of its 8 x 8
     block is masked (diffusers samples one pixel), and generate_image always pastes the unmasked source pixels back.
+  * FLUX.1 Fill [dev] (model_version "black-forest-labs/FLUX.1-Fill-dev", FluxPipeline with `mask_image=` and
+    `image_path`), DESIGN.md §18: the masked source and the mask enter the x-embedder instead of the §17 blend; the
+    unmasked source pixels are still pasted back.
 """
 from __future__ import annotations
 
@@ -36,7 +39,7 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 import torch
 
-from . import inpaint, ops
+from . import fill, inpaint, ops
 from ._lib import DkError, dtype_code, ptr
 from .config import MODEL_CONFIGS, T5_MAX_LENGTH, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig
 from .mmdit import MMDiT
@@ -55,6 +58,7 @@ MMDIT_CKPT = {  # reference mlx/__init__.py:37-44
     "argmaxinc/mlx-FLUX.1-dev": "argmaxinc/mlx-FLUX.1-dev",
     "stabilityai/stable-diffusion-3.5-medium": "stabilityai/stable-diffusion-3.5-medium",
     "black-forest-labs/FLUX.1-Kontext-dev": "black-forest-labs/FLUX.1-Kontext-dev",
+    "black-forest-labs/FLUX.1-Fill-dev": "black-forest-labs/FLUX.1-Fill-dev",
 }
 
 # FLUX.1-dev's guidance when the caller passes none (BFL's default for the dev checkpoint)
@@ -427,7 +431,8 @@ class DiffusionPipeline:
                             out[part] = sub
             elif isinstance(self, FluxPipeline):
                 params = model_io.flux_checkpoint_to_params(sd, self.config.hidden_size, self.config.mlp_ratio,
-                                                            guidance_embed=self.config.guidance_embed)
+                                                            guidance_embed=self.config.guidance_embed,
+                                                            cond_channels=self.config.x_embedder_cond_channels)
             else:
                 params = model_io.sd3_checkpoint_to_params(sd, k_bias=self.config.attn_k_bias)
                 if "vae" not in paths and any("decoder." in k for k in sd):
@@ -689,7 +694,7 @@ class DiffusionPipeline:
                                  " build the pipeline with mmdit_config=FLUX_DEV (or guidance_embed=True)")
             return None
         if guidance is None:
-            guidance = DEFAULT_GUIDANCE
+            guidance = fill.DEFAULT_GUIDANCE if self.config.x_embedder_cond_channels else DEFAULT_GUIDANCE
         if np.ndim(guidance) == 0:
             vals = [float(guidance)] * n_images
         else:
@@ -700,6 +705,18 @@ class DiffusionPipeline:
         if not all(math.isfinite(g) for g in vals):
             raise ValueError(f"guidance must be finite, got {vals}")
         return vals
+
+    def _check_fill(self, image_path, mask_image, reference_image, reference_latents):
+        """FLUX.1 Fill's arguments, refused with ValueError before any GPU work (nothing to check on other models)"""
+        if not self.config.x_embedder_cond_channels:
+            return
+        if not isinstance(self, FluxPipeline):
+            raise ValueError("a FLUX.1 Fill config (x_embedder_cond_channels) runs in FluxPipeline only")
+        if image_path is None or mask_image is None:
+            raise ValueError("FLUX.1 Fill needs image_path and mask_image: the model is conditioned on the masked "
+                             "source and the mask")
+        if reference_image is not None or reference_latents is not None:
+            raise ValueError("FLUX.1 Fill takes no Kontext reference")
 
     def _reference_input(self, reference_image, reference_latents, n_images: int):
         """FluxPipeline's Kontext reference -> None, or (uint8 HWC image or fp32 latents, its (Hr, Wr) latent size).
@@ -800,9 +817,10 @@ class DiffusionPipeline:
 
     def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
                          denoise, *, noise, solver, guidance, slg=None, reference_image=None, reference_latents=None,
-                         redux_image=None, redux_log=None, eta=None, sde_log=None, mask_image=None):
+                         redux_image=None, redux_log=None, eta=None, sde_log=None, mask_image=None, fill_log=None):
         _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
+        self._check_fill(image_path, mask_image, reference_image, reference_latents)
         if image_path is None:
             denoise = 1.0                                                   # :270-271
         elif not (0.0 <= denoise <= 1.0):
@@ -882,7 +900,19 @@ class DiffusionPipeline:
             extra_args["slg"] = slg
         if reference is not None:
             extra_args["reference"] = self._reference_latent(reference[0], reps * B)
-        if source is not None:
+        if source is not None and self.config.x_embedder_cond_channels:
+            # FLUX.1 Fill: the masked source and the mask condition the x-embedder, once per call; no latent blend
+            t0 = time.time()
+            lf = self.latent_format
+            src = torch.from_numpy(source).unsqueeze(0).to(self.device)
+            rows = fill.conditioning_rows(self.encoder, src, torch.from_numpy(mask_image.pixels).to(self.device),
+                                          lf.shift_factor, lf.scale_factor, self.activation_dtype)
+            self.mmdit.cache_fill_conditioning(rows)
+            if fill_log is not None:
+                torch.cuda.synchronize(self.device)
+                fill_log.update(latent_size=tuple(mask_image.latent.shape), masked_fraction=mask_image.masked_fraction,
+                                time=round(time.time() - t0, 3))
+        elif source is not None:
             # eps = the seeded noise and x0 = the encoded source of the start above, both (B, H, W, 16) in process_in
             lm = torch.from_numpy(mask_image.latent).to(self.device)
             extra_args["inpaint"] = inpaint.InpaintBlend(noise, x_T, lm)
@@ -931,6 +961,7 @@ class DiffusionPipeline:
                         reference_latents=None, redux_image=None, eta=None, mask_image=None):
         _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
+        self._check_fill(image_path, mask_image, reference_image, reference_latents)
         n_images = len(seed) if isinstance(seed, (list, tuple)) else 1
         guidance = self._guidance_values(guidance, n_images)
         reference = self._reference_input(reference_image, reference_latents, n_images)
@@ -970,11 +1001,11 @@ class DiffusionPipeline:
         torch.cuda.reset_peak_memory_stats(self.device)
         t0 = time.time()
         log["denoising"]["pre"] = mem()
-        redux_log, sde_log = {}, {}
+        redux_log, sde_log, fill_log = {}, {}, {}
         latents, iter_time = self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight,
                                                    latent_size, seed, image_path, denoise, noise=None, solver=solver,
                                                    guidance=guidance, slg=slg, redux_log=redux_log, eta=eta,
-                                                   sde_log=sde_log, mask_image=mask_image,
+                                                   sde_log=sde_log, mask_image=mask_image, fill_log=fill_log,
                                                    redux_image=redux if redux is None or len(redux) == n_images
                                                    else redux[0], **ref_kw)
         torch.cuda.synchronize(self.device)
@@ -995,7 +1026,9 @@ class DiffusionPipeline:
             log["denoising"]["reference"] = {"latent_size": (Hr, Wr), "tokens": (Hr // 2) * (Wr // 2)}
         if redux is not None:
             log["denoising"]["redux"] = redux_log
-        if source is not None:
+        if fill_log:
+            log["denoising"]["fill"] = fill_log
+        elif source is not None:
             log["denoising"]["inpaint"] = {"latent_size": tuple(mask_image.latent.shape),
                                            "masked_fraction": mask_image.masked_fraction}
         if slg is not None:
@@ -1172,7 +1205,13 @@ class FluxPipeline(DiffusionPipeline):
 
         FLUX.1 Redux image prompt (DESIGN.md §15, after load_redux): `redux_image` is one image for every seed or a list
         with one per seed (each as encode_redux takes it).  It is encoded once per call, and its tokens are appended to
-        each image's conditioning rows, which then hold T + tokens rows.  Needs cfg_weight == 0."""
+        each image's conditioning rows, which then hold T + tokens rows.  Needs cfg_weight == 0.
+
+        FLUX.1 Fill [dev] (DESIGN.md §18; model_version "black-forest-labs/FLUX.1-Fill-dev" or mmdit_config=
+        FLUX_FILL_DEV): `image_path` and `mask_image` are required, `mask_image` as in DiffusionPipeline.  The source with
+        its masked pixels zeroed is encoded once into its posterior mean and, with the mask, conditions every forward
+        through the x-embedder; there is no latent blend.  `guidance` None means 30.0 on this model.  No Kontext
+        reference."""
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
                                      image_path, denoise, noise=noise, solver=solver, guidance=guidance,
                                      reference_image=reference_image, reference_latents=reference_latents,
@@ -1188,7 +1227,9 @@ class FluxPipeline(DiffusionPipeline):
         as in denoise_latents; with a guidance embedder the log holds the value of each image under
         log["denoising"]["guidance"], with a reference its latent size and token count under
         log["denoising"]["reference"], and with an image prompt {"images", "tokens", "time"} of its encode under
-        log["denoising"]["redux"]."""
+        log["denoising"]["redux"].  On a FLUX.1 Fill model the unmasked source pixels are pasted back as with any mask,
+        and the log holds {"latent_size", "masked_fraction", "time"} of the conditioning under log["denoising"]["fill"]
+        instead of log["denoising"]["inpaint"]."""
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
                                     solver=solver, guidance=guidance, reference_image=reference_image,

@@ -22,11 +22,11 @@ Same parameter names as the reference module tree (SURVEY.md App. C).  Kernels (
 from __future__ import annotations
 
 import math
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 
-from . import ops
+from . import fill, ops
 from ._lib import DkError
 from .config import VAEDecoderConfig, VAEEncoderConfig
 from .graphs import ShapeCache, default_settings
@@ -213,14 +213,20 @@ class VAEEncoder(_VAEBlocks):
         h, st = self._resnet(h, st, "mid_blocks.2")
         return self._conv(h, "conv_out", "conv_norm_out", st)[0]
 
-    def __call__(self, image: torch.Tensor) -> torch.Tensor:
-        """image: uint8 NHWC (B, H, W, >=3) on the device, or a 16/32-bit float NHWC (B, H, W, 3) already in [-1, 1]."""
+    def __call__(self, image: torch.Tensor, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """image: uint8 NHWC (B, H, W, >=3) on the device, or a 16/32-bit float NHWC (B, H, W, 3) already in [-1, 1].
+        mask (FLUX.1 Fill's masked image, DESIGN.md §18): uint8 (H, W) on the device for one uint8 image; the pixels
+        with a nonzero mask byte enter the encoder as 0."""
         if image.dim() != 4:
             raise ValueError(f"VAEEncoder expects NHWC rank-4 input, got rank {image.dim()}")
         if image.shape[1] % 8 or image.shape[2] % 8:
             raise ValueError(f"VAEEncoder: image size {tuple(image.shape[1:3])} must be a multiple of 8")
         image = image.to(self.device)
-        if image.dtype == torch.uint8:
+        if mask is not None:
+            if image.dtype != torch.uint8 or image.shape[0] != 1:
+                raise ValueError("VAEEncoder: a mask goes with one uint8 image")
+            x16 = fill.image_pre_masked(image.contiguous(), mask.to(self.device).contiguous(), self.dtype, self.cin_pad)
+        elif image.dtype == torch.uint8:
             x16 = ops.image_pre(image.contiguous(), self.dtype, self.cin_pad)
         else:
             x16 = torch.zeros((*image.shape[:3], self.cin_pad), dtype=self.dtype, device=self.device)

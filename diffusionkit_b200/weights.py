@@ -30,7 +30,8 @@ def mmdit_param_specs(cfg: MMDiTConfig) -> List[Spec]:
             specs.append((name + ".bias", (out_f,), "b"))
 
     if cfg.patchify_via_reshape:
-        specs.append(("x_embedder.proj.weight", (h, 1, 1, cfg.vae_latent_dim * p * p), "w"))
+        specs.append(("x_embedder.proj.weight", (h, 1, 1, cfg.vae_latent_dim * p * p + cfg.x_embedder_cond_channels),
+                      "w"))
     else:
         specs.append(("x_embedder.proj.weight", (h, p, p, cfg.vae_latent_dim), "w"))
     specs.append(("x_embedder.proj.bias", (h,), "b"))

@@ -268,6 +268,17 @@ int dk_dequant_q4(dk_ctx* ctx, int dtype, const uint32_t* wq, const void* scales
  * u8 / 255 * 2 - 1, the padding channels are zero */
 int dk_image_pre(dk_ctx* ctx, int dtype, const uint8_t* img, void* out, long long pixels, int src_channels, int cpad,
                  void* stream);
+/* FLUX.1 Fill's masked image (DESIGN.md §18): dk_image_pre of one uint8 (H, W, src_channels >= 3) image into 16-bit
+ * (H, W, cpad), except that every pixel with mask[p] != 0 (uint8 (H, W)) is +0 in every channel.  Kept pixels round
+ * exactly as dk_image_pre rounds them.  H, W positive multiples of 16; out 16-byte aligned; cpad % 8 == 0. */
+int dk_image_pre_masked(dk_ctx* ctx, int dtype, const uint8_t* img, const uint8_t* mask, void* out, int H, int W,
+                        int src_channels, int cpad, void* stream);
+/* FLUX.1 Fill's conditioning rows (DESIGN.md §18): lat (N, 64) 16-bit packed masked-image latent rows, N = (H/16)(W/16)
+ * tokens, and the uint8 (H, W) pixel mask -> out (N, 320) = [lat | mask channels].  Mask channel c * 4 + ph * 2 + pw,
+ * c = ph1 * 8 + pw1, of token (h, w) is 1 when mask[(2h + ph) * 8 + ph1, (2w + pw) * 8 + pw1] != 0, else 0.
+ * H, W positive multiples of 16; lat and out 16-byte aligned and contiguous. */
+int dk_fill_cond_rows(dk_ctx* ctx, int dtype, const void* lat, const uint8_t* mask, void* out, int H, int W,
+                      void* stream);
 /* FLUX.1 Redux's SigLIP patch embedding (DESIGN.md §15): uint8 NHWC [B, H, W, src_channels >= 3] -> 16-bit patch rows
  * [B * (H/p) * (W/p), kp] of the stride-p, p x p convolution without padding (the last H % p rows and W % p columns are
  * dropped).  Column k < 3p^2 holds channel k % 3 of pixel (k / 3p, (k / 3) % p) of the patch, normalised like
