@@ -8,8 +8,9 @@ DiffusionPipeline / FluxPipeline API (reference: argmaxinc/DiffusionKit, python/
                                      conditioning=cond, pooled_conditioning=pooled)
 """
 from ._lib import DkError  # noqa: F401
-from .config import (FLUX_DEV, FLUX_FILL_DEV, FLUX_SCHNELL, SD3_2b, SD3_8b, SD35_MEDIUM,  # noqa: F401
-                     SIGLIP_SO400M_PATCH14_384, MMDiTConfig, SiglipVisionConfig, VAEDecoderConfig, VAEEncoderConfig)
+from .config import (FLUX_CANNY_DEV, FLUX_DEPTH_DEV, FLUX_DEV, FLUX_FILL_DEV, FLUX_SCHNELL, SD3_2b,  # noqa: F401
+                     SD3_8b, SD35_MEDIUM, SIGLIP_SO400M_PATCH14_384, MMDiTConfig, SiglipVisionConfig,
+                     VAEDecoderConfig, VAEEncoderConfig)
 from .image_encoders import ReduxImageEncoder, SiglipVisionModel  # noqa: F401
 from .lora import LoRA, load_lora  # noqa: F401
 from .mmdit import MMDiT  # noqa: F401

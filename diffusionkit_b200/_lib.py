@@ -85,6 +85,7 @@ SIGNATURES = {
     "dk_image_pre": (i32, [vp, i32, vp, vp, i64, i32, i32, vp]),
     "dk_image_pre_masked": (i32, [vp, i32, vp, vp, vp, i32, i32, i32, i32, vp]),
     "dk_fill_cond_rows": (i32, [vp, i32, vp, vp, vp, i32, i32, vp]),
+    "dk_canny": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "dk_image_patches": (i32, [vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
     "dk_axpby_f32": (i32, [vp, vp, vp, vp, i64, f32, f32, vp]),
     "dk_vae_sample_latent": (i32, [vp, i32, vp, vp, vp, i64, i32, f32, f32, vp]),

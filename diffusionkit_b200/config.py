@@ -54,6 +54,9 @@ class MMDiTConfig:
     # FLUX.1 Fill: input channels of the x-embedder beyond the packed latent's, the masked-image latent (64) and the
     # mask (256) of every token (DESIGN.md §18); 0 for every other model
     x_embedder_cond_channels: int = 0
+    # FLUX.1 Canny / Depth [dev]: "canny" or "depth" names the control image's preprocessing and the default guidance
+    # (DESIGN.md §19); None for every other model
+    control: Optional[str] = None
 
     @property
     def head_dim(self) -> int:
@@ -90,6 +93,11 @@ FLUX_DEV = replace(FLUX_SCHNELL, guidance_embed=True)
 
 # FLUX.1 Fill [dev]: FLUX.1-dev with 320 conditioning channels per token in the x-embedder input (DESIGN.md §18)
 FLUX_FILL_DEV = replace(FLUX_DEV, x_embedder_cond_channels=320)
+
+# FLUX.1 Canny [dev] and FLUX.1 Depth [dev]: FLUX.1-dev with the control image's 64 latent channels per token in the
+# x-embedder input (DESIGN.md §19)
+FLUX_CANNY_DEV = replace(FLUX_DEV, x_embedder_cond_channels=64, control="canny")
+FLUX_DEPTH_DEV = replace(FLUX_DEV, x_embedder_cond_channels=64, control="depth")
 
 
 @dataclass
@@ -129,6 +137,13 @@ MODEL_CONFIGS = {
     "black-forest-labs/FLUX.1-Fill-dev": FLUX_FILL_DEV,
 }
 
+# model_version -> config of the structural-control models (DESIGN.md §19), resolved like MODEL_CONFIGS; a table of
+# their own because FLUX.1 Fill is the only model of MODEL_CONFIGS with conditioning channels in the x-embedder
+CONTROL_MODEL_CONFIGS = {
+    "black-forest-labs/FLUX.1-Canny-dev": FLUX_CANNY_DEV,
+    "black-forest-labs/FLUX.1-Depth-dev": FLUX_DEPTH_DEV,
+}
+
 # T5 sequence lengths (mlx/__init__.py:46-53)
 T5_MAX_LENGTH = {
     "argmaxinc/mlx-stable-diffusion-3-medium": 512,
@@ -140,6 +155,8 @@ T5_MAX_LENGTH = {
     "stabilityai/stable-diffusion-3.5-medium": 512,
     "black-forest-labs/FLUX.1-Kontext-dev": 512,
     "black-forest-labs/FLUX.1-Fill-dev": 512,
+    "black-forest-labs/FLUX.1-Canny-dev": 512,
+    "black-forest-labs/FLUX.1-Depth-dev": 512,
 }
 
 

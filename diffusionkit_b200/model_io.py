@@ -54,7 +54,8 @@ def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, ml
     The K-projection bias is dropped (quirk Q3).  Without `guidance_embed` guidance_in.* is ignored, as the reference
     does (quirk Q1); with it, FLUX.1-dev's guidance embedder is loaded and must be present.
     `cond_channels` (MMDiTConfig.x_embedder_cond_channels): img_in.weight must have 64 + cond_channels columns, 384 for
-    FLUX.1 Fill's `flux1-fill-dev.safetensors` (DESIGN.md §18); a ValueError names the key otherwise.
+    FLUX.1 Fill's `flux1-fill-dev.safetensors` (DESIGN.md §18), 128 for `flux1-canny-dev.safetensors` and
+    `flux1-depth-dev.safetensors` (cond_channels 64, DESIGN.md §19); a ValueError names the key otherwise.
     """
     h = hidden_size
     out: Dict[str, Tensor] = {}
@@ -115,7 +116,7 @@ def flux_checkpoint_to_params(sd: Dict[str, Tensor], hidden_size: int = 3072, ml
         if key.startswith("img_in."):
             leaf = key[7:]
             if leaf == "weight" and v.shape[1] != 64 + cond_channels:
-                kind = "a FLUX.1 Fill" if cond_channels else "a plain FLUX"
+                kind = {0: "a plain FLUX", 64: "a FLUX.1 Canny / Depth"}.get(cond_channels, "a FLUX.1 Fill")
                 raise ValueError(f"{key} has {v.shape[1]} input columns, {kind} config takes {64 + cond_channels} "
                                  f"(x_embedder_cond_channels = {cond_channels})")
             out[f"x_embedder.proj.{leaf}"] = v.reshape(v.shape[0], 1, 1, v.shape[1]).contiguous() if leaf == "weight" else v

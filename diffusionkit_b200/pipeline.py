@@ -29,6 +29,9 @@ Differences that are deliberate (documented in DESIGN.md):
   * FLUX.1 Fill [dev] (model_version "black-forest-labs/FLUX.1-Fill-dev", FluxPipeline with `mask_image=` and
     `image_path`), DESIGN.md §18: the masked source and the mask enter the x-embedder instead of the §17 blend; the
     unmasked source pixels are still pasted back.
+  * FLUX.1 Canny / Depth [dev] (model_version "black-forest-labs/FLUX.1-Canny-dev" / "-Depth-dev", FluxPipeline with
+    `control_image=`), DESIGN.md §19: the control image's posterior-mean latent enters the x-embedder; no depth
+    estimator is included, a Depth model takes the depth map the caller gives.
 """
 from __future__ import annotations
 
@@ -39,9 +42,9 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 import torch
 
-from . import fill, inpaint, ops
+from . import control, fill, inpaint, ops
 from ._lib import DkError, dtype_code, ptr
-from .config import MODEL_CONFIGS, T5_MAX_LENGTH, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig
+from .config import CONTROL_MODEL_CONFIGS, MODEL_CONFIGS, T5_MAX_LENGTH, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig
 from .mmdit import MMDiT
 from .sampler import (FluxSampler, ModelSamplingDiscreteFlow, SkipLayerGuidance, check_eta, check_skip_layer_guidance,
                       dpmpp_2m_coefficients, dpmpp_2m_sde_coefficients, euler_ancestral_coefficients,
@@ -59,6 +62,8 @@ MMDIT_CKPT = {  # reference mlx/__init__.py:37-44
     "stabilityai/stable-diffusion-3.5-medium": "stabilityai/stable-diffusion-3.5-medium",
     "black-forest-labs/FLUX.1-Kontext-dev": "black-forest-labs/FLUX.1-Kontext-dev",
     "black-forest-labs/FLUX.1-Fill-dev": "black-forest-labs/FLUX.1-Fill-dev",
+    "black-forest-labs/FLUX.1-Canny-dev": "black-forest-labs/FLUX.1-Canny-dev",
+    "black-forest-labs/FLUX.1-Depth-dev": "black-forest-labs/FLUX.1-Depth-dev",
 }
 
 # FLUX.1-dev's guidance when the caller passes none (BFL's default for the dev checkpoint)
@@ -395,7 +400,10 @@ class DiffusionPipeline:
         if device is None:
             raise DkError("no CUDA device: diffusionkit_b200 runs on H100 only; there is no CPU fallback")
         self.device = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
-        self.config = mmdit_config if mmdit_config is not None else MODEL_CONFIGS[model_version]
+        if mmdit_config is not None:
+            self.config = mmdit_config
+        else:
+            self.config = MODEL_CONFIGS.get(model_version) or CONTROL_MODEL_CONFIGS[model_version]
         self._weight_seed = weight_seed
         self._params, self._vae_params = params, vae_params
         self._load_decoder = load_decoder
@@ -694,7 +702,10 @@ class DiffusionPipeline:
                                  " build the pipeline with mmdit_config=FLUX_DEV (or guidance_embed=True)")
             return None
         if guidance is None:
-            guidance = fill.DEFAULT_GUIDANCE if self.config.x_embedder_cond_channels else DEFAULT_GUIDANCE
+            if self.config.control:
+                guidance = control.DEFAULT_GUIDANCE[self.config.control]
+            else:
+                guidance = fill.DEFAULT_GUIDANCE if self.config.x_embedder_cond_channels else DEFAULT_GUIDANCE
         if np.ndim(guidance) == 0:
             vals = [float(guidance)] * n_images
         else:
@@ -708,7 +719,7 @@ class DiffusionPipeline:
 
     def _check_fill(self, image_path, mask_image, reference_image, reference_latents):
         """FLUX.1 Fill's arguments, refused with ValueError before any GPU work (nothing to check on other models)"""
-        if not self.config.x_embedder_cond_channels:
+        if not self.config.x_embedder_cond_channels or self.config.control:
             return
         if not isinstance(self, FluxPipeline):
             raise ValueError("a FLUX.1 Fill config (x_embedder_cond_channels) runs in FluxPipeline only")
@@ -717,6 +728,31 @@ class DiffusionPipeline:
                              "source and the mask")
         if reference_image is not None or reference_latents is not None:
             raise ValueError("FLUX.1 Fill takes no Kontext reference")
+
+    def _check_control(self, control_image, canny_thresholds, reference_image, reference_latents):
+        """FLUX.1 Canny / Depth's arguments, refused with ValueError before any GPU work -> canny_thresholds checked
+        ((low, high) or None) on a Canny model, None otherwise"""
+        kind = self.config.control
+        if kind != "canny" and canny_thresholds != control.DEFAULT_THRESHOLDS:
+            raise ValueError("canny_thresholds applies to a FLUX.1 Canny model only")
+        if kind is None:
+            if control_image is not None:
+                raise ValueError("control_image conditions a FLUX.1 Canny or Depth model (config.control); this model "
+                                 "has none")
+            return None
+        if kind not in control.KINDS:
+            raise ValueError(f"config.control must be one of {control.KINDS}, got {kind!r}")
+        if self.config.x_embedder_cond_channels != control.LATENT_CHANNELS:
+            raise ValueError(f"a {kind} control model takes {control.LATENT_CHANNELS} conditioning channels, the "
+                             f"config has x_embedder_cond_channels = {self.config.x_embedder_cond_channels}")
+        name = f"FLUX.1 {kind.capitalize()}"
+        if not isinstance(self, FluxPipeline):
+            raise ValueError(f"a {name} config runs in FluxPipeline only")
+        if control_image is None:
+            raise ValueError(f"{name} needs control_image: the model is conditioned on it")
+        if reference_image is not None or reference_latents is not None:
+            raise ValueError(f"{name} takes no Kontext reference")
+        return control.check_thresholds(canny_thresholds) if kind == "canny" else None
 
     def _reference_input(self, reference_image, reference_latents, n_images: int):
         """FluxPipeline's Kontext reference -> None, or (uint8 HWC image or fp32 latents, its (Hr, Wr) latent size).
@@ -817,10 +853,12 @@ class DiffusionPipeline:
 
     def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
                          denoise, *, noise, solver, guidance, slg=None, reference_image=None, reference_latents=None,
-                         redux_image=None, redux_log=None, eta=None, sde_log=None, mask_image=None, fill_log=None):
+                         redux_image=None, redux_log=None, eta=None, sde_log=None, mask_image=None, fill_log=None,
+                         control_image=None, canny_thresholds=control.DEFAULT_THRESHOLDS, control_log=None):
         _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
         self._check_fill(image_path, mask_image, reference_image, reference_latents)
+        thresholds = self._check_control(control_image, canny_thresholds, reference_image, reference_latents)
         if image_path is None:
             denoise = 1.0                                                   # :270-271
         elif not (0.0 <= denoise <= 1.0):
@@ -829,6 +867,14 @@ class DiffusionPipeline:
         if mask_image is not None:
             # generate_image passes the source array and the mask it prepared; the source is read once either way
             source, mask_image = self._inpaint_input(image_path, mask_image)
+        if control_image is not None:
+            # the control image takes the target's pixel size: the source's when there is one (read once here)
+            if image_path is not None and source is None:
+                image_path = self._load_image_u8(image_path)
+            target = source if source is not None else image_path
+            size = ((target.shape[1], target.shape[0]) if target is not None
+                    else (8 * latent_size[1], 8 * latent_size[0]))
+            control_image = control.load_control_image(control_image, size)
         seeds: List[int]
         if seed is None:
             seeds = [int(time.time())]
@@ -900,7 +946,20 @@ class DiffusionPipeline:
             extra_args["slg"] = slg
         if reference is not None:
             extra_args["reference"] = self._reference_latent(reference[0], reps * B)
-        if source is not None and self.config.x_embedder_cond_channels:
+        if control_image is not None:
+            # FLUX.1 Canny / Depth: the control image's latent conditions the x-embedder, once per call
+            t0 = time.time()
+            if not hasattr(self, "encoder"):
+                self.load_encoder()
+            lf = self.latent_format
+            rows = control.control_rows(self.encoder, torch.from_numpy(control_image).to(self.device),
+                                        self.config.control, lf.shift_factor, lf.scale_factor, self.activation_dtype,
+                                        thresholds)
+            self.mmdit.cache_fill_conditioning(rows)
+            if control_log is not None:
+                torch.cuda.synchronize(self.device)
+                control_log.update(kind=self.config.control, latent_size=(H, W), time=round(time.time() - t0, 3))
+        if source is not None and self.config.x_embedder_cond_channels and not self.config.control:
             # FLUX.1 Fill: the masked source and the mask condition the x-embedder, once per call; no latent blend
             t0 = time.time()
             lf = self.latent_format
@@ -958,10 +1017,12 @@ class DiffusionPipeline:
 
     def _generate_image(self, text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                         denoise, *, conditioning, pooled_conditioning, solver, guidance, slg=None, reference_image=None,
-                        reference_latents=None, redux_image=None, eta=None, mask_image=None):
+                        reference_latents=None, redux_image=None, eta=None, mask_image=None, control_image=None,
+                        canny_thresholds=control.DEFAULT_THRESHOLDS):
         _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
         self._check_fill(image_path, mask_image, reference_image, reference_latents)
+        self._check_control(control_image, canny_thresholds, reference_image, reference_latents)
         n_images = len(seed) if isinstance(seed, (list, tuple)) else 1
         guidance = self._guidance_values(guidance, n_images)
         reference = self._reference_input(reference_image, reference_latents, n_images)
@@ -1001,11 +1062,13 @@ class DiffusionPipeline:
         torch.cuda.reset_peak_memory_stats(self.device)
         t0 = time.time()
         log["denoising"]["pre"] = mem()
-        redux_log, sde_log, fill_log = {}, {}, {}
+        redux_log, sde_log, fill_log, control_log = {}, {}, {}, {}
         latents, iter_time = self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight,
                                                    latent_size, seed, image_path, denoise, noise=None, solver=solver,
                                                    guidance=guidance, slg=slg, redux_log=redux_log, eta=eta,
                                                    sde_log=sde_log, mask_image=mask_image, fill_log=fill_log,
+                                                   control_image=control_image, canny_thresholds=canny_thresholds,
+                                                   control_log=control_log,
                                                    redux_image=redux if redux is None or len(redux) == n_images
                                                    else redux[0], **ref_kw)
         torch.cuda.synchronize(self.device)
@@ -1026,6 +1089,8 @@ class DiffusionPipeline:
             log["denoising"]["reference"] = {"latent_size": (Hr, Wr), "tokens": (Hr // 2) * (Wr // 2)}
         if redux is not None:
             log["denoising"]["redux"] = redux_log
+        if control_log:
+            log["denoising"]["control"] = control_log
         if fill_log:
             log["denoising"]["fill"] = fill_log
         elif source is not None:
@@ -1192,7 +1257,8 @@ class FluxPipeline(DiffusionPipeline):
                         latent_size: Tuple[int, int] = (64, 64), seed=None, image_path: Optional[str] = None,
                         denoise: float = 1.0, *, noise: Optional[torch.Tensor] = None, solver: str = "euler",
                         guidance=None, reference_image=None, reference_latents: Optional[torch.Tensor] = None,
-                        redux_image=None, eta: Optional[float] = None, mask_image=None):
+                        redux_image=None, eta: Optional[float] = None, mask_image=None, control_image=None,
+                        canny_thresholds=control.DEFAULT_THRESHOLDS):
         """DiffusionPipeline.denoise_latents (`solver`, `eta` and `mask_image` included), plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
         float for every image or one per seed, and None means DEFAULT_GUIDANCE (3.5) when the model has a guidance
         embedder (mmdit_config=FLUX_DEV).  A model without one refuses any value but None.
@@ -1211,30 +1277,43 @@ class FluxPipeline(DiffusionPipeline):
         FLUX_FILL_DEV): `image_path` and `mask_image` are required, `mask_image` as in DiffusionPipeline.  The source with
         its masked pixels zeroed is encoded once into its posterior mean and, with the mask, conditions every forward
         through the x-embedder; there is no latent blend.  `guidance` None means 30.0 on this model.  No Kontext
-        reference."""
+        reference.
+
+        FLUX.1 Canny / Depth [dev] (DESIGN.md §19; model_version "black-forest-labs/FLUX.1-Canny-dev" / "-Depth-dev",
+        or mmdit_config=FLUX_CANNY_DEV / FLUX_DEPTH_DEV): `control_image` is required, a path, a PIL image or a uint8
+        (H, W) / (H, W, 1|3|4) array, converted to RGB and resized with PIL LANCZOS to exactly the target's pixel size
+        (the source's with image_path, else 8 x latent_size).  On Canny it goes through BFL's round trip and
+        cv2.Canny(img, *canny_thresholds) on the GPU first (canny_thresholds None: it is already an edge map); on
+        Depth it is the depth map.  It is encoded once into its posterior mean and conditions every forward through
+        the x-embedder.  `guidance` None means 30.0 on Canny and 10.0 on Depth.  img2img, mask_image (§17's blend),
+        Redux and every solver combine with it; a Kontext reference does not.  Other models refuse control_image."""
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
                                      image_path, denoise, noise=noise, solver=solver, guidance=guidance,
                                      reference_image=reference_image, reference_latents=reference_latents,
-                                     redux_image=redux_image, eta=eta, mask_image=mask_image)
+                                     redux_image=redux_image, eta=eta, mask_image=mask_image,
+                                     control_image=control_image, canny_thresholds=canny_thresholds)
 
     def generate_image(self, text: str, num_steps: int = 2, cfg_weight: float = 0.0, negative_text: str = "",
                        latent_size: Tuple[int, int] = (64, 64), seed=None, verbose: bool = True,
                        image_path: Optional[str] = None, denoise: float = 1.0, *, conditioning=None,
                        pooled_conditioning=None, solver: str = "euler", guidance=None, reference_image=None,
                        reference_latents: Optional[torch.Tensor] = None, redux_image=None, eta: Optional[float] = None,
-                       mask_image=None):
+                       mask_image=None, control_image=None, canny_thresholds=control.DEFAULT_THRESHOLDS):
         """DiffusionPipeline.generate_image (`solver`, `eta`, `mask_image` and their logs included) with `guidance`, `reference_image`, `reference_latents` and `redux_image`
         as in denoise_latents; with a guidance embedder the log holds the value of each image under
         log["denoising"]["guidance"], with a reference its latent size and token count under
         log["denoising"]["reference"], and with an image prompt {"images", "tokens", "time"} of its encode under
         log["denoising"]["redux"].  On a FLUX.1 Fill model the unmasked source pixels are pasted back as with any mask,
         and the log holds {"latent_size", "masked_fraction", "time"} of the conditioning under log["denoising"]["fill"]
-        instead of log["denoising"]["inpaint"]."""
+        instead of log["denoising"]["inpaint"].  `control_image` and `canny_thresholds` as in denoise_latents; on a
+        Canny or Depth model the log holds {"kind", "latent_size", "time"} of the conditioning under
+        log["denoising"]["control"]."""
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
                                     solver=solver, guidance=guidance, reference_image=reference_image,
                                     reference_latents=reference_latents, redux_image=redux_image, eta=eta,
-                                    mask_image=mask_image)
+                                    mask_image=mask_image, control_image=control_image,
+                                    canny_thresholds=canny_thresholds)
 
     def load_redux(self, siglip=None, redux=None, *, siglip_config=None):
         """Build FLUX.1 Redux's image encoder on the device: SigLIP (siglip_config, default

@@ -279,6 +279,14 @@ int dk_image_pre_masked(dk_ctx* ctx, int dtype, const uint8_t* img, const uint8_
  * H, W positive multiples of 16; lat and out 16-byte aligned and contiguous. */
 int dk_fill_cond_rows(dk_ctx* ctx, int dtype, const void* lat, const uint8_t* mask, void* out, int H, int W,
                       void* stream);
+/* FLUX.1 Canny's edge map (DESIGN.md §19): OpenCV's cv2.Canny(lut[img], low, high) (L1 gradient, 3 x 3 Sobel,
+ * replicated borders, the channel of largest |dx| + |dy|, exact 8-connected hysteresis) of channels 0-2 of a uint8
+ * (H, W, src_channels >= 3) image, each value first mapped through the 256-entry uint8 table lut -> out uint8 (H, W, 3),
+ * 255 on edges and 0 elsewhere in all three channels.  A candidate has magnitude > low, a strong pixel > high;
+ * 0 <= low <= high.  ws: DK_CANNY_WS_BYTES_PER_PIXEL * H * W bytes, 16-byte aligned.  H * W < 2^31.  Five launches. */
+#define DK_CANNY_WS_BYTES_PER_PIXEL 10
+int dk_canny(dk_ctx* ctx, const uint8_t* img, const uint8_t* lut, uint8_t* out, void* ws, int H, int W,
+             int src_channels, int low, int high, void* stream);
 /* FLUX.1 Redux's SigLIP patch embedding (DESIGN.md §15): uint8 NHWC [B, H, W, src_channels >= 3] -> 16-bit patch rows
  * [B * (H/p) * (W/p), kp] of the stride-p, p x p convolution without padding (the last H % p rows and W % p columns are
  * dropped).  Column k < 3p^2 holds channel k % 3 of pixel (k / 3p, (k / 3) % p) of the patch, normalised like
