@@ -8,9 +8,10 @@ DiffusionPipeline / FluxPipeline API (reference: argmaxinc/DiffusionKit, python/
                                      conditioning=cond, pooled_conditioning=pooled)
 """
 from ._lib import DkError  # noqa: F401
-from .config import (FLUX_CANNY_DEV, FLUX_DEPTH_DEV, FLUX_DEV, FLUX_FILL_DEV, FLUX_SCHNELL, SD3_2b,  # noqa: F401
+from .config import (DEPTH_ANYTHING_LARGE, FLUX_CANNY_DEV, FLUX_DEPTH_DEV, FLUX_DEV, FLUX_FILL_DEV, FLUX_SCHNELL, SD3_2b,  # noqa: F401
                      SD3_8b, SD35_MEDIUM, SIGLIP_SO400M_PATCH14_384, MMDiTConfig, SiglipVisionConfig,
-                     VAEDecoderConfig, VAEEncoderConfig)
+                     VAEDecoderConfig, VAEEncoderConfig, DepthAnythingConfig)
+from .depth import DepthAnythingModel  # noqa: F401
 from .image_encoders import ReduxImageEncoder, SiglipVisionModel  # noqa: F401
 from .lora import LoRA, load_lora  # noqa: F401
 from .mmdit import MMDiT  # noqa: F401

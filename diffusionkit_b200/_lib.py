@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdkb200.so")
 HEADER_PATH = os.path.join(_HERE, "..", "include", "dkb200.h")
 
-DK_BF16, DK_FP16 = 0, 1
+DK_BF16, DK_FP16, DK_F32 = 0, 1, 2
 ACT_NONE, ACT_GELU_ERF, ACT_SILU, ACT_QUICK_GELU, ACT_GELU_TANH = 0, 1, 2, 3, 4
 
 vp = C.c_void_p
@@ -87,6 +87,9 @@ SIGNATURES = {
     "dk_fill_cond_rows": (i32, [vp, i32, vp, vp, vp, i32, i32, vp]),
     "dk_canny": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "dk_image_patches": (i32, [vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+    "dk_resample": (i32, [vp, i32, i32, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, vp]),
+    "dk_depth_add_relu": (i32, [vp, i32, vp, vp, vp, vp, i64, vp]),
+    "dk_depth_head": (i32, [vp, i32, vp, vp, f32, vp, i64, i32, vp]),
     "dk_axpby_f32": (i32, [vp, vp, vp, vp, i64, f32, f32, vp]),
     "dk_vae_sample_latent": (i32, [vp, i32, vp, vp, vp, i64, i32, f32, f32, vp]),
     "dk_cast_f32_to_16": (i32, [vp, i32, vp, vp, i64, vp]),
@@ -98,6 +101,7 @@ SIGNATURES = {
     "dk_groupnorm_apply": (i32, [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "dk_conv3x3": (i32, [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "dk_conv3x3_s2": (i32, [vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+    "dk_conv3x3_s2_p1": (i32, [vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "dk_conv_fused_supported": (i32, [i32, i32, i32, i32]),
     "dk_conv3x3_fused": (i32, [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp, i32, vp]),
     "dk_conv_up_weights": (i32, [vp, i32, vp, vp, i32, i32, vp]),

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdkb200.so")
-SOURCES = ["api.cu", "gemm.cu", "conv_fused.cu", "attention.cu", "elementwise.cu", "text.cu", "canny.cu"]
+SOURCES = ["api.cu", "gemm.cu", "conv_fused.cu", "attention.cu", "elementwise.cu", "text.cu", "canny.cu", "depth.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -258,6 +258,48 @@ def tiny_siglip_config(image_size: int = 98, layers: int = 2) -> SiglipVisionCon
                               image_size=image_size)
 
 
+@dataclass
+class DepthAnythingConfig:
+    """The fields of transformers.DepthAnythingConfig (with its Dinov2Config backbone) that FLUX.1 Depth's depth
+    estimator reads (DESIGN.md §20)."""
+
+    hidden_size: int = 1024
+    num_attention_heads: int = 16
+    intermediate_size: int = 4096
+    num_hidden_layers: int = 24
+    patch_size: int = 14
+    image_size: int = 518                      # the position table covers (image_size / patch_size)^2 patches
+    layer_norm_eps: float = 1e-6
+    hidden_act: str = "gelu"
+    out_indices: Tuple[int, ...] = (21, 22, 23, 24)
+    neck_hidden_sizes: Tuple[int, ...] = (256, 512, 1024, 1024)
+    reassemble_factors: Tuple[float, ...] = (4, 2, 1, 0.5)
+    fusion_hidden_size: int = 256
+    head_hidden_size: int = 32
+    depth_estimation_type: str = "relative"
+
+    @property
+    def head_dim(self) -> int:
+        return self.hidden_size // self.num_attention_heads
+
+    @property
+    def pos_grid(self) -> int:
+        """side of the square position table without its CLS row: 518 / 14 = 37"""
+        return self.image_size // self.patch_size
+
+
+# LiheYoung/depth-anything-large-hf, the estimator of BFL's FLUX.1 Depth [dev] (DepthImageEncoder)
+DEPTH_ANYTHING_LARGE = DepthAnythingConfig()
+
+
+def tiny_depth_anything_config(layers: int = 4) -> DepthAnythingConfig:
+    """Small Depth Anything for tests: 2 heads of 64, the last four layers as the stages, the smallest widths the
+    kernels take (channel counts multiples of 64, fusion width 128 so the head's first convolution gives 64)."""
+    return DepthAnythingConfig(hidden_size=128, num_attention_heads=2, intermediate_size=512, num_hidden_layers=layers,
+                               out_indices=tuple(range(layers - 3, layers + 1)), neck_hidden_sizes=(64, 128, 128, 128),
+                               fusion_hidden_size=128)
+
+
 def tiny_clip_config(projection: bool = True, act: str = "quick_gelu") -> CLIPTextModelConfig:
     return CLIPTextModelConfig(num_layers=3, model_dims=128, num_heads=2, max_length=77, vocab_size=1000,
                                projection_dim=64 if projection else None, hidden_act=act)

@@ -77,10 +77,10 @@ def check_thresholds(thresholds) -> Optional[Tuple[int, int]]:
     return int(low), int(high)
 
 
-def load_control_image(image, size: Tuple[int, int]) -> np.ndarray:
+def load_control_image(image, size: Optional[Tuple[int, int]]) -> np.ndarray:
     """a path, a PIL image or a uint8 (H, W) / (H, W, 1|3|4) array -> uint8 (height, width, 3) RGB resized with PIL
-    LANCZOS to exactly size = (width, height), aspect ratio not kept (BFL's prepare_control); ValueError for an input
-    that is none of these"""
+    LANCZOS to exactly size = (width, height), aspect ratio not kept (BFL's prepare_control; None keeps the image's
+    size); ValueError for an input that is none of these"""
     from PIL import Image
 
     if isinstance(image, (str, bytes)) or hasattr(image, "__fspath__"):
@@ -97,14 +97,15 @@ def load_control_image(image, size: Tuple[int, int]) -> np.ndarray:
     if not isinstance(image, Image.Image):
         raise ValueError(f"control_image must be a path, a PIL image or a uint8 array, got {type(image).__name__}")
     image = image.convert("RGB")
-    if image.size != tuple(size):
+    if size is not None and image.size != tuple(size):
         image = image.resize(tuple(size), Image.LANCZOS)
     return np.array(image)
 
 
 def control_rows(encoder, image_u8: torch.Tensor, kind: str, shift: float, scale: float, dtype,
                  thresholds: Optional[Tuple[int, int]] = DEFAULT_THRESHOLDS) -> torch.Tensor:
-    """the (N, 64) control rows of one control image: image_u8 uint8 (H, W, 3) on the device, N = (H / 16)(W / 16).
+    """the (N, 64) control rows of one control image: image_u8 uint8 (H, W, 3) on the device, or the float (H, W, 3)
+    image in [-1, 1] the VAE encoder also takes (FLUX.1 Depth's estimated depth, DESIGN.md §20), N = (H / 16)(W / 16).
     kind "canny" with thresholds runs canny first (thresholds None: the image is already an edge map); the image is
     encoded once into its posterior mean (seed-independent; BFL samples the posterior), then (mean - shift) * scale,
     rounded to dtype and packed like the target latent."""

@@ -402,7 +402,7 @@ extern "C" int dk_gemm_fp8(dk_ctx* ctx, const dk_gemm_args* a, const float* a_sc
 
 // The entry point named fn has run DK_ENTRY and DK_DTYPE_OK.
 static int conv3x3_impl(const char* fn, dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias,
-                        const void* res, void* out, int B, int Hin, int Win, int Cin, int Cout, int stride,
+                        const void* res, void* out, int B, int Hin, int Win, int Cin, int Cout, int stride, int pad,
                         cudaStream_t stream) {
   DK_REQUIRE(B > 0 && Hin > 0 && Win > 0, "%s: empty input", fn);
   DK_REQUIRE(Cin % 64 == 0, "%s: Cin (%d) must be a multiple of 64 (pad the channels)", fn, Cin);
@@ -410,16 +410,18 @@ static int conv3x3_impl(const char* fn, dk_ctx* ctx, int dtype, const void* x, c
   DK_REQUIRE(dk_aligned16(x) && dk_aligned16(w) && dk_aligned16(out), "%s: x/w/out must be 16-byte aligned", fn);
   DK_REQUIRE(bias == nullptr || dk_aligned16(bias), "%s: bias alignment", fn);
   DK_REQUIRE(res == nullptr || dk_aligned16(res), "%s: residual alignment", fn);
-  DK_REQUIRE(stride == 1 || (Hin % 2 == 0 && Win % 2 == 0), "%s: input size must be even (got %dx%d)", fn, Hin, Win);
+  DK_REQUIRE(stride == 1 || pad == 1 || (Hin % 2 == 0 && Win % 2 == 0), "%s: input size must be even (got %dx%d)", fn,
+             Hin, Win);
 
-  const int H = Hin / stride, W = Win / stride;   // output size
+  // output size: stride 1 keeps it; stride 2 halves it (pad 0: even input), or rounds up with a pad of 1 on every side
+  const int H = (Hin + (stride - 1) * pad) / stride, W = (Win + (stride - 1) * pad) / stride;
   ConvGeom g;
   g.B = B;
   g.H = H;
   g.W = W;
   g.Cin = Cin;
   g.stride = stride;
-  g.pad = stride == 1 ? 1 : 0;
+  g.pad = pad;
   if (W < 128 && 128 % W == 0) {
     g.TW = W;
     g.TH = 128 / W;
@@ -474,7 +476,7 @@ extern "C" int dk_conv3x3(dk_ctx* ctx, int dtype, const void* x, const void* w, 
                           void* out, int B, int H, int W, int Cin, int Cout, void* stream_) {
   DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
-  return conv3x3_impl(__func__, ctx, dtype, x, w, bias, res, out, B, H, W, Cin, Cout, 1,
+  return conv3x3_impl(__func__, ctx, dtype, x, w, bias, res, out, B, H, W, Cin, Cout, 1, 1,
                       static_cast<cudaStream_t>(stream_));
 }
 
@@ -482,6 +484,16 @@ extern "C" int dk_conv3x3_s2(dk_ctx* ctx, int dtype, const void* x, const void* 
                              int H, int W, int Cin, int Cout, void* stream_) {
   DK_ENTRY(ctx);
   DK_DTYPE_OK(dtype);
-  return conv3x3_impl(__func__, ctx, dtype, x, w, bias, nullptr, out, B, H, W, Cin, Cout, 2,
+  return conv3x3_impl(__func__, ctx, dtype, x, w, bias, nullptr, out, B, H, W, Cin, Cout, 2, 0,
+                      static_cast<cudaStream_t>(stream_));
+}
+
+// The taps of output pixel (y, x) start at input (2y - 1, 2x - 1): the negative coordinate and the row / column past an
+// odd input's end are zero-filled by the TMA unit, so an odd size needs no special case.
+extern "C" int dk_conv3x3_s2_p1(dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias, void* out,
+                                int B, int H, int W, int Cin, int Cout, void* stream_) {
+  DK_ENTRY(ctx);
+  DK_DTYPE_OK(dtype);
+  return conv3x3_impl(__func__, ctx, dtype, x, w, bias, nullptr, out, B, H, W, Cin, Cout, 2, 1,
                       static_cast<cudaStream_t>(stream_));
 }

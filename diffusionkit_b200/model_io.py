@@ -410,3 +410,60 @@ def redux_checkpoint_to_params(sd: Dict[str, Tensor], token_level_text_embed_dim
     if extra:
         raise ValueError(f"Redux checkpoint: unexpected keys {extra}")
     return {n: sd[n] for n in want}
+
+
+# ------------------------------------------------------------------------------------------------ FLUX.1 Depth
+def depth_anything_config(config_json: dict):
+    """a transformers DepthAnything `config.json` (as a dict) -> DepthAnythingConfig.  The backbone's MLP width is
+    hidden_size * mlp_ratio (Dinov2Config); its stages come from out_indices, or from out_features ("stageN")."""
+    from .config import DepthAnythingConfig
+
+    bb = config_json.get("backbone_config") or {}
+    D = int(bb.get("hidden_size", 1024))
+    if "out_indices" in bb and bb["out_indices"] is not None:
+        out_indices = tuple(int(i) for i in bb["out_indices"])
+    elif bb.get("out_features"):
+        out_indices = tuple(int(str(f).replace("stage", "")) for f in bb["out_features"])
+    else:
+        out_indices = DepthAnythingConfig.out_indices
+    rh = config_json.get("reassemble_hidden_size", D)
+    if rh != D:
+        raise ValueError(f"Depth Anything config: reassemble_hidden_size {rh} differs from the backbone width {D}")
+    return DepthAnythingConfig(
+        hidden_size=D, num_attention_heads=int(bb.get("num_attention_heads", 16)),
+        intermediate_size=int(D * bb.get("mlp_ratio", 4)), num_hidden_layers=int(bb.get("num_hidden_layers", 24)),
+        patch_size=int(bb.get("patch_size", 14)), image_size=int(bb.get("image_size", 518)),
+        layer_norm_eps=float(bb.get("layer_norm_eps", 1e-6)), hidden_act=bb.get("hidden_act", "gelu"),
+        out_indices=out_indices,
+        neck_hidden_sizes=tuple(int(c) for c in config_json.get("neck_hidden_sizes", (256, 512, 1024, 1024))),
+        reassemble_factors=tuple(config_json.get("reassemble_factors", (4, 2, 1, 0.5))),
+        fusion_hidden_size=int(config_json.get("fusion_hidden_size", 256)),
+        head_hidden_size=int(config_json.get("head_hidden_size", 32)),
+        depth_estimation_type=config_json.get("depth_estimation_type", "relative"))
+
+
+_DEPTH_DROPPED = ("backbone.embeddings.mask_token", "neck.fusion_stage.layers.0.residual_layer1.")
+
+
+def depth_anything_checkpoint_to_params(sd: Dict[str, Tensor], config=None) -> Dict[str, Tensor]:
+    """transformers DepthAnythingForDepthEstimation safetensors (`backbone.*`, `neck.*`, `head.*`) -> the engine's
+    DepthAnythingModel tree (depth.pack_depth_params, fp32).  backbone.embeddings.mask_token and the unused
+    neck.fusion_stage.layers.0.residual_layer1.* are dropped.  A missing key, an unexpected one or a wrong shape raises
+    ValueError naming it, as does a configuration the kernels cannot run.  config: a DepthAnythingConfig (default
+    LiheYoung/depth-anything-large-hf)."""
+    from .config import DEPTH_ANYTHING_LARGE
+    from .depth import check_config, depth_param_specs, pack_depth_params
+
+    cfg = config if config is not None else DEPTH_ANYTHING_LARGE
+    check_config(cfg)
+    out = {k: v for k, v in sd.items() if not k.startswith(_DEPTH_DROPPED)}
+    want = {n: tuple(s) for n, s, _ in depth_param_specs(cfg)}
+    for n, s in want.items():
+        if n not in out:
+            raise ValueError(f"Depth Anything checkpoint: missing {n}")
+        if tuple(out[n].shape) != s:
+            raise ValueError(f"Depth Anything checkpoint: {n} has shape {tuple(out[n].shape)}, expected {s}")
+    extra = sorted(set(out) - set(want))
+    if extra:
+        raise ValueError(f"Depth Anything checkpoint: unexpected keys {extra[:5]} (+{max(0, len(extra) - 5)})")
+    return pack_depth_params(out, cfg)

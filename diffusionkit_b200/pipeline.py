@@ -30,8 +30,9 @@ Differences that are deliberate (documented in DESIGN.md):
     `image_path`), DESIGN.md §18: the masked source and the mask enter the x-embedder instead of the §17 blend; the
     unmasked source pixels are still pasted back.
   * FLUX.1 Canny / Depth [dev] (model_version "black-forest-labs/FLUX.1-Canny-dev" / "-Depth-dev", FluxPipeline with
-    `control_image=`), DESIGN.md §19: the control image's posterior-mean latent enters the x-embedder; no depth
-    estimator is included, a Depth model takes the depth map the caller gives.
+    `control_image=`), DESIGN.md §19: the control image's posterior-mean latent enters the x-embedder; a Depth model
+    takes the depth map the caller gives, or with `estimate_depth=True` (after FluxPipeline.load_depth_estimator) a
+    photo whose depth Depth Anything estimates on the engine's kernels, DESIGN.md §20.
 """
 from __future__ import annotations
 
@@ -42,7 +43,7 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 import torch
 
-from . import control, fill, inpaint, ops
+from . import control, depth, fill, inpaint, ops
 from ._lib import DkError, dtype_code, ptr
 from .config import CONTROL_MODEL_CONFIGS, MODEL_CONFIGS, T5_MAX_LENGTH, MMDiTConfig, VAEDecoderConfig, VAEEncoderConfig
 from .mmdit import MMDiT
@@ -729,10 +730,17 @@ class DiffusionPipeline:
         if reference_image is not None or reference_latents is not None:
             raise ValueError("FLUX.1 Fill takes no Kontext reference")
 
-    def _check_control(self, control_image, canny_thresholds, reference_image, reference_latents):
-        """FLUX.1 Canny / Depth's arguments, refused with ValueError before any GPU work -> canny_thresholds checked
-        ((low, high) or None) on a Canny model, None otherwise"""
+    def _check_control(self, control_image, canny_thresholds, reference_image, reference_latents,
+                       estimate_depth=False):
+        """FLUX.1 Canny / Depth's arguments, refused with ValueError (DkError for a missing depth estimator) before
+        any GPU work -> canny_thresholds checked ((low, high) or None) on a Canny model, None otherwise"""
         kind = self.config.control
+        if estimate_depth:
+            if kind != "depth" or not isinstance(self, FluxPipeline):
+                raise ValueError("estimate_depth runs on a FLUX.1 Depth model in FluxPipeline only")
+            if control_image is None:
+                raise ValueError("estimate_depth needs control_image: the photo the depth map is estimated from")
+            self._need_depth_estimator()
         if kind != "canny" and canny_thresholds != control.DEFAULT_THRESHOLDS:
             raise ValueError("canny_thresholds applies to a FLUX.1 Canny model only")
         if kind is None:
@@ -854,11 +862,13 @@ class DiffusionPipeline:
     def _denoise_latents(self, conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed, image_path,
                          denoise, *, noise, solver, guidance, slg=None, reference_image=None, reference_latents=None,
                          redux_image=None, redux_log=None, eta=None, sde_log=None, mask_image=None, fill_log=None,
-                         control_image=None, canny_thresholds=control.DEFAULT_THRESHOLDS, control_log=None):
+                         control_image=None, canny_thresholds=control.DEFAULT_THRESHOLDS, control_log=None,
+                         estimate_depth=False):
         _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
         self._check_fill(image_path, mask_image, reference_image, reference_latents)
-        thresholds = self._check_control(control_image, canny_thresholds, reference_image, reference_latents)
+        thresholds = self._check_control(control_image, canny_thresholds, reference_image, reference_latents,
+                                         estimate_depth)
         if image_path is None:
             denoise = 1.0                                                   # :270-271
         elif not (0.0 <= denoise <= 1.0):
@@ -952,13 +962,24 @@ class DiffusionPipeline:
             if not hasattr(self, "encoder"):
                 self.load_encoder()
             lf = self.latent_format
-            rows = control.control_rows(self.encoder, torch.from_numpy(control_image).to(self.device),
-                                        self.config.control, lf.shift_factor, lf.scale_factor, self.activation_dtype,
-                                        thresholds)
+            if estimate_depth:
+                # FLUX.1 Depth from a photo: BFL's DepthImageEncoder, then the estimated map is the control image
+                t1 = time.time()
+                image = self._depth_image(control_image, rgb=True)
+                if control_log is not None:
+                    torch.cuda.synchronize(self.device)
+                    depth_log = {"input_size": depth.network_size(*control_image.shape[:2]),
+                                 "time": round(time.time() - t1, 3)}
+            else:
+                image = torch.from_numpy(control_image).to(self.device)
+            rows = control.control_rows(self.encoder, image, self.config.control, lf.shift_factor, lf.scale_factor,
+                                        self.activation_dtype, thresholds)
             self.mmdit.cache_fill_conditioning(rows)
             if control_log is not None:
                 torch.cuda.synchronize(self.device)
                 control_log.update(kind=self.config.control, latent_size=(H, W), time=round(time.time() - t0, 3))
+                if estimate_depth:
+                    control_log["depth"] = depth_log
         if source is not None and self.config.x_embedder_cond_channels and not self.config.control:
             # FLUX.1 Fill: the masked source and the mask condition the x-embedder, once per call; no latent blend
             t0 = time.time()
@@ -1018,11 +1039,11 @@ class DiffusionPipeline:
     def _generate_image(self, text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                         denoise, *, conditioning, pooled_conditioning, solver, guidance, slg=None, reference_image=None,
                         reference_latents=None, redux_image=None, eta=None, mask_image=None, control_image=None,
-                        canny_thresholds=control.DEFAULT_THRESHOLDS):
+                        canny_thresholds=control.DEFAULT_THRESHOLDS, estimate_depth=False):
         _check_solver(solver, eta)
         _check_slg(slg, cfg_weight, self.config)
         self._check_fill(image_path, mask_image, reference_image, reference_latents)
-        self._check_control(control_image, canny_thresholds, reference_image, reference_latents)
+        self._check_control(control_image, canny_thresholds, reference_image, reference_latents, estimate_depth)
         n_images = len(seed) if isinstance(seed, (list, tuple)) else 1
         guidance = self._guidance_values(guidance, n_images)
         reference = self._reference_input(reference_image, reference_latents, n_images)
@@ -1068,7 +1089,7 @@ class DiffusionPipeline:
                                                    guidance=guidance, slg=slg, redux_log=redux_log, eta=eta,
                                                    sde_log=sde_log, mask_image=mask_image, fill_log=fill_log,
                                                    control_image=control_image, canny_thresholds=canny_thresholds,
-                                                   control_log=control_log,
+                                                   control_log=control_log, estimate_depth=estimate_depth,
                                                    redux_image=redux if redux is None or len(redux) == n_images
                                                    else redux[0], **ref_kw)
         torch.cuda.synchronize(self.device)
@@ -1258,7 +1279,7 @@ class FluxPipeline(DiffusionPipeline):
                         denoise: float = 1.0, *, noise: Optional[torch.Tensor] = None, solver: str = "euler",
                         guidance=None, reference_image=None, reference_latents: Optional[torch.Tensor] = None,
                         redux_image=None, eta: Optional[float] = None, mask_image=None, control_image=None,
-                        canny_thresholds=control.DEFAULT_THRESHOLDS):
+                        canny_thresholds=control.DEFAULT_THRESHOLDS, estimate_depth: bool = False):
         """DiffusionPipeline.denoise_latents (`solver`, `eta` and `mask_image` included), plus FLUX.1-dev's distilled guidance (DESIGN.md §12): `guidance` is one
         float for every image or one per seed, and None means DEFAULT_GUIDANCE (3.5) when the model has a guidance
         embedder (mmdit_config=FLUX_DEV).  A model without one refuses any value but None.
@@ -1286,19 +1307,25 @@ class FluxPipeline(DiffusionPipeline):
         cv2.Canny(img, *canny_thresholds) on the GPU first (canny_thresholds None: it is already an edge map); on
         Depth it is the depth map.  It is encoded once into its posterior mean and conditions every forward through
         the x-embedder.  `guidance` None means 30.0 on Canny and 10.0 on Depth.  img2img, mask_image (§17's blend),
-        Redux and every solver combine with it; a Kontext reference does not.  Other models refuse control_image."""
+        Redux and every solver combine with it; a Kontext reference does not.  Other models refuse control_image.
+
+        `estimate_depth=True` (FLUX.1 Depth only, after load_depth_estimator; DESIGN.md §20): `control_image` is a photo,
+        and the depth map is estimated from it once per call as BFL's DepthImageEncoder does (estimate_depth)
+        before it is encoded."""
         return self._denoise_latents(conditioning, pooled_conditioning, num_steps, cfg_weight, latent_size, seed,
                                      image_path, denoise, noise=noise, solver=solver, guidance=guidance,
                                      reference_image=reference_image, reference_latents=reference_latents,
                                      redux_image=redux_image, eta=eta, mask_image=mask_image,
-                                     control_image=control_image, canny_thresholds=canny_thresholds)
+                                     control_image=control_image, canny_thresholds=canny_thresholds,
+                                     estimate_depth=estimate_depth)
 
     def generate_image(self, text: str, num_steps: int = 2, cfg_weight: float = 0.0, negative_text: str = "",
                        latent_size: Tuple[int, int] = (64, 64), seed=None, verbose: bool = True,
                        image_path: Optional[str] = None, denoise: float = 1.0, *, conditioning=None,
                        pooled_conditioning=None, solver: str = "euler", guidance=None, reference_image=None,
                        reference_latents: Optional[torch.Tensor] = None, redux_image=None, eta: Optional[float] = None,
-                       mask_image=None, control_image=None, canny_thresholds=control.DEFAULT_THRESHOLDS):
+                       mask_image=None, control_image=None, canny_thresholds=control.DEFAULT_THRESHOLDS,
+                       estimate_depth: bool = False):
         """DiffusionPipeline.generate_image (`solver`, `eta`, `mask_image` and their logs included) with `guidance`, `reference_image`, `reference_latents` and `redux_image`
         as in denoise_latents; with a guidance embedder the log holds the value of each image under
         log["denoising"]["guidance"], with a reference its latent size and token count under
@@ -1307,13 +1334,45 @@ class FluxPipeline(DiffusionPipeline):
         and the log holds {"latent_size", "masked_fraction", "time"} of the conditioning under log["denoising"]["fill"]
         instead of log["denoising"]["inpaint"].  `control_image` and `canny_thresholds` as in denoise_latents; on a
         Canny or Depth model the log holds {"kind", "latent_size", "time"} of the conditioning under
-        log["denoising"]["control"]."""
+        log["denoising"]["control"], and with `estimate_depth` also "depth": {"input_size", "time"} of the estimator."""
         return self._generate_image(text, num_steps, cfg_weight, negative_text, latent_size, seed, verbose, image_path,
                                     denoise, conditioning=conditioning, pooled_conditioning=pooled_conditioning,
                                     solver=solver, guidance=guidance, reference_image=reference_image,
                                     reference_latents=reference_latents, redux_image=redux_image, eta=eta,
                                     mask_image=mask_image, control_image=control_image,
-                                    canny_thresholds=canny_thresholds)
+                                    canny_thresholds=canny_thresholds, estimate_depth=estimate_depth)
+
+    def load_depth_estimator(self, params=None, *, config=None):
+        """Build FLUX.1 Depth's depth estimator on the device: Depth Anything (config, default
+        LiheYoung/depth-anything-large-hf).  params: the engine's tree (model_io.depth_anything_checkpoint_to_params
+        converts the upstream safetensors), or None for the deterministic synthetic initialiser.  It runs in the
+        pipeline's 16-bit dtype; BFL runs it in fp32 (DESIGN.md §20)."""
+        from .config import DEPTH_ANYTHING_LARGE
+
+        cfg = config or DEPTH_ANYTHING_LARGE
+        if params is None:
+            params = depth.init_depth_params(cfg, seed=self._weight_seed + 8)
+        self.depth_estimator = depth.DepthAnythingModel(params, cfg, dtype=self.dtype, device=self.device)
+
+    def _need_depth_estimator(self):
+        if getattr(self, "depth_estimator", None) is None:
+            raise DkError("estimate_depth needs the depth estimator: call load_depth_estimator(...) with local weights "
+                          "first (nothing can be downloaded here), or pass the depth map itself as control_image")
+
+    def _depth_image(self, image_u8: np.ndarray, rgb: bool) -> torch.Tensor:
+        """BFL's DepthImageEncoder of a uint8 (H, W, 3) host image at the target size: the round trip and the
+        processor's resize on the host, the estimator, the antialiased bicubic back to (H, W) -> fp32 depth (H, W), or
+        with rgb the VAE's (H, W, 3) input depth / 127.5 - 1 in the pipeline dtype"""
+        net = torch.from_numpy(depth.network_input(image_u8)).to(self.device)
+        est = self.depth_estimator
+        return est.depth(est(net), image_u8.shape[:2], rgb=rgb)
+
+    def estimate_depth(self, image) -> torch.Tensor:
+        """BFL's `depth` of one image (a path, a PIL image or a uint8 (H, W) / (H, W, 1|3|4) array, converted to RGB):
+        fp32 (H, W) on the device, before depth / 127.5 - 1, at the image's own size (after load_depth_estimator)"""
+        self._need_depth_estimator()
+        arr = control.load_control_image(image, None)
+        return self._depth_image(arr, rgb=False)
 
     def load_redux(self, siglip=None, redux=None, *, siglip_config=None):
         """Build FLUX.1 Redux's image encoder on the device: SigLIP (siglip_config, default

@@ -45,6 +45,7 @@ extern "C" {
 
 #define DK_BF16 0
 #define DK_FP16 1
+#define DK_F32 2 /* dk_resample's fp32 input / output only */
 
 #define DK_ACT_NONE 0
 #define DK_ACT_GELU_ERF 1 /* mlx nn.GELU() exact erf — mmdit.py:421,835 */
@@ -294,6 +295,23 @@ int dk_canny(dk_ctx* ctx, const uint8_t* img, const uint8_t* lut, uint8_t* out, 
  * rows feed dk_gemm with the conv weight permuted to (O, kh, kw, c) and zero-padded to kp. */
 int dk_image_patches(dk_ctx* ctx, int dtype, const uint8_t* img, void* out, int B, int H, int W, int src_channels,
                      int p, int kp, void* stream);
+/* FLUX.1 Depth's depth estimator (DESIGN.md §20, csrc/depth.cu).
+ * dk_resample: separable linear resampling of an NHWC map in [Hi, Wi, C] -> out [Ho, Wo, C] through per-axis tap tables:
+ *   out(y, x, c) = sum_t wy[y * ty + t] * sum_u wx[x * tx + u] * in(y0[y] + t, x0[x] + u, c), in fp32.  y0 int32 [Ho],
+ *   wy fp32 [Ho * ty], x0 int32 [Wo], wx fp32 [Wo * tx] (device), every index y0[y] + t in [0, Hi) (x likewise).
+ *   in_dtype / out_dtype: DK_BF16, DK_FP16 or DK_F32.  mode 0 writes the map; mode 1 (C == 1) writes BFL's
+ *   v / 127.5 - 1 to all three channels of out [Ho, Wo, 3].  1 <= ty, tx <= 64.  One launch. */
+int dk_resample(dk_ctx* ctx, int in_dtype, int out_dtype, const void* in, void* out, int Hi, int Wi, int C, int Ho,
+                int Wo, const int* y0, const float* wy, int ty, const int* x0, const float* wx, int tx, int mode,
+                void* stream);
+/* sum = a + b (b null: a) rounded to 16 bits, relu = max(sum, 0); sum or relu may be null, either may alias a.  n
+ * elements.  The DPT residual units' pre-activations and fusion sums.  One launch. */
+int dk_depth_add_relu(dk_ctx* ctx, int dtype, const void* a, const void* b, void* sum, void* relu, long long n,
+                      void* stream);
+/* Depth Anything's head tail: out[p] = max(sum_k w[k] * max(x[p, k], 0) + b, 0) in fp32, summed in channel order with
+ * every product and sum rounded; x 16-bit [pixels, C], w fp32 [C] (device), out fp32 [pixels].  One launch. */
+int dk_depth_head(dk_ctx* ctx, int dtype, const void* x, const float* w, float b, float* out, long long pixels, int C,
+                  void* stream);
 /* out = a * x + b * y (fp32): img2img noise scaling sigma * noise + (1 - sigma) * latent (sampler.py:41-42) */
 int dk_axpby_f32(dk_ctx* ctx, const float* x, const float* y, float* out, long long n, float a, float b, void* stream);
 /* VAE-encoder posterior sample + process_in: hidden [pixels, 2C] 16-bit = (mean | logvar);
@@ -337,6 +355,11 @@ int dk_conv3x3(dk_ctx* ctx, int dtype, const void* x, const void* w, const void*
  * a 4-D box traversed with element stride 2. */
 int dk_conv3x3_s2(dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias, void* out, int B, int H, int W,
                   int Cin, int Cout, void* stream);
+/* 3x3 convolution with stride 2 and one pixel of zero padding on every side (PyTorch's Conv2d(3, stride=2, padding=1),
+ * Depth Anything's DPT downsample, DESIGN.md §20).  x [B,H,W,Cin] (any H, W) -> out [B,ceil(H/2),ceil(W/2),Cout]: output
+ * pixel (y, x) reads input rows 2y - 1 .. 2y + 1; the TMA unit zero-fills the taps outside the image. */
+int dk_conv3x3_s2_p1(dk_ctx* ctx, int dtype, const void* x, const void* w, const void* bias, void* out, int B, int H,
+                     int W, int Cin, int Cout, void* stream);
 /* K7f fused ResNet-path convolution (csrc/conv_fused.cu): [GroupNorm-apply + SiLU on the input] -> [nearest 2x] ->
  *     conv 3x3 (+ bias, + skip) -> output AND the GroupNorm partial statistics of the output, in ONE kernel.
  *     replaces nn.GroupNorm + nn.SiLU + nn.Conv2d (+ skip) of ResnetBlock2D (vae.py:60-101) and
